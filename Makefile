@@ -3,7 +3,7 @@ PY ?= python
 
 .PHONY: build helpers test test-gpu smoke bench bench-ref clean
 
-build:            ## nvcc -gencode arch=compute_100a,code=sm_100a -> relora_b200/_C.so ; g++ -> relora_b200/_data_helpers.so
+build:            ## nvcc -gencode arch=compute_90a,code=sm_90a -> relora_b200/_C.so ; g++ -> relora_b200/_data_helpers.so
 	$(PY) -c "import __graft_entry__ as g; g.build()"
 
 helpers:          ## only the C++17 / pybind11 dataset index builders
@@ -12,7 +12,7 @@ helpers:          ## only the C++17 / pybind11 dataset index builders
 test:             ## CPU / gloo suite
 	$(PY) -m pytest tests -x -q -m "not gpu"
 
-test-gpu:         ## kernel numerics + fused executor (needs a B200)
+test-gpu:         ## kernel numerics + fused executor (needs an H100)
 	$(PY) -m pytest tests -x -q -m gpu
 
 smoke:

@@ -1,7 +1,7 @@
 """Headline benchmark: ReLoRA training throughput (tokens/s, whole job) on synthetic tokens.
 
     python bench.py --gpus 1 --steps 8 --warmup 3                    # this engine
-    python bench.py --impl reference --gpus 1 --steps 8 --warmup 3   # unmodified reference (baseline/_ref)
+    python bench.py --impl reference --gpus 1 --steps 8 --warmup 3   # unmodified reference (oracle/_ref)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus 8 --steps 8 --warmup 3
 
@@ -11,12 +11,11 @@ global batch 144·N sequences).  One *step* = one optimizer update = 6 micro-bat
 gradient reduction, clipping, AdamW and the LR schedule.  Random-init weights, synthetic token ids.
 
 The same line carries a ``"llama_1b"`` block (BASELINE.json config 4: llama_1b ReLoRA r=128, seq 512, micro-batch 16 x
-accumulation 4, ``optimizer_magnitude_pruning 0.9``), measured the same way with fewer steps so that both models fit
-in one driver invocation; ``--no-1b`` drops it, ``--model X`` benchmarks X alone.
+accumulation 4, ``optimizer_magnitude_pruning 0.9``), measured the same way with the same ``--steps`` / ``--warmup``; ``--no-1b`` drops it, ``--model X`` benchmarks X alone.
 
-Timing: W >= 3 untimed steps, then exactly K steps bracketed by barrier + cuda synchronize, CUDA events on
+Timing: W untimed steps, then exactly K steps bracketed by barrier + cuda synchronize, CUDA events on
 the launching stream, max over ranks.  The working set of a step (0.5 GB of weights + >1 GB of activations)
-exceeds the 126 MB L2, so no explicit flush is needed.  `value` is measured with device-resident inputs;
+exceeds the 50 MB L2 of an H100, so no explicit flush is needed.  `value` is measured with device-resident inputs;
 `e2e.value` goes through the public API (`TrainingEngine.train_step`): pinned-host token ids are copied to
 the device every step and the loss is read back to the host every step.
 
@@ -71,10 +70,11 @@ def parse():
     ap.add_argument("--optimizer", type=str, default="adam")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-1b", action="store_true", help="skip the llama_1b block")
-    ap.add_argument("--steps-1b", type=int, default=6, help="timed steps of the llama_1b block (capped by --steps)")
     ap.add_argument("--frozen_dtype", type=str, default=None, help="fp8: E4M3 tensor-core path for the frozen weights (opt-in)")
     ap.add_argument("--attention", type=str, default="auto", choices=["auto", "native", "sdpa"])
     ap.add_argument("--cuda_graphs", type=str, default="true")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<model>_<name>.npy")
     return ap.parse_args()
 
 
@@ -171,7 +171,8 @@ def make_tokens(steps, ga, batch, seq, vocab, rank, pinned):
     embedding's padding row (all zeros, never trained; ``modeling_llama.py:433-436``) and real text never contains that id.
     A sequence that *starts* with it keeps an exactly-zero residual row through every layer (v = 0, no biases, LoRA B = 0), where
     RMSNorm's backward has gain 1/sqrt(eps) = 1000 per norm; the gradient overflows after ~17 layers.  That is what turned both arms
-    non-finite at 4 and 8 GPUs in round 1 (P = 1/32100 per sequence: ~55 % of 45-step runs at N = 4); see DESIGN.md "root cause"."""
+    non-finite at 4 and 8 GPUs in round 1 (P = 1/32100 per sequence: ~55 % of 45-step runs at N = 4); see
+    tests/test_models.py::test_sequence_starting_with_the_padding_row_overflows_the_reference_gradient."""
     import torch
 
     g = torch.Generator().manual_seed(1234 + rank)
@@ -212,6 +213,24 @@ def gather_rows(t):
 
 
 # --------------------------------------------------------------------------------------------- our arm
+DUMP_PARAM_SAMPLE = 4 << 20  # parameters sampled into <model>_params.npy (16 MB of float32 per model)
+
+
+def dump_outputs(eng, model, out_dir):
+    """What a caller of the timed step receives from its last call: the loss and gradient norm of that update (float64) and
+    the parameters it produced, as a fixed seeded sample (float32; same indices for the same model on every build)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"{model}_loss.npy"), np.array([float(eng.last_local_loss)], dtype=np.float64))
+    np.save(os.path.join(out_dir, f"{model}_grad_norm.npy"), np.array([float(eng.last_grad_norm.reshape(()))], dtype=np.float64))
+    params = eng.stepper.store.params.reshape(-1)
+    n = params.numel()
+    idx = torch.randint(0, n, (min(n, DUMP_PARAM_SAMPLE),), generator=torch.Generator().manual_seed(0)).sort().values
+    np.save(os.path.join(out_dir, f"{model}_params.npy"), params[idx.to(params.device)].float().cpu().numpy())
+
+
 def run_ours_case(args, info, model, steps, warmup, rank, local, world):
     import torch
 
@@ -262,6 +281,8 @@ def run_ours_case(args, info, model, steps, warmup, rank, local, world):
         sampler.start()
     secs = timed(lambda i: dev_step(warmup + i), steps, world, dev)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, model, args.dump_outputs)
     launches = int(getattr(eng.stepper, "launches_in_window", lambda n: C.launch_count())(steps))
     tokens = eng.tokens_per_step * steps
     value = tokens / secs
@@ -292,7 +313,7 @@ def run_ours_case(args, info, model, steps, warmup, rank, local, world):
         "value": value, "unit": "tokens/s", "ms_per_step": secs / steps * 1e3, "steps": steps, "warmup": warmup,
         "config": case_config(model, batch, ga, args.seq, args.lora_r, world, args.optimizer, rec["reset"]),
         "impl_details": {"executor": type(eng.stepper).__name__, "comm": getattr(eng.stepper.sync, "transport", "none"),
-                         "attention": "tcgen05 (this repo)" if getattr(eng.stepper, "native_attn", False) else "torch SDPA (cuDNN)",
+                         "attention": "wgmma (this repo)" if getattr(eng.stepper, "native_attn", False) else "torch SDPA (cuDNN)",
                          "cuda_graphs": bool(getattr(eng.stepper, "use_graphs", False))},
         "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "valid": valid,
         "final_loss": float(losses_all[:, n_done - 1].mean()), "final_grad_norm": float(norms_all[0, n_done - 1]),
@@ -325,7 +346,7 @@ def run_ours(args):
     head = run_ours_case(args, info, head_model, args.steps, args.warmup, rank, local, world)
     extra = None
     if args.model is None and not args.no_1b:
-        extra = run_ours_case(args, info, "llama_1b", max(1, min(args.steps, args.steps_1b)), max(3, min(args.warmup, 3)), rank, local, world)
+        extra = run_ours_case(args, info, "llama_1b", args.steps, args.warmup, rank, local, world)
     valid = head["valid"] and (extra is None or extra["valid"])
     if rank == 0:
         out = {
@@ -351,7 +372,7 @@ def run_ours(args):
 # --------------------------------------------------------------------------------------------- reference arm
 def _stub_missing_modules():
     """The reference imports bitsandbytes at module level (relora.py:10-11); the package is not in this image.
-    A stub satisfies the import — the non-quantised code path never touches it.  Nothing in baseline/_ref is edited."""
+    A stub satisfies the import — the non-quantised code path never touches it.  Nothing in oracle/_ref is edited."""
     for name in ("bitsandbytes", "bitsandbytes.nn", "bitsandbytes.functional"):
         if name not in sys.modules:
             sys.modules[name] = types.ModuleType(name)
@@ -445,9 +466,9 @@ def run_reference_case(args, mods, model_name, steps, warmup, rank, local, world
 
 
 def run_reference(args):
-    ref_dir = os.path.join(ROOT, "baseline", "_ref")
+    ref_dir = os.path.join(ROOT, "oracle", "_ref")
     if not os.path.isdir(os.path.join(ref_dir, "peft_pretraining")):
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref is not installed (pip --target baseline/_ref /root/reference)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref is not installed (python oracle/install_reference.py <upstream checkout>)"}))
         return 0
     import torch  # noqa: F401
 
@@ -470,7 +491,7 @@ def run_reference(args):
     head = run_reference_case(args, mods, args.model or "llama_250m", args.steps, args.warmup, rank, local, world)
     extra = None
     if args.model is None and not args.no_1b and head["valid"]:
-        extra = run_reference_case(args, mods, "llama_1b", max(1, min(args.steps, args.steps_1b)), max(3, min(args.warmup, 3)), rank, local, world)
+        extra = run_reference_case(args, mods, "llama_1b", args.steps, args.warmup, rank, local, world)
     valid = head["valid"] and (extra is None or extra["valid"])
     if rank == 0:
         out = {

@@ -1,4 +1,4 @@
-"""tcgen05 attention kernels vs torch SDPA (cuDNN flash) on the training shapes. CUDA events, L2 flushed between launches."""
+"""wgmma attention kernels vs torch SDPA (cuDNN flash) on the training shapes. CUDA events, L2 flushed between launches."""
 import math, os, sys, json, torch
 import torch.nn.functional as Fn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -40,6 +40,5 @@ for name, B, T, nh, hd in (("250m", 24, 512, 16, 48), ("1b", 16, 512, 32, 64), (
     rec = {"shape": name, "B": B, "T": T, "nh": nh, "hd": hd, "ours_fwd_us": t_f, "sdpa_fwd_us": t_sf, "ours_bwd_us": t_b, "ours_bwd_recompute_us": t_b_recompute, "sdpa_bwd_us": t_sb,
            "ours_fwd_tflops": fl / t_f / 1e6, "ours_bwd_tflops": 2.5 * fl / t_b / 1e6}
     rows.append(rec); print(json.dumps({k: (round(x, 1) if isinstance(x, float) else x) for k, x in rec.items()}), flush=True)
-print("resident CTAs per SM (fwd, dq, dkv):", [C.attention_occupancy(i) for i in range(3)])
 if len(sys.argv) > 1:
     json.dump(rows, open(sys.argv[1], "w"), indent=1)

@@ -1,4 +1,4 @@
-"""Run the tcgen05 attention kernels a few times (target for `ncu -k regex:attn_`)."""
+"""Run the wgmma attention kernels a few times (a short, profiler-friendly workload)."""
 import math, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from relora_b200.ops import fused as F

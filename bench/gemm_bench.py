@@ -1,6 +1,6 @@
-"""Per-kernel roofline bench: tcgen05 GEMM (plain / fused-LoRA / MN-major / split-K) vs cuBLAS via torch.matmul.
+"""Per-kernel roofline bench: wgmma GEMM (plain / fused-LoRA / MN-major / split-K) vs cuBLAS via torch.matmul.
 
-    python bench/gemm_bench.py [--out gpurun_out/gemm_bench.json]
+    python bench/gemm_bench.py [--out gemm_bench.json]
 
 CUDA-event timing, 3 warm-up + 10 timed launches, a 256 MB write between launches flushes the 126 MB L2.
 Fractions are reported against MEASURED_PEAKS.json (bf16_tflops burst) when present.

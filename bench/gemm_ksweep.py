@@ -1,7 +1,7 @@
 """T(K) sweep at fixed M, N: separates the per-tile fixed cost (epilogue, tile hand-off) from the per-k-block cost
-(tensor pipe / L2 feed) for the single-CTA and CTA-pair variants of the tcgen05 GEMM.
+(tensor pipe / L2 feed) for the 128- and 256-wide tiles of the wgmma GEMM.
 
-    python bench/gemm_ksweep.py [--M 12288] [--N 2304] [--out gpurun_out/gemm_ksweep.json]
+    python bench/gemm_ksweep.py [--M 12288] [--N 2304] [--out gemm_ksweep.json]
 """
 import argparse, json, os, sys
 import torch

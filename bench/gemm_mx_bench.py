@@ -1,6 +1,6 @@
-"""Block-scaled MXFP8 GEMM (csrc/gemm_mx.cu) vs the bf16 tcgen05 GEMM on the model's projection shapes; operands pre-quantised.
+"""Block-scaled MXFP8 GEMM (csrc/gemm_mx.cu) vs the bf16 wgmma GEMM on the model's projection shapes; operands pre-quantised.
 
-    python bench/gemm_mx_bench.py [--out gpurun_out/gemm_mx_bench.json]        (target for `ncu -k regex:gemm_mx_kernel`)
+    python bench/gemm_mx_bench.py [--out gemm_mx_bench.json]
 """
 import argparse, json, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

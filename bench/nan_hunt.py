@@ -61,7 +61,7 @@ def run_ours(a):
     rank, world, local = _setup()
     info = init_distributed("cuda", "nccl")
     w = _writer(a.tag, rank)
-    if a.sdpa_backend != "default":  # which library kernel torch SDPA may pick (the default on sm_100 is cuDNN's)
+    if a.sdpa_backend != "default":  # which library kernel torch SDPA may pick (by default cuDNN's)
         torch.backends.cuda.enable_cudnn_sdp(a.sdpa_backend == "cudnn")
         torch.backends.cuda.enable_flash_sdp(a.sdpa_backend == "flash")
         torch.backends.cuda.enable_mem_efficient_sdp(a.sdpa_backend == "efficient")

@@ -67,7 +67,7 @@ ENGINE_FLAGS = (
 
 
 def build_parser() -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description="ReLoRA pre-training (B200-native engine)")
+    p = argparse.ArgumentParser(description="ReLoRA pre-training (H100-native engine)")
     p.add_argument("--training_config", type=str, default=None,
                    help="Path to a yaml file with the training run config; overrides all parameters.")
 
@@ -136,13 +136,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--comm", type=str, default="auto", choices=["auto", "nccl", "p2p"],
                    help="gradient all-reduce: NCCL baseline or the NVLink peer-memory kernels")
     p.add_argument("--engine", type=str, default="auto", choices=["auto", "fused", "module"],
-                   help="fused: whole-layer sm_100a executor (+CUDA graphs); module: nn.Module path")
+                   help="fused: whole-layer sm_90a executor (+CUDA graphs); module: nn.Module path")
     p.add_argument("--lora_dropout", type=float, default=0.1, help="hard-coded to 0.1 upstream (torchrun_main.py:546)")
     _add_bool(p, "--cuda_graphs", True)
     _add_bool(p, "--deterministic", False,
               help="fixed summation order for the weight-gradient GEMMs (no split-K atomics; slower) on top of the always-deterministic embedding backward")
     p.add_argument("--attention", type=str, default="auto", choices=["auto", "native", "sdpa"],
-                   help="native: tcgen05 flash-attention kernels of this repo (head_dim <= 64); sdpa: torch SDPA (cuDNN)")
+                   help="native: wgmma flash-attention kernels of this repo (head_dim <= 64); sdpa: torch SDPA (cuDNN)")
     p.add_argument("--frozen_dtype", type=str, default=None, choices=[None, "bf16", "fp8", "fp8_full", "mxfp8", "nvfp4"],
                    help="fp8: E4M3 tensor-core path for the frozen weights on the fused executor (per-tensor scales, delayed "
                         "activation scaling), forward GEMMs only; fp8_full: also the input-gradient GEMMs (E5M2 gradients); mxfp8 / nvfp4: block-scaled storage on the module path (alias of --quantize)")

@@ -1,7 +1,7 @@
-"""sm_100a sources of the in-tree extension ``relora_b200/_C.so`` (+ the host C++ data helpers).
+"""sm_90a sources of the in-tree extension ``relora_b200/_C.so`` (+ the host C++ data helpers).
 
-    gemm_tcgen05.cu   persistent tcgen05 / TMEM / TMA GEMM (LoRA K-extension, CTA pairs, split-K, fp8), LoRA input-gradient kernels
-    attention.cu      causal flash attention forward / dQ / dK,dV on tcgen05
+    gemm_wgmma.cu     persistent TMA + wgmma GEMM (LoRA K-extension, split-K, fp8), LoRA input-gradient kernel
+    attention.cu      causal flash attention forward / dQ / dK,dV on wgmma
     norm_warp.cu      RMSNorm forward (+ dropout-expanded copies) / backward
     elementwise.cu    dropout expand / combine, SwiGLU, embedding, transpose, hash re-init
     rope.cu           rotary embedding (Llama layout), fused dq/dk/dv pack + inverse rotation
@@ -12,6 +12,6 @@
     comm.cu           NVLink peer-memory collectives (P2P + multimem): all-reduce, fused reduce-scatter / clip / AdamW / all-gather
     bindings.cpp      pybind11 / torch::Tensor glue;  data_helpers.cpp  index-map builders of the NeoX data pipeline
 
-Build: ``python -m relora_b200.csrc.build`` (nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo; cross-compiles without a GPU).
+Build: ``python -m relora_b200.csrc.build`` (nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo; cross-compiles without a GPU).
 """
 from .build import CPP_SOURCES, CUDA_SOURCES, HEADERS, build  # noqa: F401

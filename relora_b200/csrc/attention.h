@@ -1,4 +1,4 @@
-// Causal self-attention on tcgen05 (forward + backward), reading q/k/v in place from the packed projection output.
+// Causal self-attention on wgmma (forward + backward), reading q/k/v in place from the packed projection output.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,17 +35,12 @@ struct AttnBwdDesc {
   long long ld_dqkv = 0;
   int B = 0, T = 0, nh = 0, hd = 0;
   float scale = 1.0f;
-  // optional bf16 workspace of attention_ds_workspace_elems(B, T, nh) elements: the dK/dV kernel stores its dSᵀ tiles there and dQ
-  // becomes a plain TMA -> MMA kernel (dQ = dS·K) instead of recomputing S and dP; nullptr = the recomputing dQ kernel
+  // optional bf16 workspace of attention_ds_workspace_elems(B, T, nh) elements; not read by the sm_90 kernels (the dQ kernel
+  // recomputes S and dP), kept so callers that size it need no change
   void* ds_workspace = nullptr;
 };
 void attention_bwd(const AttnBwdDesc& d, cudaStream_t stream);
 long long attention_ds_pitch(int T);
 long long attention_ds_workspace_elems(int B, int T, int nh);
-
-// Diagnostics: the heaviest forward CTA writes clock64 stamps (8 x 64 int64) into `buf`; nullptr = off.
-void attention_set_trace(void* buf);
-// resident CTAs per SM of the forward (0), dQ (1) and dK/dV (2) kernels, as reported by the occupancy calculator after first use
-int attention_occupancy(int which);
 
 }  // namespace rb

@@ -1,4 +1,4 @@
-// Python bindings (pybind11 over torch::Tensor) for the sm_100a kernels.  Every function launches on the
+// Python bindings (pybind11 over torch::Tensor) for the sm_90a kernels.  Every function launches on the
 // current PyTorch CUDA stream, so the ops compose with torch streams and CUDA-graph capture.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -63,11 +63,10 @@ rb::Fp8Out fp8_out(const OptTensor& q8, const OptTensor& inv_scale, const OptTen
 void gemm(const Tensor& a1, const Tensor& b1, Tensor& out, int64_t M, int64_t N, int64_t K1, const OptTensor& a2, const OptTensor& b2,
           int64_t K2, bool a1_mn, bool b1_mn, int64_t n_per_group, int64_t a1_group_kofs, int64_t a2_group_kofs,
           const OptTensor& residual, double alpha, bool accumulate, int64_t block_n, int64_t split_k, int64_t b1_group_kofs,
-          bool b1_local_n, int64_t m_per_group, int64_t b1_mn_ofs_per_mgroup, const OptTensor& bias, int64_t cta_pair, int64_t fp8,
+          bool b1_local_n, int64_t m_per_group, int64_t b1_mn_ofs_per_mgroup, const OptTensor& bias, int64_t /*cta_pair: no CTA-pair MMA on sm_90*/, int64_t fp8,
           const OptTensor& alpha_dev) {
   c10::cuda::CUDAGuard guard(out.device());
   rb::GemmDesc d;
-  d.cta_pair = (int)cta_pair;
   if (fp8) {
     // E4M3 bytes (torch.uint8 / float8_e4m3fn storage), K-major; leading dimensions in bytes
     TORCH_CHECK(!a1_mn && !b1_mn, "fp8 operands must be K-major");
@@ -606,15 +605,9 @@ void reset_launch_count() { rb::g_launch_count = 0; }
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "relora_b200 sm_100a kernels";
-  m.def("gemm", &gemm, "tcgen05 GEMM with fused LoRA K-extension");
+  m.doc() = "relora_b200 sm_90a kernels";
+  m.def("gemm", &gemm, "wgmma GEMM with fused LoRA K-extension");
   m.def("gemm_clear_descriptor_cache", &rb::gemm_clear_descriptor_cache);
-  m.def("gemm_pair_clusters", &rb::gemm_pair_clusters);
-  m.def("gemm_set_trace", [](const OptTensor& t) {
-    if (!t.has_value()) { rb::gemm_set_trace(nullptr); return; }
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() >= 16 * 512, "trace buffer: int64 CUDA tensor of >= 8192 elements");
-    rb::gemm_set_trace(t->data_ptr());
-  });
   m.def("rmsnorm_fwd", &rmsnorm_fwd, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("rstd"), py::arg("eps"), py::arg("xd"), py::arg("seed"),
         py::arg("keys"), py::arg("p"), py::arg("q8") = py::none(), py::arg("q_inv_scale") = py::none(), py::arg("q_amax") = py::none());
   m.def("rmsnorm_bwd", &rmsnorm_bwd);
@@ -628,12 +621,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fp8_prep", &fp8_prep, py::arg("state"), py::arg("w_scale"), py::arg("inv_sx"), py::arg("alpha_main"), py::arg("alpha_inv"), py::arg("margin"),
         py::arg("n_e4m3") = -1);
   m.def("attention_fwd", &attention_fwd);
-  m.def("attention_occupancy", &rb::attention_occupancy);
-  m.def("attention_set_trace", [](const OptTensor& t) {
-    if (!t.has_value()) { rb::attention_set_trace(nullptr); return; }
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kLong && t->is_contiguous() && t->numel() >= 8 * 64, "trace buffer: int64 CUDA tensor of >= 512 elements");
-    rb::attention_set_trace(t->data_ptr());
-  });
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("delta"), py::arg("dqkv"),
         py::arg("B"), py::arg("T"), py::arg("nh"), py::arg("hd"), py::arg("scale"), py::arg("ds_workspace") = py::none());
   m.def("attention_ds_workspace_elems", &rb::attention_ds_workspace_elems);

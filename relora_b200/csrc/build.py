@@ -1,12 +1,12 @@
-"""Build the in-tree sm_100a extension ``relora_b200/_C.so``.
+"""Build the in-tree sm_90a extension ``relora_b200/_C.so``.
 
     python -m relora_b200.csrc.build [--force] [--verbose]
 
 Kernel sources are plain CUDA (no torch headers) compiled with
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo``; ``bindings.cpp`` (pybind11 over
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo``; ``bindings.cpp`` (pybind11 over
 ``torch::Tensor``) is compiled with the host compiler and everything is linked into one shared
 object next to the package.  nvcc cross-compiles without a GPU, so this runs on the CPU build box;
-the resulting ``.so`` travels with the repository snapshot to the B200.  A content hash of the
+the resulting ``.so`` travels with the repository snapshot to the H100.  A content hash of the
 sources + flags makes rebuilds incremental.
 """
 from __future__ import annotations
@@ -27,12 +27,12 @@ PKG = os.path.dirname(HERE)
 BUILD_DIR = os.path.join(HERE, "_build")
 TARGET = os.path.join(PKG, "_C.so")
 
-CUDA_SOURCES = ["gemm_tcgen05.cu", "elementwise.cu", "norm_warp.cu", "rope.cu", "optim.cu", "loss.cu", "attention.cu", "fp8.cu", "comm.cu", "neox.cu", "gemm_mx.cu"]
+CUDA_SOURCES = ["gemm_wgmma.cu", "elementwise.cu", "norm_warp.cu", "rope.cu", "optim.cu", "loss.cu", "attention.cu", "fp8.cu", "comm.cu", "neox.cu", "gemm_mx.cu"]
 CPP_SOURCES = ["bindings.cpp"]
-HEADERS = ["common.cuh", "sm100.cuh", "gemm.h", "tensormap.h", "fp8out.h", "kernels.h", "attention.h", "comm.h"]
+HEADERS = ["common.cuh", "sm90.cuh", "gemm.h", "tensormap.h", "fp8out.h", "kernels.h", "attention.h", "comm.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ] + os.environ.get("RB_EXTRA_NVCC_FLAGS", "").split()  # e.g. -DRB_ATTN_GROUPS_FWD=3 for kernel experiments
 

@@ -1,4 +1,4 @@
-// Hand-written NVLink collectives for the data-parallel update (sm_100a, NVLink 5 / NVSwitch).
+// Hand-written NVLink collectives for the data-parallel update (sm_90a, NVLink 4 / NVSwitch).
 //
 // The reference all-reduces every gradient bucket through NCCL on every micro-batch (DDP without no_sync,
 // torchrun_main.py:616-622, 796-800) and then runs clip_grad_norm_ and torch.optim.AdamW as separate passes.

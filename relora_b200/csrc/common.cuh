@@ -42,7 +42,7 @@ inline void check(cudaError_t e, const char* what) {
 inline bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
-    const char* e = getenv("RB_PDL");  // opt-in: measured neutral on B200 inside the captured micro-step (404.3 k vs 405.2 k tokens/s)
+    const char* e = getenv("RB_PDL");  // opt-in
     v = (e != nullptr && atoi(e) != 0) ? 1 : 0;
   }
   return v != 0;

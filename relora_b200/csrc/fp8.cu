@@ -1,4 +1,4 @@
-// E4M3 quantisation for the fp8 frozen-weight path (tcgen05 kind::f8f6f4 GEMMs, csrc/gemm_tcgen05.cu).
+// E4M3 quantisation for the fp8 frozen-weight path (e4m3 wgmma GEMMs, csrc/gemm_wgmma.cu).
 // Capability being replaced: the reference's bitsandbytes-quantised frozen weights (peft_pretraining/relora.py:224-236,
 // 277-299, 314-317: NF4 / int8 storage, dequantise -> bf16 matmul); here the frozen GEMMs themselves run in fp8.
 //

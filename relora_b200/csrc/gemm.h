@@ -1,4 +1,4 @@
-// Host API of the tcgen05 GEMM family (implemented in gemm_tcgen05.cu).
+// Host API of the wgmma GEMM family (implemented in gemm_wgmma.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,7 +44,6 @@ struct GemmDesc {
   bool fp8 = false;  // A1 / B1 hold E4M3 bytes (K-major, leading dimensions in bytes); A2 / B2 (the LoRA branch) stay bf16
   int block_n = 0;  // 0 = auto, else 128 or 256
   int split_k = 1;  // 1 = off, 0 = auto, >1 = fixed (fp32 accumulate outputs only: partial sums via atomics)
-  int cta_pair = -1; // -1 = auto, 0 = single-CTA tiles, 1 = CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles; needs block_n 256)
   // dropout-combine epilogue (backward of the LoRA branch): if n_lora_acc > 0 the A2/B2 products of
   // the first n_lora_acc K2-windows (each of width lora_r) are kept in separate accumulators and combined as
   //     out = acc0 + sum_g keep_g(row, col) * acc_{1+g} * inv_keep
@@ -68,8 +67,8 @@ struct LoraDxDesc {
   void* out = nullptr;
   long long ldc = 0;
   int M = 0, N = 0, Kb = 0, r = 0, groups = 1;
-  // Kb == 0: `base` [M, N] bf16 already holds dy·W (computed by the 256-wide / CTA-pair GEMM, the better choice for long
-  // reductions); this kernel then only adds the masked low-rank terms
+  // Kb == 0: `base` [M, N] bf16 already holds dy·W (computed by a separate GEMM); this kernel then only adds the masked
+  // low-rank terms
   const void* base = nullptr;
   long long ld_base = 0;
   uint32_t drop_threshold16 = 0;  // round(p * 65536); 0 = keep everything (no dropout)
@@ -81,12 +80,5 @@ void lora_dx(const LoraDxDesc& d, cudaStream_t stream);
 
 // Drop cached TMA descriptors (call when buffers are freed / reallocated).
 void gemm_clear_descriptor_cache();
-
-// Co-resident CTA pairs the hardware reports for the cta_group::2 GEMM (0 until the first pair launch).
-int gemm_pair_clusters();
-
-// Diagnostics: CTA 0 of every following GEMM launch writes clock64 stamps of its pipeline events into `buf`
-// (6 x 512 int64: producer issue / MMA full / MMA acc-free / MMA tile commit / epilogue start / epilogue end); nullptr = off.
-void gemm_set_trace(void* buf);
 
 }  // namespace rb

@@ -1,5 +1,5 @@
-// Block-scaled MXFP8 path for the frozen weights (SURVEY K15): tcgen05.mma.kind::mxf8f6f4.block_scale with the ue8m0 scale
-// factors staged shared memory -> tensor memory by tcgen05.cp, plus the quantisation / requantisation kernels.
+// Block-scaled MXFP8 path for the frozen weights (SURVEY K15): e4m3 wgmma per 32-element scale block with the ue8m0 scale
+// factors applied to the fp32 partial products in registers, plus the quantisation / requantisation kernels.
 //
 // Replaces the reference's bitsandbytes storage (peft_pretraining/relora.py:222-238 Params4bit / Int8Params, :314-317 matmul_4bit /
 // bnb.matmul, :277-299 dequantise -> add -> requantise merge).  Formats (OCP MX): E4M3 elements, one UE8M0 (power of two) scale per
@@ -10,11 +10,11 @@
 //       - the forward GEMM  y = x · Wᵀ   (B operand K-major,  scale of (n, k/32) = tile scale)
 //       - the backward GEMM dx = dy · W  (B operand MN-major, scale of (k, n/32) = the same tile scale)
 //     -> 1 byte per parameter + two expanded scale arrays (1/32 byte each) instead of two fp8 copies.
+//     wgmma reads 8-bit operands K-major only: an MN-major B tile is transposed in shared memory by the consumer warpgroups.
 //
-// Scale-factor layout in global memory (the layout tcgen05.cp / the MMA expect, cf. CUTLASS Sm1xxBlockScaledBasicChunk): for a
-// block of 128 rows x 4 scale columns (= 128 reduction elements) 512 contiguous bytes,
+// Scale-factor layout in global memory: for a block of 128 rows x 4 scale columns (= 128 reduction elements) 512 contiguous bytes,
 //     byte[(r % 32) * 16 + (r / 32) * 4 + j]  =  scale(row r, scale column j)
-// blocks ordered [row block][k group].  One such block is one TMEM "column quad" after  tcgen05.cp.32x128b.warpx4 .
+// blocks ordered [row block][k group].
 #include <cuda.h>
 #include <cuda_fp8.h>
 
@@ -23,70 +23,33 @@
 
 #include "common.cuh"
 #include "kernels.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "tensormap.h"
 
 namespace rb {
 
-using namespace sm100;
+using namespace sm90;
 
 namespace {
 
 constexpr int BM = 128, BN = 128;
 constexpr int KB8 = 128;  // fp8 elements per k-block (128 bytes = one swizzle row)
 constexpr int KB16 = 64;  // bf16 elements per k-block of the optional second (LoRA) segment
-constexpr int kStages = 4;
+constexpr int kStages = 5;
 constexpr int kTileBytes = BM * 128;           // 16 KB per operand tile
 constexpr int kStageBytes = 2 * kTileBytes;    // A + B
 constexpr int kSfBytes = 512;                  // one 128-row x 4-scale block
-constexpr int kSlabBytes = BM * 128;           // 128 x 64 bf16 output slab
-constexpr int kSlabs = 2;
-constexpr int kSmemTiles = kStages * kStageBytes;             // 128 KB
-constexpr int kSmemSf = kStages * 2 * kSfBytes;               // 4 KB
-constexpr int kSmemTotal = kSmemTiles + kSmemSf + 1024 + kSlabs * kSlabBytes + 1024;
-constexpr uint32_t kTmemCols = 512;  // 2 x 128 accumulator columns + 2 x 8 scale columns -> next power of two
-constexpr uint32_t kSfCol0 = 256;    // scale factors live behind the two accumulator stages
-
-// ---- instruction descriptor of kind::mxf8f6f4.block_scale (cute::UMMA::InstrDescriptorBlockScaled):
-//   [4,6) b_sf_id  [7,10) a_format (0 = E4M3)  [10,13) b_format  [15] a_major  [16] b_major  [17,23) N>>3  [23] scale_format (1 = UE8M0)
-//   [24,29) M>>4  [29,31) a_sf_id
-__device__ __forceinline__ uint32_t make_idesc_mx(int M, int N, int b_mn_major, uint32_t a_sf_id, uint32_t b_sf_id) {
-  return (b_sf_id << 4) | (uint32_t(b_mn_major) << 16) | (uint32_t(N >> 3) << 17) | (1u << 23) | (uint32_t(M >> 4) << 24) | (a_sf_id << 29);
-}
-__device__ __forceinline__ void umma_mx_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t tmem_sfa, uint32_t tmem_sfb,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(tmem_sfa), "r"(tmem_sfb)
-      : "memory");
-}
-// shared memory -> tensor memory: 32 rows x 128 bits, replicated into the four 32-lane quadrants (the scale-factor copy)
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t tmem_dst, uint64_t smem_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(tmem_dst), "l"(smem_desc) : "memory");
-}
-// K-major, no swizzle: 8-row groups of 16-byte rows are 128 bytes apart (SBO); one 16-byte column -> LBO unused
-__device__ __forceinline__ uint64_t make_desc_sf(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= uint64_t((smem_addr >> 4) & 0x3FFF);
-  d |= uint64_t(1) << 16;            // LBO (unused: a single 16-byte column)
-  d |= uint64_t(128 >> 4) << 32;     // SBO
-  d |= uint64_t(1) << 46;            // descriptor version (sm_100)
-  return d;                          // layout type 0 = no swizzle ("interleave")
-}
-// fp8 operand descriptors (128-byte swizzle).  K-major: rows of 128 B = 128 elements, 32 elements (32 B) per MMA.
-// MN-major: rows of 128 B = 128 MN elements, 8-row (K) groups 1024 B apart, 32 K rows (4096 B) per MMA.
-__device__ __forceinline__ uint64_t desc8_k(uint32_t smem_addr, int kstep) { return make_desc_sw128(smem_addr + kstep * 32, 16, 1024); }
-__device__ __forceinline__ uint64_t desc8_mn(uint32_t smem_addr, int kstep) { return make_desc_sw128(smem_addr + kstep * 4096, 16384, 1024); }
-__device__ __forceinline__ uint64_t desc16_k(uint32_t smem_addr, int kstep) { return make_desc_sw128(smem_addr + kstep * 32, 16, 1024); }
+constexpr int kSmemTiles = kStages * kStageBytes;             // 160 KB
+constexpr int kSmemSf = kStages * 2 * kSfBytes;               // 5 KB
+constexpr int kSmemTotal = kSmemTiles + kTileBytes + kSmemSf + 1024 + 1024;  // + transposed B tile, barriers, alignment
 
 __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+__device__ __forceinline__ float ue8m0_value(uint8_t e) { return __uint_as_float(e == 0 ? 0x00400000u : uint32_t(e) << 23); }
+__device__ __forceinline__ int sf_byte(int r, int j) { return (r & 31) * 16 + (r >> 5) * 4 + j; }
 
 struct MxArgs {
   int M, N, K8, K2;                 // K8: fp8 reduction length (multiple of 128), K2: bf16 LoRA segment (multiple of 64, may be 0)
@@ -94,220 +57,169 @@ struct MxArgs {
   const uint8_t* sfb;               // [n blocks][sfb_kg][512]
   int sfa_kg, sfb_kg;               // 128-element k groups per row block in the arrays
   int num_m_tiles, num_n_tiles;
-  int has_res;
-  float alpha2;                     // unused (the LoRA operand already carries its scale)
+  bf16* out;
+  long long ldc;
+  const bf16* residual;
+  long long ldr;
 };
 
+// 256 consumer threads: MN-major [128 K rows][128 N bytes] (128-byte swizzle) -> K-major [128 N rows][128 K bytes] (same swizzle)
+__device__ __forceinline__ void transpose_fp8_tile(const uint8_t* src, uint8_t* dst, int t) {
+#pragma unroll 1
+  for (int item = t; item < 128 * 8; item += 256) {
+    const int n = item & 127, c = item >> 7;  // output row n, 16-byte chunk c (K = 16c .. 16c + 15)
+    uint32_t w[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int e = 0; e < 16; ++e) {
+      const int k = c * 16 + e;
+      const uint32_t v = src[k * 128 + ((((n >> 4) ^ (k & 7))) << 4) + (n & 15)];
+      w[e >> 2] |= v << ((e & 3) * 8);
+    }
+    *reinterpret_cast<uint4*>(dst + n * 128 + ((c ^ (n & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
 template <bool B_MN>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 gemm_mx_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_a2,
-               const __grid_constant__ CUtensorMap map_b2, const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
-               const MxArgs p) {
+               const __grid_constant__ CUtensorMap map_b2, const MxArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sf_base = smem + kSmemTiles;
+  uint8_t* bt = smem + kSmemTiles;  // transposed B tile (MN-major B only)
+  uint8_t* sf_base = bt + kTileBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(sf_base + kSmemSf);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* res_bar = tmem_empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + kSlabs);
-  uint8_t* slab_base = sf_base + kSmemSf + 1024;
 
-  const uint32_t warp = warp_id(), lane = lane_id();
-  if (warp == 0 && lane == 0) {
+  const uint32_t warp = warp_id();
+  const int wg = threadIdx.x / 128;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    tma_prefetch_desc(&map_out);
     if (p.K2 > 0) {
       tma_prefetch_desc(&map_a2);
       tma_prefetch_desc(&map_b2);
     }
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 256);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 128);
-    }
-    for (int a = 0; a < kSlabs; ++a) mbar_init(&res_bar[a], 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);  // known warp-uniform
 
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
   const int kb8 = p.K8 / KB8, kb16 = p.K2 / KB16;
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer: the whole warp walks the loop, one elected lane
-    // issues (uniform control flow lets ptxas keep addresses / descriptors in uniform registers instead of wrapping every
-    // UTMALDG / UTC*MMA in an ELECT + R2UR + BRA.U.ANY loop; see gemm_tcgen05.cu)
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int tm = tile / p.num_n_tiles, tn = tile % p.num_n_tiles;
-        const int m0 = tm * BM, n0 = tn * BN;
-        for (int kb = 0; kb < kb8 + kb16; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * kStageBytes;
-          uint8_t* sb = sa + kTileBytes;
-          if (!elect_one()) {
-          } else if (kb < kb8) {
-            mbar_arrive_expect_tx(&full_bar[stage], kStageBytes + 2 * kSfBytes);
-            tma_load_2d(&map_a, &full_bar[stage], sa, kb * KB8, m0, kEvictNormal);
-            if constexpr (B_MN) tma_load_2d(&map_b, &full_bar[stage], sb, n0, kb * KB8, kEvictLast);  // box {128 (MN), 128 (K rows)}
-            else tma_load_2d(&map_b, &full_bar[stage], sb, kb * KB8, n0, kEvictLast);
-            bulk_copy_g2s(sf_base + stage * 2 * kSfBytes, p.sfa + ((long long)tm * p.sfa_kg + kb) * kSfBytes, kSfBytes, &full_bar[stage]);
-            bulk_copy_g2s(sf_base + stage * 2 * kSfBytes + kSfBytes, p.sfb + ((long long)tn * p.sfb_kg + kb) * kSfBytes, kSfBytes,
-                          &full_bar[stage]);
-          } else {  // bf16 LoRA segment: [x | u]·[W | B]ᵀ shares the accumulator
-            const int k = (kb - kb8) * KB16;
-            mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-            tma_load_2d(&map_a2, &full_bar[stage], sa, k, m0, kEvictNormal);
-            tma_load_2d(&map_b2, &full_bar[stage], sb, k, n0, kEvictLast);
-          }
-          __syncwarp();
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (whole warp, one elected lane issues)
-    {
-      constexpr uint32_t idesc16 = make_idesc_bf16(BM, BN, 0, 0);
-      int stage = 0, acc = 0, sfbuf = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kb8 + kb16; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem) + stage * kStageBytes;
-          const uint32_t sb = sa + kTileBytes;
-          if (!elect_one()) {
-          } else if (kb < kb8) {
-            // scale factors of this k-block: shared memory -> 4 + 4 tensor-memory columns (tcgen05.cp and tcgen05.mma execute in
-            // issue order, so the copies are complete before the MMAs below read them; two buffers alternate anyway)
-            const uint32_t sfa_t = tmem_base + kSfCol0 + sfbuf * 8, sfb_t = sfa_t + 4;
-            const uint32_t sf_s = smem_u32(sf_base + stage * 2 * kSfBytes);
-            tmem_cp_32x128b_warpx4(sfa_t, make_desc_sf(sf_s));
-            tmem_cp_32x128b_warpx4(sfb_t, make_desc_sf(sf_s + kSfBytes));
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k) {  // K = 32 per instruction; scale column k of the block (sf id, also in bits 30-31 of the address)
-              const uint64_t da = desc8_k(sa, k);
-              const uint64_t db = B_MN ? desc8_mn(sb, k) : desc8_k(sb, k);
-              umma_mx_ss(d_tmem, da, db, make_idesc_mx(BM, BN, B_MN ? 1 : 0, k, k), sfa_t | (k << 30), sfb_t | (k << 30), (kb | (int)k) != 0);
-            }
-            umma_commit(&empty_bar[stage]);
-          } else {
-#pragma unroll
-            for (int k = 0; k < KB16 / 16; ++k) umma_f16_ss(d_tmem, desc16_k(sa, k), desc16_k(sb, k), idesc16, 1u);
-            umma_commit(&empty_bar[stage]);
-          }
-          __syncwarp();
-          if (kb < kb8) sfbuf ^= 1;
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (elect_one()) umma_commit(&tmem_full[acc]);
-        __syncwarp();
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue: TMEM -> bf16 slab (+ residual by TMA) -> TMA store
-    const uint32_t quad = warp & 3;
-    const uint32_t rloc = quad * 32 + lane;
-    const bool issuer = (threadIdx.x == 128);
-    int acc = 0, slab_counter = 0;
-    uint32_t acc_phase = 0;
+  if (wg == 0) {
+    // ===================================================================== TMA producer (whole warp walks the loop, one lane issues)
+    setmaxnreg_dec<40>();
+    if (warp != 0) return;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile / p.num_n_tiles) * BM, n0 = (tile % p.num_n_tiles) * BN;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int sl = 0; sl < BN / 64; ++sl) {
-        const int sb_i = slab_counter % kSlabs;
-        uint8_t* slab = slab_base + sb_i * kSlabBytes;
-        uint8_t* rowp = slab + rloc * 128;
-        if (p.has_res) {
-          if (issuer) {
-            mbar_arrive_expect_tx(&res_bar[sb_i], kSlabBytes);
-            tma_load_2d(&map_res, &res_bar[sb_i], slab, n0 + sl * 64, m0, kEvictNormal);
-          }
-          mbar_wait(&res_bar[sb_i], (slab_counter / kSlabs) & 1);
+      const int tm = tile / p.num_n_tiles, tn = tile % p.num_n_tiles;
+      const int m0 = tm * BM, n0 = tn * BN;
+      for (int kb = 0; kb < kb8 + kb16; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * kStageBytes;
+        uint8_t* sb = sa + kTileBytes;
+        if (!elect_one()) {
+        } else if (kb < kb8) {
+          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes + 2 * kSfBytes);
+          tma_load_2d(&map_a, &full_bar[stage], sa, kb * KB8, m0, kEvictNormal);
+          if constexpr (B_MN) tma_load_2d(&map_b, &full_bar[stage], sb, n0, kb * KB8, kEvictLast);  // box {128 (MN), 128 (K rows)}
+          else tma_load_2d(&map_b, &full_bar[stage], sb, kb * KB8, n0, kEvictLast);
+          bulk_copy_g2s(sf_base + stage * 2 * kSfBytes, p.sfa + ((long long)tm * p.sfa_kg + kb) * kSfBytes, kSfBytes, &full_bar[stage]);
+          bulk_copy_g2s(sf_base + stage * 2 * kSfBytes + kSfBytes, p.sfb + ((long long)tn * p.sfb_kg + kb) * kSfBytes, kSfBytes,
+                        &full_bar[stage]);
+        } else {  // bf16 LoRA segment: [x | u]·[W | B]ᵀ shares the accumulator
+          const int k = (kb - kb8) * KB16;
+          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+          tma_load_2d(&map_a2, &full_bar[stage], sa, k, m0, kEvictNormal);
+          tma_load_2d(&map_b2, &full_bar[stage], sb, k, n0, kEvictLast);
         }
-        uint32_t r0[32], r1[32];
-        tmem_ld_32x32b_x32(tmem_addr(tmem_base, quad * 32, acc * BN + sl * 64), r0);
-        tmem_ld_32x32b_x32(tmem_addr(tmem_base, quad * 32, acc * BN + sl * 64 + 32), r1);
-        tmem_ld_wait();
-        if (sl == BN / 64 - 1) {
-          tc_fence_before();
-          mbar_arrive(&tmem_empty[acc]);
+        __syncwarp();
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
         }
-        uint4 packed[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          float f[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) f[i] = __uint_as_float((q < 4) ? r0[q * 8 + i] : r1[(q - 4) * 8 + i]);
-          if (p.has_res) {
-            float a[8];
-            unpack8(*reinterpret_cast<const uint4*>(rowp + ((q ^ (rloc & 7)) << 4)), a);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) f[i] += a[i];
-          }
-          packed[q] = pack8(f);
-        }
-#pragma unroll
-        for (int q = 0; q < 8; ++q) *reinterpret_cast<uint4*>(rowp + ((q ^ (rloc & 7)) << 4)) = packed[q];
-        fence_proxy_async_smem();
-        named_bar_sync(1, 128);
-        if (issuer) {
-          if (n0 + sl * 64 < p.N) {
-            tma_store_2d(&map_out, slab, n0 + sl * 64, m0);
-            tma_store_commit();
-          }
-          tma_store_wait_read<kSlabs - 1>();  // the other slab (the next one to be written) has been read by its store
-        }
-        named_bar_sync(1, 128);
-        ++slab_counter;
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
       }
     }
-    if (issuer) tma_store_wait<0>();
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+
+  // ======================================================================= consumers: 64 rows each
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;
+  const int ct = threadIdx.x - 128;
+  const uint32_t smem0 = smem_u32(smem);
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2], part[BN / 2];
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m0 = (tile / p.num_n_tiles) * BM, n0 = (tile % p.num_n_tiles) * BN;
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < kb8 + kb16; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem0 + stage * kStageBytes + cw * 8192;
+      uint32_t sb = smem0 + stage * kStageBytes + kTileBytes;
+      if (kb < kb8) {
+        if constexpr (B_MN) {
+          named_bar_sync(1, 256);  // both warpgroups are done with the previous transposed tile
+          transpose_fp8_tile(smem + stage * kStageBytes + kTileBytes, bt, ct);
+          fence_proxy_async_smem();
+          named_bar_sync(1, 256);
+          sb = smem_u32(bt);
+        }
+        const uint8_t* sfa = sf_base + stage * 2 * kSfBytes;
+        const uint8_t* sfb = sfa + kSfBytes;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {  // one K = 32 wgmma per scale column, scaled into the accumulator
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+          wgmma_fence();
+          wgmma_e4m3_ss_n128(part, desc_kmajor(sa + kk * 32), desc_kmajor(sb + kk * 32));
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs(part);
+          const float s_lo = ue8m0_value(sfa[sf_byte(cw * 64 + frag_row(0), kk)]);
+          const float s_hi = ue8m0_value(sfa[sf_byte(cw * 64 + frag_row(2), kk)]);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) {
+            const float sbv = ue8m0_value(sfb[sf_byte(frag_col(i), kk)]);
+            acc[i] = fmaf(part[i], (((i >> 1) & 1) ? s_hi : s_lo) * sbv, acc[i]);
+          }
+        }
+      } else {
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < KB16 / 16; ++k) wgmma_bf16_ss_n128<0, 0>(acc, desc_kmajor(sa + k * 32), desc_kmajor(sb + k * 32));
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(acc);
+      }
+      mbar_arrive(&empty_bar[stage]);
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = m0 + cw * 64 + frag_row(i), col = n0 + frag_col(i);
+      if (row >= p.M || col >= p.N) continue;  // N is a multiple of 8: column pairs are whole
+      float v0 = acc[i], v1 = acc[i + 1];
+      if (p.residual != nullptr) {
+        const float2 r = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.residual + (long long)row * p.ldr + col));
+        v0 += r.x;
+        v1 += r.y;
+      }
+      *reinterpret_cast<uint32_t*>(p.out + (long long)row * p.ldc + col) = pack_bf16x2(v0, v1);
+    }
   }
 }
+
 
 // ---------------------------------------------------------------------------------------------- quantisation
 __device__ __forceinline__ uint32_t sf_offset(long long row, int sfcol, int kg_per_block) {
@@ -500,36 +412,35 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   const int K8 = (d.K + 127) / 128 * 128;
   if (d.K2 % KB16) throw std::runtime_error("gemm_mx: the bf16 segment must be a multiple of 64");
   if (d.ldc % 8 || (reinterpret_cast<uintptr_t>(d.out) & 15)) throw std::runtime_error("gemm_mx: output must be 16-byte aligned");
+  if (d.N % 8) throw std::runtime_error("gemm_mx: N must be a multiple of 8");
   MxArgs p;
   p.M = d.M; p.N = d.N; p.K8 = K8; p.K2 = d.K2;
   p.sfa = reinterpret_cast<const uint8_t*>(d.sfa); p.sfb = reinterpret_cast<const uint8_t*>(d.sfb);
   p.sfa_kg = K8 / 128; p.sfb_kg = K8 / 128;
   p.num_m_tiles = ceil_div(d.M, BM); p.num_n_tiles = ceil_div(d.N, BN);
-  p.has_res = d.residual != nullptr ? 1 : 0;
-  p.alpha2 = 1.f;
+  p.out = reinterpret_cast<bf16*>(d.out); p.ldc = d.ldc;
+  p.residual = reinterpret_cast<const bf16*>(d.residual); p.ldr = d.ldr;
   // operands: fp8 bytes; A [M, K8] K-major (pitch lda); B K-major [N, K8] (pitch ldb) or MN-major [K8 rows, N] (pitch ldb)
   CUtensorMap ma = make_map_2d_sw128(d.a, K8, d.M, d.lda, KB8, BM, 1);
   CUtensorMap mb = d.b_mn_major ? make_map_2d_sw128(d.b, d.N, K8, d.ldb, 128, KB8, 1) : make_map_2d_sw128(d.b, K8, d.N, d.ldb, KB8, BN, 1);
-  CUtensorMap mo = make_map_2d_sw128(d.out, d.N, d.M, d.ldc, 64, BM, 2);
-  CUtensorMap ma2 = ma, mb2 = mb, mr = mo;
+  CUtensorMap ma2 = ma, mb2 = mb;
   if (d.K2 > 0) {
     ma2 = make_map_2d_sw128(d.a2, d.K2, d.M, d.lda2, KB16, BM, 2);
     mb2 = make_map_2d_sw128(d.b2, d.K2, d.N, d.ldb2, KB16, BN, 2);
   }
   if (d.residual != nullptr) {
     if (d.ldr % 8 || (reinterpret_cast<uintptr_t>(d.residual) & 15)) throw std::runtime_error("gemm_mx: residual must be 16-byte aligned");
-    mr = make_map_2d_sw128(d.residual, d.N, d.M, d.ldr, 64, BM, 2);
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   if (d.b_mn_major) {
     static bool cfg = false;
     if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
-    launch_k(gemm_mx_kernel<true>, grid, 256, kSmemTotal, stream, ma, mb, ma2, mb2, mo, mr, p);
+    launch_k(gemm_mx_kernel<true>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
   } else {
     static bool cfg = false;
     if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
-    launch_k(gemm_mx_kernel<false>, grid, 256, kSmemTotal, stream, ma, mb, ma2, mb2, mo, mr, p);
+    launch_k(gemm_mx_kernel<false>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
   }
   RB_CHECK_LAUNCH("gemm_mx");
 }

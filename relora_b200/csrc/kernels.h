@@ -66,7 +66,7 @@ void neox_rope(void* qkv, long long ld, long long rows, int T, int nh, int hd, i
                bool inverse, cudaStream_t s);
 
 // ---- block-scaled MXFP8 path (gemm_mx.cu) ------------------------------------------------------
-// Scale factors live in [row block of 128][group of 128 reduction elements][512 bytes] blocks (the tcgen05.cp / MMA layout).
+// Scale factors live in [row block of 128][group of 128 reduction elements][512 bytes] blocks (the layout the MX GEMM stages per k-block).
 long long mx_sf_bytes(long long rows, long long k_elems);
 // x bf16 [M, K] (pitch ldx) -> E4M3 q [M, Kpad] (pitch ldq >= Kpad = K rounded up to 128, padding written as zero) + UE8M0 scales per (row, 32 cols)
 void mx_quantize_rows(const void* x, long long ldx, void* q, long long ldq, void* sf, int M, int K, cudaStream_t s);

@@ -1,4 +1,4 @@
-"""Whole-model fused executor for Llama + ReLoRA on B200.
+"""Whole-model fused executor for Llama + ReLoRA on H100.
 
 The reference executes one ``ReLoRaLinear`` as ~8 eager kernels (``relora.py:319-322``) and a decoder
 layer as ~100 (``modeling_llama.py:243-308``), re-reading every activation several times, and is
@@ -7,7 +7,7 @@ launch/CPU-bound at the 250M scale.  This executor instead
 * keeps the frozen weights of a layer *stacked* (``Wqkv [3h,h]``, ``Wgu [2f,h]``) and the LoRA factors
   stacked alongside (``A_qkv [3r,h]``, ``B_qkv [3h,r]`` …) — the ``nn.Module`` parameters are views into these
   buffers, so checkpoints keep the reference layout;
-* runs every projection as ONE tcgen05 GEMM launch with the low-rank up-projection folded into the K loop
+* runs every projection as ONE wgmma GEMM launch with the low-rank up-projection folded into the K loop
   (``y = [x | u]·[W | B]ᵀ``, residual add in the epilogue), the three / two down-projections of a stacked group
   as one grouped launch, and all backward GEMMs (``dx``, ``du``, stacked ``dA`` / ``dB`` with split-K) on the same
   kernel reading operands MN-major in place — no transposed copies, no autograd graph;
@@ -93,7 +93,7 @@ class FusedLlamaStepper:
         cfg = self.inner.config
         self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
         self.hd = self.h // self.nh
-        self.fp = (self.f + 127) // 128 * 128  # padded intermediate size (zero rows / columns, see DESIGN.md §2)
+        self.fp = (self.f + 127) // 128 * 128  # padded intermediate size (zero rows / columns keep every GEMM extent a multiple of the 128-wide tile)
         self.r = model.r
         self.L = cfg.num_hidden_layers
         self.eps = cfg.rms_norm_eps
@@ -268,15 +268,14 @@ class FusedLlamaStepper:
         native_ok = self.hd % 8 == 0 and self.hd <= 64
         if attention == "native" and not native_ok:
             raise RuntimeError(f"--attention native supports head_dim <= 64 (multiple of 8), got {self.hd}")
-        # auto: this repo's tcgen05 kernels (csrc/attention.cu) wherever they apply -- the hot path then contains no library
-        # attention call; `--attention sdpa` selects torch SDPA (cuDNN's sm100 kernels; measured per layer at B 24 x T 512 x 16 x 48
-        # in bench/attn_bench.py, see profiles/) and is what larger head dims fall back to
+        # auto: this repo's wgmma kernels (csrc/attention.cu) wherever they apply -- the hot path then contains no library
+        # attention call; `--attention sdpa` selects torch SDPA (cuDNN; bench/attn_bench.py times both) and is what larger head
+        # dims fall back to
         self.native_attn = attention == "native" or (attention == "auto" and native_ok)
         self.side = torch.cuda.Stream(device=dev) if overlap_wgrad else None
         self.fused_dx = os.environ.get("RELORA_B200_FUSED_DX", "1") != "0"
-        # stacked output width from which dx uses two kernels (frozen-path GEMM on 256-wide / CTA-pair tiles + a mask-and-add pass).
-        # The pass costs 30-120 us, so it only pays for long reductions: per-group timings in profiles/ROOFLINE.md put the bf16
-        # break-even near 4096; with fp8 input-gradient GEMMs (twice the rate) at 2048.
+        # stacked output width from which dx uses two kernels (frozen-path GEMM on 256-wide tiles + a mask-and-add pass) instead of
+        # the one-kernel form; the thresholds (4096 bf16, 2048 with fp8 input-gradient GEMMs) have not been re-tuned on the H100.
         self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0")) or (2048 if self.fp8_bwd else 4096)
         self._wg_done: Dict[str, torch.cuda.Event] = {}
         # --deterministic: the stacked dA / dB weight-gradient GEMMs run without split-K (one CTA owns an output tile for the whole token
@@ -345,9 +344,6 @@ class FusedLlamaStepper:
             self.attn_o = e(L, M, h)
             self.lse = torch.empty(L, B, self.nh, T, dtype=torch.float32, device=dev)
             self.delta = torch.empty(B, self.nh, T, dtype=torch.float32, device=dev)
-            # dSᵀ workspace of the backward: the dK/dV kernel stores its tiles, dQ = dS·K runs as a plain TMA -> MMA kernel
-            self.ds_ws = (e(self.C.attention_ds_workspace_elems(B, T, self.nh))
-                          if os.environ.get("RELORA_B200_ATTN_DS", "1") != "0" else None)
         self.parts = e(M, max(3 * h, f))
         ldv = (self.V + 7) // 8 * 8
         self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
@@ -360,7 +356,7 @@ class FusedLlamaStepper:
     def _attention(self, qkv: torch.Tensor, train: bool, sl: int = 0):
         B, T, nh, hd = self.B_, self.T_, self.nh, self.hd
         if self.native_attn:
-            # tcgen05 flash attention straight out of the packed projection buffer (csrc/attention.cu); the output and the
+            # wgmma flash attention straight out of the packed projection buffer (csrc/attention.cu); the output and the
             # log-sum-exp of the layer are what the backward kernels need
             out = self.attn_o[sl]
             self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd))
@@ -525,7 +521,7 @@ class FusedLlamaStepper:
                     g(dy, S_W, base_out, M=M, N=K, K1=G * Ng, b1_mn=True)
                 C.lora_dx(None, None, du, S_A, out, sd, ks, pp, base_out)
             else:
-                # one kernel: out = dy·W + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)  (1+G accumulators in tensor memory, masks in the epilogue)
+                # one kernel: out = dy·W + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)  (masked LoRA terms folded into the register accumulator)
                 C.lora_dx(dy, S_W, du, S_A, out, sd, ks, pp)
         else:
             # frozen path: base = dy · W     (W stacked [G·Ng, K], read MN-major)
@@ -571,7 +567,7 @@ class FusedLlamaStepper:
             if self.native_attn:
                 self._join("qkv")  # the previous layer's qkv weight gradients read dqkv / du_qkv
                 C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
-                                1.0 / math.sqrt(hd), self.ds_ws)
+                                1.0 / math.sqrt(hd))
                 C.rope_inplace(self.dqkv, T, 2 * nh, hd, hd, self.cos, self.sin, True, 0)  # back through the rotation of q, k
                 dq = None
             else:
@@ -729,7 +725,7 @@ class FusedLlamaStepper:
 
     @torch.no_grad()
     def merge_and_reinit(self):
-        """W += s·B@A on the stacked buffers (tcgen05 GEMM accumulating into W in fp32), then hash re-init."""
+        """W += s·B@A on the stacked buffers (wgmma GEMM accumulating into W in fp32), then hash re-init."""
         from ..ops import reference as ref
 
         g, r = fused.gemm, self.r

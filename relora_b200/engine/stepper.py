@@ -9,7 +9,7 @@ transport and exposes two calls:
 This mirrors one iteration of the reference hot loop (``torchrun_main.py:783-826``) with the
 gradient all-reduce hoisted out of the accumulation loop.  :class:`ModuleStepper` drives any
 ``nn.Module`` whose forward returns ``.loss`` (CPU/gloo and the generic GPU path);
-:class:`relora_b200.engine.fused_llama.FusedLlamaStepper` is the B200 executor (whole-layer fused
+:class:`relora_b200.engine.fused_llama.FusedLlamaStepper` is the H100 executor (whole-layer fused
 kernels, CUDA graphs) with the same interface.
 """
 from __future__ import annotations
@@ -201,7 +201,7 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
             raise RuntimeError(f"--engine fused requested but not applicable: {why}")
     if info.device.type != "cuda":
         kw["transport"] = "nccl"  # CPU: the process group's own reduction (gloo)
-    # the fp8 tensor-core path and the tcgen05 attention kernels belong to the fused executor: say so instead of silently
+    # the fp8 tensor-core path and the wgmma attention kernels belong to the fused executor: say so instead of silently
     # training in bf16 / with SDPA
     from ..obs import logger
 

@@ -15,7 +15,7 @@ Two execution paths share these parameters:
 * the module-by-module path below (PyTorch expressions; on CUDA/bf16 the leaf modules dispatch to
   the native kernels through :mod:`relora_b200.ops.dispatch`);
 * the whole-layer fused executor in :mod:`relora_b200.engine.fused_llama`, which the trainer uses on
-  B200 (stacked QKV / gate-up weights, LoRA folded into the GEMM, CUDA-graph captured).
+  H100 (stacked QKV / gate-up weights, LoRA folded into the GEMM, CUDA-graph captured).
 """
 from __future__ import annotations
 
@@ -188,7 +188,7 @@ class LlamaAttention(nn.Module):
             mask = torch.ones(T, kv_len, dtype=torch.bool, device=q.device).tril(diagonal=kv_len - T)
             out = F.scaled_dot_product_attention(q, k, v, attn_mask=mask)
         elif causal and past_key_value is None and _use_native_attention(q, self.head_dim):
-            # this repo's tcgen05 flash-attention kernels (csrc/attention.cu) instead of the library SDPA call
+            # this repo's wgmma flash-attention kernels (csrc/attention.cu) instead of the library SDPA call
             from ..ops import fused
 
             out = fused.causal_attention(q, k, v)
@@ -199,7 +199,7 @@ class LlamaAttention(nn.Module):
 
 
 def _use_native_attention(q: torch.Tensor, head_dim: int) -> bool:
-    """CUDA + bf16 + head_dim <= 64 (multiple of 8): the tcgen05 kernels; RELORA_B200_ATTENTION=sdpa forces the library call."""
+    """CUDA + bf16 + head_dim <= 64 (multiple of 8): the wgmma kernels; RELORA_B200_ATTENTION=sdpa forces the library call."""
     if not q.is_cuda or os.environ.get("RELORA_B200_ATTENTION", "auto") == "sdpa":
         return False
     from ..ops import dispatch, fused

@@ -188,7 +188,7 @@ class GPTNeoXAttention(nn.Module):
 
     def _forward_native(self, qkv, B, T):
         """CUDA / bf16 training path: partial rotary in place on the fused projection output (csrc/neox.cu), then causal attention
-        on the tcgen05 kernels when the head size allows (<= 64), torch SDPA otherwise.  Positions are 0..T-1 (no cache)."""
+        on the wgmma kernels when the head size allows (<= 64), torch SDPA otherwise.  Positions are 0..T-1 (no cache)."""
         from ..ops import fused
 
         nh, hd, rd = self.num_attention_heads, self.head_size, self.rotary_ndims

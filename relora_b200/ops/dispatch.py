@@ -1,4 +1,4 @@
-"""Run-time selection between the PyTorch reference ops and the native sm_100a kernels.
+"""Run-time selection between the PyTorch reference ops and the native sm_90a kernels.
 
 Policy: tensors on a CUDA device in bf16 take the native path.  If the process is on a CUDA box and
 the extension cannot be loaded this raises instead of silently falling back (a silent eager fallback

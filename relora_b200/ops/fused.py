@@ -1,4 +1,4 @@
-"""Python face of the native sm_100a kernels: thin wrappers + autograd functions.
+"""Python face of the native sm_90a kernels: thin wrappers + autograd functions.
 
 Everything here requires the in-tree extension (``relora_b200/_C.so``); :mod:`.dispatch` decides
 when these are used.  Numerics oracles live in :mod:`.reference`.
@@ -89,9 +89,9 @@ def gemm(
     fp8: int = 0,
     alpha_dev: Optional[torch.Tensor] = None,
 ) -> torch.Tensor:
-    """``out[M,N] = alpha·(a1·b1ᵀ + a2·b2ᵀ) (+ residual) (+ out)`` on the tcgen05 kernel.
+    """``out[M,N] = alpha·(a1·b1ᵀ + a2·b2ᵀ) (+ residual) (+ out)`` on the wgmma kernel.
 
-    ``pair``: -1 auto, 0 single-CTA tiles, 1 CTA pairs (``tcgen05 cta_group::2``, 256x256 tiles; needs ``block_n`` 256).
+    ``pair``: accepted and ignored (sm_90 has no CTA-pair MMA; tiles are always single-CTA).
     ``fp8``: 1 = ``a1`` / ``b1`` hold E4M3 bytes (K-major), 2 = ``a1`` is E5M2 (gradients); ``alpha_dev``: fp32 device scalar multiplied into ``alpha``.
 
     K-major operands are ``[rows, K]`` row-major; with ``a1_mn`` / ``b1_mn`` the tensor is
@@ -345,12 +345,12 @@ def relora_linear_module(module, x: torch.Tensor) -> torch.Tensor:
 
 # ----------------------------------------------------------------------------- causal attention (module path)
 def native_attention_supported(q: torch.Tensor, head_dim: int) -> bool:
-    """The tcgen05 attention kernels (csrc/attention.cu): CUDA bf16, head_dim a multiple of 8 and <= 64."""
+    """The wgmma attention kernels (csrc/attention.cu): CUDA bf16, head_dim a multiple of 8 and <= 64."""
     return q.is_cuda and q.dtype == _BF16 and head_dim % 8 == 0 and head_dim <= 64
 
 
 class _CausalAttentionFn(torch.autograd.Function):
-    """Causal self-attention on the tcgen05 kernels for ``q, k, v [B, nh, T, hd]`` (RoPE already applied).
+    """Causal self-attention on the wgmma kernels for ``q, k, v [B, nh, T, hd]`` (RoPE already applied).
 
     The kernels read a packed ``[B*T, 3*nh*hd]`` projection buffer in place (that is what the fused executor hands them);
     the module path packs its three projection outputs once.  Replaces ``F.scaled_dot_product_attention(is_causal=True)``
@@ -384,10 +384,7 @@ class _CausalAttentionFn(torch.autograd.Function):
             do = do.contiguous()
         dqkv = torch.empty_like(qkv)
         delta = torch.empty(B, nh, T, dtype=torch.float32, device=qkv.device)
-        ds_ws = None
-        if os.environ.get("RELORA_B200_ATTN_DS", "1") != "0":
-            ds_ws = torch.empty(C.attention_ds_workspace_elems(B, T, nh), dtype=_BF16, device=qkv.device)
-        C.attention_bwd(qkv, out, do, lse, delta, dqkv, B, T, nh, hd, scale, ds_ws)
+        C.attention_bwd(qkv, out, do, lse, delta, dqkv, B, T, nh, hd, scale)
         d5 = dqkv.view(B, T, 3, nh, hd)
         return d5[:, :, 0].transpose(1, 2), d5[:, :, 1].transpose(1, 2), d5[:, :, 2].transpose(1, 2), None
 
@@ -449,7 +446,7 @@ def lm_head_cross_entropy(h: torch.Tensor, w_head: torch.Tensor, labels: torch.T
 # ----------------------------------------------------------------------------- merge / re-init
 @torch.no_grad()
 def merge_and_reinit_modules(modules: Sequence, *, seed: int, restart_index: int) -> bool:
-    """``W += s·B@A`` (tcgen05 GEMM accumulating into W in fp32, one rounding) + hash-based kaiming
+    """``W += s·B@A`` (wgmma GEMM accumulating into W in fp32, one rounding) + hash-based kaiming
     re-init of A + zeroing of B, for a list of :class:`ReLoRaLinear`.  Reference: relora.py:269-307."""
     C = _C()
     for m in modules:

@@ -5,7 +5,7 @@
   UE8M0 scale per 32 x 32 tile, expanded into the two scale-factor arrays the tensor core reads (forward: reduction over ``K``;
   input gradient: reduction over ``N``, same bytes read MN-major).  1.06 bytes per parameter instead of 2.
 * :func:`linear` — autograd function ``y = x · Wᵀ (+ bias)``: activations are quantised per (row, 32 columns) on the fly, both GEMMs run
-  ``tcgen05.mma.kind::mxf8f6f4.block_scale`` with the scale factors staged to tensor memory by ``tcgen05.cp``.
+  e4m3 ``wgmma`` per 32-element block with the scale factors applied to the fp32 partial products.
 * :func:`merge_` — the ReLoRA merge on packed storage: dequantise → fp32 add → requantise with fresh tile scales, in place
   (reference ``relora.py:277-299``).
 
@@ -38,7 +38,7 @@ def supported(n: int, k: int) -> bool:
 @dataclass
 class MxWeight:
     q: torch.Tensor        # uint8 [Npad, Kpad] E4M3 bytes (zero padding)
-    sf_fwd: torch.Tensor   # uint8, scale of (row n, 32-block of k) in the tcgen05 layout
+    sf_fwd: torch.Tensor   # uint8, scale of (row n, 32-block of k) in the blocked layout of csrc/gemm_mx.cu
     sf_bwd: torch.Tensor   # uint8, scale of (row k, 32-block of n)
     N: int
     K: int

@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a extension ``relora_b200/_C.so`` (built by ``__graft_entry__.build``
+"""Loader for the in-tree sm_90a extension ``relora_b200/_C.so`` (built by ``__graft_entry__.build``
 or ``python -m relora_b200.csrc.build``).  The shared object is kept in the source tree so it travels
 with the repository snapshot to the GPU box; nothing is JIT-compiled at import time.
 """
@@ -45,7 +45,7 @@ def require():
     _try_load()
     if _mod is None:
         raise RuntimeError(
-            "relora_b200._C (sm_100a kernels) could not be loaded on a CUDA device: "
+            "relora_b200._C (sm_90a kernels) could not be loaded on a CUDA device: "
             f"{_err!r}. Build it with `python -c 'import __graft_entry__ as g; g.build()'`."
         )
     return _mod

@@ -8,7 +8,7 @@ block-scaled formats instead, so this engine stores the frozen weight as
 * ``nvfp4``  — NVFP4: e2m1 elements, one e4m3 scale per 16 elements of K and one fp32 tensor scale.
 
 ``4bit`` and ``8bit`` are accepted as aliases (``4bit -> nvfp4``, ``8bit -> mxfp8``).  Layout: data
-is row-major ``[N, K]`` (K contiguous, the K-major operand layout ``tcgen05.mma`` wants), scales are
+is row-major ``[N, K]`` (K contiguous, the K-major operand layout fp8 ``wgmma`` wants), scales are
 ``[N, K/block]``.  The functions here are the numerics oracle for the CUDA kernels and the CPU path.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """Plain PyTorch definitions of every fused operator (the numerics oracle + the CPU path).
 
-Each function states the exact math the sm_100a kernel of the same name implements; GPU tests
+Each function states the exact math the sm_90a kernel of the same name implements; GPU tests
 compare kernel output against these evaluated in fp32.  Reference sites are cited per op.
 """
 from __future__ import annotations

@@ -9,7 +9,7 @@ Transports:
 
 * ``nccl``  — one ``all_reduce`` (or ``reduce_scatter`` + ``all_gather`` for ZeRO-1) on the flat
   buffer: the baseline path implemented here, also used with gloo on CPU;
-* ``p2p``   — :class:`relora_b200.parallel.symm.SymmComm.fused_update`: hand-written sm_100a kernels over NVLink
+* ``p2p``   — :class:`relora_b200.parallel.symm.SymmComm.fused_update`: hand-written sm_90a kernels over NVLink
   peer memory / NVLS multicast (reduce-scatter + Σg² + AdamW + parameter broadcast in one chain).  The steppers
   call it directly and bypass :meth:`GradSync.reduce`; ``transport`` is then only a label.
 

@@ -79,9 +79,8 @@ class SymmComm:
         self.device = torch.device("cuda", torch.cuda.current_device())
         self.C = native.require()
         if use_multicast is None:
-            # NVLS (multimem.ld_reduce / multimem.st through the switch) wins at 8 ranks (fused update 697 vs 800 us); at 4 the two are
-            # level (708 vs 707 us, all-reduce 519 vs 573 GB/s at 64 MB) and between two GPUs plain peer loads / stores are clearly faster
-            # (550 vs 738 us, 522 vs 330 GB/s): profiles/multigpu/allreduce_n{2,4,8}_round2.json
+            # NVLS (multimem.ld_reduce / multimem.st through the switch) above 4 ranks, plain peer loads / stores below; this crossover
+            # has not been measured on H100 boxes (bench/allreduce_bench.py measures both)
             env = os.environ.get("RELORA_B200_MULTICAST")
             use_multicast = (env == "1") if env is not None else self.world > 4
         self.use_multicast = use_multicast

@@ -11,7 +11,7 @@ reference's (``weight``, ``bias``, ``lora_A.weight`` [r, in], ``lora_B.weight`` 
 * the merge accumulates ``W += s·B@A`` in fp32 before rounding back to the storage dtype;
 * re-initialisation of ``A`` draws from a counter-based generator keyed by
   ``(seed, restart_index, module_index)`` so all data-parallel ranks agree by construction;
-* on CUDA the forward/backward dispatches to the fused sm_100a kernels in :mod:`relora_b200.ops`
+* on CUDA the forward/backward dispatches to the fused sm_90a kernels in :mod:`relora_b200.ops`
   (one pass over ``x`` for frozen + low-rank branch); the PyTorch expression below is the
   reference implementation used on CPU and for numerics tests.
 """
@@ -138,7 +138,7 @@ class ReLoRaLinear(nn.Module):
 
     def _pack(self, value: torch.Tensor):
         """Packed form of ``value``: on CUDA, ``mxfp8`` uses the tensor-core layout of csrc/gemm_mx.cu (E4M3 + one UE8M0 scale per
-        32 x 32 tile, read by ``tcgen05.mma.kind::mxf8f6f4.block_scale`` in forward and input gradient); everything else (CPU, nvfp4) the
+        32 x 32 tile, read by the e4m3 wgmma MX GEMM in forward and input gradient); everything else (CPU, nvfp4) the
         reference layout of ops/quant.py."""
         if self.quantize == "mxfp8" and value.is_cuda:
             from ..ops import mx, native

@@ -8,7 +8,7 @@ pruning primitives) and ``:267-364`` (``optimizer_reset``).  Three mutually excl
 * ``optimizer_random_pruning=p`` — keep each element with probability ``1-p``;
 * ``optimizer_magnitude_pruning=p`` — keep ``|x| > quantile(|x|, p)`` (strict inequality).
 
-Differences by design (documented in DESIGN.md):
+Differences by design:
 
 * the random mask is drawn from an explicit counter-based generator keyed by
   ``(seed, reset_index, tensor_index)`` so every data-parallel rank prunes identically without

@@ -6,7 +6,7 @@ from setuptools import find_packages, setup
 setup(
     name="relora_b200",
     version="0.1.0",
-    description="Blackwell-native (sm_100a) ReLoRA pre-training engine",
+    description="Hopper-native (sm_90a) ReLoRA pre-training engine",
     packages=find_packages(include=["relora_b200", "relora_b200.*", "tools"]),
     package_data={"relora_b200": ["_C.so", "_data_helpers.so", "csrc/*.cu", "csrc/*.cuh", "csrc/*.h", "csrc/*.cpp"]},
     python_requires=">=3.10",

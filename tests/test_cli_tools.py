@@ -8,6 +8,18 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CFG = os.path.join(ROOT, "configs", "llama_9m.json")
 
 
+@pytest.fixture(autouse=True)
+def private_hf_cache(tmp_path, monkeypatch):
+    """Keep the datasets / transformers caches of these runs in the test's own directory: the user's HF_HOME may not be
+    writable (or may belong to someone else)."""
+    import datasets
+
+    cache = str(tmp_path / "hf_cache")
+    monkeypatch.setenv("HF_HOME", cache)
+    monkeypatch.setenv("HF_DATASETS_CACHE", os.path.join(cache, "datasets"))
+    monkeypatch.setattr(datasets.config, "HF_DATASETS_CACHE", os.path.join(cache, "datasets"))
+
+
 @pytest.fixture(scope="module")
 def tiny_tokenizer(tmp_path_factory):
     from tokenizers import Tokenizer, models, pre_tokenizers

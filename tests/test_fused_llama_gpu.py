@@ -1,4 +1,4 @@
-"""Fused whole-model executor vs the module-by-module path on identical weights / dropout masks (B200: -m gpu)."""
+"""Fused whole-model executor vs the module-by-module path on identical weights / dropout masks (H100: -m gpu)."""
 import copy
 import os
 
@@ -104,7 +104,7 @@ def test_fused_merge_and_checkpoint_roundtrip(tmp_path, inter):
 
 
 def test_native_attention_matches_sdpa_in_the_executor():
-    """The tcgen05 attention kernels and torch SDPA (cuDNN) give the same loss and gradients inside the fused executor."""
+    """The wgmma attention kernels and torch SDPA (cuDNN) give the same loss and gradients inside the fused executor."""
     from relora_b200.engine.fused_llama import FusedLlamaStepper
     from relora_b200.ops import fused
 
@@ -167,8 +167,8 @@ def test_fp8_frozen_path_tracks_bf16_executor(backward, monkeypatch):
 
 @pytest.mark.parametrize("extra", [[], ["--frozen_dtype", "fp8", "--attention", "native"]])
 def test_cli_end_to_end_on_the_fused_executor(tmp_path, extra):
-    """torchrun_main on the B200 executor: ReLoRA resets, magnitude pruning, checkpoint layout, autoresume; also with the fp8
-    frozen-weight path and the tcgen05 attention kernels selected from the command line."""
+    """torchrun_main on the H100 executor: ReLoRA resets, magnitude pruning, checkpoint layout, autoresume; also with the fp8
+    frozen-weight path and the wgmma attention kernels selected from the command line."""
     import json
     import os
 

@@ -1,4 +1,4 @@
-"""Numerics of the sm_100a kernels against plain PyTorch fp32 references (run on the B200: -m gpu)."""
+"""Numerics of the sm_90a kernels against plain PyTorch fp32 references (run on an H100: -m gpu)."""
 import math
 
 import pytest
@@ -106,7 +106,7 @@ def test_gemm_ragged_groups_and_tma_residual(F, block_n):
     (384, 256, 192, True, False), (12288, 2304, 768, False, False),
 ])
 def test_gemm_cta_pair(F, M, N, K, a_mn, b_mn):
-    """tcgen05 cta_group::2: one M=256 instruction per CTA pair, each CTA stages half of the B tile."""
+    """The CTA-pair request of the Blackwell build is accepted on sm_90 (no cta_group::2 MMA there) and computes the same product."""
     torch.manual_seed(M + N)
     a = _rand(K, M) if a_mn else _rand(M, K)
     b = _rand(K, N, scale=0.05) if b_mn else _rand(N, K, scale=0.05)
@@ -172,7 +172,7 @@ def test_gemm_split_k_weight_grad(F, split):
 
 def test_gemm_many_tiles_persistent(F):
     torch.manual_seed(6)
-    M, N, K = 4096, 2304, 768  # 576 tiles of 128x128 > 148 SMs: exercises the ring phases
+    M, N, K = 4096, 2304, 768  # 576 tiles of 128x128 > 132 SMs: exercises the ring phases
     a, b = _rand(M, K), _rand(N, K, scale=0.03)
     out = F.gemm(a, b, block_n=128)
     assert _relerr(out, a.float() @ b.float().t()) < 6e-3
@@ -183,7 +183,7 @@ def test_gemm_many_tiles_persistent(F):
 @pytest.mark.parametrize("G,Ng,K,M,p", [(1, 256, 256, 300, 0.1), (2, 384, 256, 512, 0.1), (3, 256, 384, 1000, 0.1), (3, 128, 128, 128, 0.0),
                                         (1, 256, 640, 20000, 0.25), (2, 5504, 2048, 256, 0.1)])
 def test_lora_dx_fused_dropout_epilogue(C, G, Ng, K, M, p):
-    """dx = dy·W + Σ_g keep_g ⊙ (du_g·A_g)/(1-p): 1+G tensor-memory accumulators, masks evaluated in the epilogue."""
+    """dx = dy·W + Σ_g keep_g ⊙ (du_g·A_g)/(1-p): masked LoRA terms folded into the register accumulator."""
     from relora_b200.ops import reference as ref
 
     r = 128
@@ -553,7 +553,7 @@ def test_llama_module_path_on_gpu_matches_cpu_reference():
 # ----------------------------------------------------------------------------------------- attention
 @pytest.mark.parametrize("B,T,nh,hd", [(2, 512, 4, 48), (1, 320, 2, 64), (3, 128, 2, 32), (1, 1000, 3, 64), (2, 64, 1, 16)])
 def test_attention_fwd_bwd(C, B, T, nh, hd):
-    """tcgen05 causal flash attention over the packed qkv buffer vs an fp32 PyTorch reference (forward, lse and dq/dk/dv)."""
+    """wgmma causal flash attention over the packed qkv buffer vs an fp32 PyTorch reference (forward, lse and dq/dk/dv)."""
     torch.manual_seed(T + hd)
     h = nh * hd
     qkv = _rand(B * T, 3 * h)
@@ -588,8 +588,8 @@ def test_attention_fwd_bwd(C, B, T, nh, hd):
 # ----------------------------------------------------------------------------------------- fp8 frozen-weight path
 @pytest.mark.parametrize("M,N,K,pair", [(256, 256, 256, 0), (1000, 768, 640, 0), (512, 1024, 2048, 1), (12288, 2304, 768, 0)])
 def test_gemm_fp8_frozen_path_with_bf16_lora_branch(C, F, M, N, K, pair):
-    """x·Wᵀ on the E4M3 tensor-core path (tcgen05 kind::f8f6f4, per-tensor scales) with the bf16 LoRA branch accumulated into
-    the same tensor-memory accumulator; checked against an fp32 product of the *dequantised* operands."""
+    """x·Wᵀ on the E4M3 tensor-core path (e4m3 wgmma, per-tensor scales) with the bf16 LoRA branch accumulated into
+    the same register accumulator; checked against an fp32 product of the *dequantised* operands."""
     torch.manual_seed(K + N)
     r = 128
     x, W = _rand(M, K), _rand(N, K, scale=0.05)
@@ -743,7 +743,7 @@ def test_pythia_native_leaf_ops_match_eager():
     assert worst < 0.08, worst
 
 
-def test_module_path_attention_uses_the_tcgen05_kernels(F):
+def test_module_path_attention_uses_the_wgmma_kernels(F):
     """`F.causal_attention` (module path) vs torch SDPA on q, k, v [B, nh, T, hd] incl. the gradients."""
     torch.manual_seed(0)
     B, nh, T, hd = 2, 4, 200, 48
@@ -785,7 +785,7 @@ def test_mx_quantisers_match_the_oracle(C):
 
 @pytest.mark.parametrize("M,N,K", [(128, 128, 128), (384, 256, 512), (300, 264, 328), (1024, 768, 768)])
 def test_mx_gemm_forward_and_input_gradient(C, M, N, K):
-    """tcgen05.mma.kind::mxf8f6f4.block_scale with tcgen05.cp-staged scale factors vs the fp32 product of the dequantised operands."""
+    """e4m3 wgmma per 32-element scale block vs the fp32 product of the dequantised operands."""
     from relora_b200.ops import mx
 
     torch.manual_seed(1)

@@ -10,22 +10,64 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CFG = os.path.join(ROOT, "configs", "llama_9m.json")
 
 
-def test_llama_matches_reference_logits_and_grads(reference_modules):
-    from transformers import AutoConfig
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_models.json")
 
+
+def _golden():
+    import json
+
+    return json.load(open(GOLDEN))
+
+
+def sample(t, k, seed=0):
+    """A fixed seeded sample of ``k`` entries of ``t`` (the same indices for the same numel)."""
+    flat = t.detach().reshape(-1)
+    idx = torch.randint(0, flat.numel(), (k,), generator=torch.Generator().manual_seed(seed))
+    return flat[idx].double()
+
+
+def llama9m_case():
+    """Seeded llama_9m and batch: the reference side of the comparison was recorded from these weights (oracle/reference_goldens.py)."""
     torch.manual_seed(0)
-    ref = reference_modules.llama.LlamaForCausalLM(AutoConfig.from_pretrained("/root/reference/configs/llama_9m.json"))
     ours = LlamaForCausalLM(load_config(CFG))
-    ours.load_state_dict(ref.state_dict(), strict=True)  # identical key set incl. rotary inv_freq buffers
-    assert set(ours.state_dict()) == set(ref.state_dict())
     ids = torch.randint(0, 32000, (2, 33))
-    a = ref(input_ids=ids, labels=ids)
+    return ours, ids
+
+
+def padding_row_case():
+    torch.manual_seed(0)
+    cfg = load_config(os.path.join(ROOT, "configs", "llama_35m.json"))
+    cfg.num_hidden_layers = 12
+    model = LlamaForCausalLM(cfg)
+    ids = {}
+    for first in (5, cfg.vocab_size - 1):
+        x = torch.randint(0, cfg.vocab_size - 1, (2, 48))
+        x[0, 0] = first
+        ids[first] = x
+    return model, ids
+
+
+def padding_row_grad_norms(model, ids, embed):
+    norms = {}
+    for first, x in ids.items():
+        emb = embed(x).detach().requires_grad_()
+        model(inputs_embeds=emb, labels=x).loss.backward()
+        norms[first] = float(emb.grad[0, 0].norm())
+    return norms
+
+
+def test_llama_matches_reference_logits_and_grads():
+    g = _golden()["llama_9m"]
+    ours, ids = llama9m_case()
+    # identical key set (incl. rotary inv_freq buffers) and shapes: the upstream state dict loads strictly
+    assert {k: list(v.shape) for k, v in ours.state_dict().items()} == g["state_dict_shapes"]
     b = ours(input_ids=ids, labels=ids)
-    assert torch.allclose(a.logits, b.logits, atol=1e-5)
-    assert abs(float(a.loss) - float(b.loss)) < 1e-6
-    a.loss.backward(); b.loss.backward()
-    for (n, p), (_, q) in zip(ref.named_parameters(), ours.named_parameters()):
-        assert torch.allclose(p.grad, q.grad, atol=1e-5), n
+    assert torch.allclose(sample(b.logits, 512), torch.tensor(g["logits_sample"], dtype=torch.float64), atol=1e-5)
+    assert abs(float(b.loss) - g["loss"]) < 1e-6
+    b.loss.backward()
+    for n, q in ours.named_parameters():
+        assert torch.allclose(sample(q.grad, 16), torch.tensor(g["grad_samples"][n], dtype=torch.float64), atol=1e-5), n
+        assert abs(float(q.grad.double().norm()) - g["grad_norms"][n]) <= 1e-4 * max(1.0, g["grad_norms"][n]), n
     # chunked LM-head loss == materialised-logits loss
     c = ours(input_ids=ids, labels=ids, return_logits=False)
     assert c.logits is None and abs(float(c.loss) - float(b.loss)) < 1e-5
@@ -132,30 +174,23 @@ def test_rope_scaling_variants():
     assert not torch.equal(inv_before, dyn.inv_freq) and dyn.cos_cached.shape[2] == 64
 
 
-def test_sequence_starting_with_the_padding_row_overflows_the_reference_gradient(reference_modules):
+def test_sequence_starting_with_the_padding_row_overflows_the_reference_gradient():
     """Root cause of round 1's non-finite 4-/8-GPU benchmark runs (both arms).  The configs' ``pad_token_id = -1`` makes row V-1
     the embedding's zero padding row; a sequence that *starts* with it keeps an exactly-zero residual row through every layer
     (v = 0, no biases), and RMSNorm's backward at x = 0 multiplies the gradient by 1/sqrt(eps) = 1000 per norm: it overflows
-    fp32 within ~12 layers of the *unmodified reference model*.  Synthetic token generators therefore never emit that id
+    fp32 within ~12 layers of the *unmodified reference model* (its gradient norms on these weights are stored in
+    tests/golden/reference_models.json) and of this model alike.  Synthetic token generators therefore never emit that id
     (real tokenised text does not contain it either)."""
-    from transformers import AutoConfig
-
     from relora_b200.data.synthetic import SyntheticTokens
 
-    hf_cfg = AutoConfig.from_pretrained("/root/reference/configs/llama_35m.json")
-    hf_cfg.num_hidden_layers = 12
-    V = hf_cfg.vocab_size
-    torch.manual_seed(0)
-    model = reference_modules.llama.LlamaForCausalLM(hf_cfg)
-    norms = {}
-    for first in (5, V - 1):
-        ids = torch.randint(0, V - 1, (2, 48))
-        ids[0, 0] = first
-        emb = model.model.embed_tokens(ids).detach().requires_grad_()
-        model(inputs_embeds=emb, labels=ids).loss.backward()
-        norms[first] = float(emb.grad[0, 0].norm())
-    assert norms[5] < 1e3                       # ordinary token: ordinary gradient
-    assert not (norms[V - 1] < 1e30)            # padding row first: overflow (inf / nan)
+    g = _golden()["padding_row"]
+    model, ids = padding_row_case()
+    V = model.config.vocab_size
+    norms = padding_row_grad_norms(model, ids, model.model.embed_tokens)
+    ref = {int(k): v for k, v in g["reference_grad_norms"].items()}
+    assert ref[5] < 1e3 and norms[5] < 1e3                       # ordinary token: ordinary gradient ...
+    assert abs(norms[5] - ref[5]) <= 1e-3 * ref[5]               # ... and the same one as the reference's
+    assert not (ref[V - 1] < 1e30) and not (norms[V - 1] < 1e30)  # padding row first: overflow (inf / nan) on both
     # ... which is why the synthetic sources draw from [0, V - 1)
     ds = SyntheticTokens(64, 128, V, seed=3)
     assert max(int(ds[i]["input_ids"].max()) for i in range(64)) < V - 1

@@ -1,4 +1,4 @@
-"""``tools/roofline_md.py`` renders the committed site-profile / all-reduce JSON into the tables of ``profiles/ROOFLINE.md``."""
+"""``tools/roofline_md.py`` renders the committed site-profile / all-reduce JSON into the tables of a ROOFLINE.md."""
 import json
 import os
 
@@ -27,17 +27,3 @@ def test_roofline_md_renders_sites_and_collectives(tmp_path):
     assert "reduce_kernel<512>` 0.09 ms" in text and "Memset" not in text           # only library kernels above 0.05 ms are listed
     assert "| 8 | 65536 | 427 (275 µs) | 576 (204 µs) | 584 (201 µs) | 0.76 |" in text
     assert "| llama_250m (98.9 M) | 8 | nvls | 697 | 496 | 449 | 0.64 |" in text
-
-
-def test_committed_roofline_matches_the_committed_json():
-    """profiles/ROOFLINE.md is what the tool produces from the JSON files next to it (no hand edits)."""
-    prof = os.path.join(ROOT, "profiles")
-    need = [os.path.join(prof, f) for f in ("site_profile_250m_round2.json", "site_profile_1b_round2.json", "ROOFLINE.md")]
-    if not all(os.path.exists(p) for p in need):
-        import pytest
-        pytest.skip("profiles not present")
-    d = json.load(open(need[0]))
-    text = open(need[2]).read()
-    top = d["sites"][0]
-    assert f"| `{top['site']}` | {top['calls']} | {top['us'] / 1e3:.3f} |" in text
-    assert f"{d['ours_ms']:.2f} ms in this repo's kernels" in text

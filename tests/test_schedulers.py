@@ -1,5 +1,7 @@
 """Golden values captured from the reference schedulers (SURVEY.md Appendix A)."""
+import json
 import math
+import os
 
 import pytest
 import torch
@@ -72,17 +74,28 @@ def test_validation_errors():
         build_multiplier("nope", num_training_steps=100, warmup_steps=10)
 
 
-def test_matches_reference_everywhere(reference_modules):
-    tu = reference_modules.training_utils
-    for adjust in (0, 5):
-        mine = build_multiplier("cosine_restarts", num_training_steps=200, warmup_steps=20, min_lr_ratio=0.05,
-                                cycle_length=50, restart_warmup_steps=7, adjust_step=adjust)
-        for s in range(200):
-            ref = tu._get_cosine_schedule_with_multiple_warmups_lambda(
-                s, num_training_steps=200, first_warmup_steps=20, restart_warmup_steps=7, restart_every=50,
-                min_lr_ratio=0.05, adjust_step=adjust)
-            assert math.isclose(mine(s), ref, rel_tol=1e-12, abs_tol=1e-12), (s, adjust)
-    mine = build_multiplier("cosine", num_training_steps=200, warmup_steps=10, min_lr_ratio=0.1, cycle_length=40)
-    for s in range(200):
-        ref = tu._get_cyclical_cosine_schedule_with_min_lr_lambda(s, num_warmup_steps=10, cycle_length=40, min_lr_ratio=0.1)
-        assert math.isclose(mine(s), ref, rel_tol=1e-12, abs_tol=1e-12)
+GOLDEN = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "reference_schedulers.json")
+# (name, build_multiplier kwargs, upstream lambda, its kwargs): every step 0..199 recorded by oracle/reference_goldens.py
+REFERENCE_CASES = [
+    ("cosine_restarts_adjust0", dict(scheduler_type="cosine_restarts", num_training_steps=200, warmup_steps=20, min_lr_ratio=0.05,
+                                     cycle_length=50, restart_warmup_steps=7, adjust_step=0),
+     "_get_cosine_schedule_with_multiple_warmups_lambda", dict(num_training_steps=200, first_warmup_steps=20, restart_warmup_steps=7,
+                                                               restart_every=50, min_lr_ratio=0.05, adjust_step=0)),
+    ("cosine_restarts_adjust5", dict(scheduler_type="cosine_restarts", num_training_steps=200, warmup_steps=20, min_lr_ratio=0.05,
+                                     cycle_length=50, restart_warmup_steps=7, adjust_step=5),
+     "_get_cosine_schedule_with_multiple_warmups_lambda", dict(num_training_steps=200, first_warmup_steps=20, restart_warmup_steps=7,
+                                                               restart_every=50, min_lr_ratio=0.05, adjust_step=5)),
+    ("cosine", dict(scheduler_type="cosine", num_training_steps=200, warmup_steps=10, min_lr_ratio=0.1, cycle_length=40),
+     "_get_cyclical_cosine_schedule_with_min_lr_lambda", dict(num_warmup_steps=10, cycle_length=40, min_lr_ratio=0.1)),
+]
+
+
+def test_matches_reference_everywhere():
+    golden = json.load(open(GOLDEN))
+    for name, kw, _, _ in REFERENCE_CASES:
+        kw = dict(kw)
+        mine = build_multiplier(kw.pop("scheduler_type"), **kw)
+        ref = golden[name]
+        assert len(ref) == 200
+        for s, r in enumerate(ref):
+            assert math.isclose(mine(s), r, rel_tol=1e-12, abs_tol=1e-12), (name, s)
