@@ -142,7 +142,8 @@ def build_parser() -> argparse.ArgumentParser:
     _add_bool(p, "--deterministic", False,
               help="fixed summation order for the weight-gradient GEMMs (no split-K atomics; slower) on top of the always-deterministic embedding backward")
     p.add_argument("--attention", type=str, default="auto", choices=["auto", "native", "sdpa"],
-                   help="native: wgmma flash-attention kernels of this repo (head_dim <= 64); sdpa: torch SDPA (cuDNN)")
+                   help="native: wgmma flash-attention kernels of this repo (head_dim a multiple of 8, <= 256); sdpa: torch SDPA (cuDNN); "
+                        "auto: the kernels for head_dim <= 64, SDPA above")
     p.add_argument("--frozen_dtype", type=str, default=None, choices=[None, "bf16", "fp8", "fp8_full", "mxfp8", "nvfp4"],
                    help="fp8: E4M3 tensor-core path for the frozen weights on the fused executor (per-tensor scales, delayed "
                         "activation scaling), forward GEMMs only; fp8_full: also the input-gradient GEMMs (E5M2 gradients); mxfp8 / nvfp4: block-scaled storage on the module path (alias of --quantize)")

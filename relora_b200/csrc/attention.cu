@@ -2,23 +2,35 @@
 // of the packed qkv projection buffer.
 //
 // Replaces the reference's F.scaled_dot_product_attention call (peft_pretraining/modeling_llama.py:241-247 and
-// modeling_pythia.py attention) for head_dim <= 64.  Three kernels, one warpgroup (128 threads, 64 rows) per CTA:
+// modeling_pythia.py attention) for head_dim <= 256 (a multiple of 8).  Three kernels, one warpgroup (128 threads, 64 rows)
+// per CTA:
 //
 //   attn_fwd_kernel      CTA = (64 queries, head, batch); per 64 keys:  S = Q·Kᵀ -> online softmax -> O += P·V
 //   attn_bwd_dq_kernel   CTA = (64 queries, head, batch); per 64 keys:  S, dP = dO·Vᵀ -> dS -> dQ += dS·K
 //   attn_bwd_dkv_kernel  CTA = (64 keys, head, batch); per 64 queries:  Sᵀ = K·Qᵀ, dPᵀ = V·dOᵀ -> Pᵀ, dSᵀ -> dV += Pᵀ·dO, dK += dSᵀ·Q
 //
-// Shared-memory tiles are [64 rows x 64 columns] bf16 (128 bytes per row, 128-byte swizzle), so the same tile serves as a
-// K-major operand (reduction over head_dim) and as an MN-major operand (reduction over its rows) by descriptor alone.  The
-// probabilities / score gradients never leave registers: the accumulator fragment of one wgmma is, packed to bf16, the
-// register A operand of the next.  The streamed operand pair is double buffered.  Each consumer issues one k-block of wgmma
-// and waits for it before the dependent math; the overlap this forgoes has not been measured on the H100.
+// Each kernel is instantiated for NP = ceil(head_dim / 64) in {1, 2, 3, 4}.  An operand tile is NP shared-memory panels of
+// [64 rows x 64 columns] bf16 (128 bytes per row, 128-byte swizzle), loaded by NP TMA boxes at column offsets 64·p; columns
+// past head_dim are zero filled.  The same panel serves as a K-major operand (reduction over head_dim) and as an MN-major
+// operand (reduction over its rows) by descriptor alone.  Products that reduce over head_dim issue only the ceil(hd / 16)
+// K = 16 steps that hold data when the head spans several panels; products that produce head_dim columns run one
+// register-A wgmma chain per panel, and the padded columns of the last panel are computed but never stored.  The
+// probabilities / score gradients never leave registers: the accumulator fragment of one wgmma is, packed to bf16, the register A operand of the next.  The streamed
+// operand pair is double buffered.  Each consumer issues one k-block of wgmma and waits for it before the dependent math;
+// the overlap this forgoes has not been measured on the H100.
+//
+// Register budget.  The output accumulators take 32 fp32 registers per panel per thread, on top of the two 32-register
+// score fragments of the backward kernels.  Where the whole head does not fit one warpgroup without spilling (dQ at NP = 4,
+// dK/dV at NP >= 3), the backward kernels split the output columns across CTAs: each CTA owns at most two panels
+// (128 columns) of dQ, or of both dK and dV, and recomputes S / dP (Sᵀ / dPᵀ) over the full head for them.  Splitting by
+// columns rather than computing dK and dV in separate CTAs keeps one kernel body for every head size.
 #include <cuda.h>
 
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
 #include <stdexcept>
+#include <string>
 #include <unordered_map>
 
 #include "attention.h"
@@ -33,10 +45,17 @@ using namespace sm90;
 namespace {
 
 constexpr int BQ = 64;                // rows per CTA (queries in fwd / dq, keys in dkv)
-constexpr int kTile = 64 * 128;       // bytes of a [64 x 64] bf16 tile
+constexpr int kPanel = 64 * 128;      // bytes of a [64 x 64] bf16 panel
 constexpr int kThreads = 128;
-constexpr int kSmem = 6 * kTile + 1024 + 1024;  // two resident tiles, two double-buffered streamed tiles, barriers, alignment
+constexpr int kMaxHeadDim = 256;
 constexpr float kNegInf = -1e30f;
+
+// dynamic shared memory: NRES resident tiles, two double-buffered streamed tiles, barriers + row statistics, alignment
+constexpr int smem_bytes(int nres, int np) { return (nres + 4) * np * kPanel + 1024 + 1024; }
+// output panels per CTA of the backward kernels (see "Register budget" above)
+constexpr int dq_out_panels(int np) { return np <= 3 ? np : 2; }
+constexpr int dkv_out_panels(int np) { return np <= 2 ? np : 2; }
+constexpr int splits(int np, int no) { return (np + no - 1) / no; }
 
 __device__ __forceinline__ float fast_exp2(float x) {  // one MUFU.EX2 (inputs are <= ~8; -1e30 -> 0)
   float y;
@@ -51,18 +70,28 @@ __device__ __forceinline__ void frag_to_a(const float (&d)[32], int kk, uint32_t
   a[2] = pack_bf16x2(d[8 * kk + 4], d[8 * kk + 5]);
   a[3] = pack_bf16x2(d[8 * kk + 6], d[8 * kk + 7]);
 }
-// d += A · Bᵀ with A, B both [64 x 64] K-major tiles (reduction over head_dim)
-__device__ __forceinline__ void mma_tiles_kk(float (&d)[32], uint32_t a, uint32_t b) {
+// d += A · Bᵀ with A, B both [64 x 64·NP] K-major tiles (reduction over head_dim); only the first nks K = 16 steps hold data.
+// A single-panel head issues all four steps unconditionally (zero-filled columns add nothing), which keeps the head_dim <= 64
+// kernels free of the per-step branches.
+template <int NP>
+__device__ __forceinline__ void mma_tiles_kk(float (&d)[32], uint32_t a, uint32_t b, int nks) {
 #pragma unroll
-  for (int kk = 0; kk < 4; ++kk) wgmma_bf16_ss_n64<0, 0>(d, desc_kmajor(a + kk * 32), desc_kmajor(b + kk * 32));
+  for (int ks = 0; ks < 4 * NP; ++ks) {
+    const uint32_t ofs = (ks >> 2) * kPanel + (ks & 3) * 32;
+    if (NP == 1 || ks < nks) wgmma_bf16_ss_n64<0, 0>(d, desc_kmajor(a + ofs), desc_kmajor(b + ofs));
+  }
 }
-// d += P · T with P in registers (rows x 64) and T a [64 x 64] tile read MN-major (reduction over its rows)
-__device__ __forceinline__ void mma_regs_tile(float (&d)[32], const float (&p)[32], uint32_t t) {
+// d[j] += P · T_j for the first nout of NO consecutive panels T_j starting at t, read MN-major (reduction over their rows);
+// P in registers (rows x 64)
+template <int NO>
+__device__ __forceinline__ void mma_regs_tile(float (&d)[NO][32], const float (&p)[32], uint32_t t, int nout) {
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) {
     uint32_t a[4];
     frag_to_a(p, kk, a);
-    wgmma_bf16_rs_n64<1>(d, a, desc_mnmajor(t + kk * 2048));
+#pragma unroll
+    for (int j = 0; j < NO; ++j)
+      if (j < nout) wgmma_bf16_rs_n64<1>(d[j], a, desc_mnmajor(t + j * kPanel + kk * 2048));
   }
 }
 __device__ __forceinline__ void zero32(float (&d)[32]) {
@@ -78,17 +107,19 @@ struct Smem {
   float* col_lse;      // [64]: per-column row statistics of the streamed block (dK/dV kernel)
   float* col_delta;    // [64]
 };
+template <int NRES, int NP>
 __device__ __forceinline__ Smem smem_layout() {
+  constexpr int kTile = NP * kPanel;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   Smem m;
   m.res[0] = s;
-  m.res[1] = s + kTile;
+  m.res[1] = s + (NRES - 1) * kTile;
   for (int b = 0; b < 2; ++b)
-    for (int o = 0; o < 2; ++o) m.str[b][o] = s + (2 + 2 * b + o) * kTile;
-  m.res_bar = reinterpret_cast<uint64_t*>(s + 6 * kTile);
+    for (int o = 0; o < 2; ++o) m.str[b][o] = s + (NRES + 2 * b + o) * kTile;
+  m.res_bar = reinterpret_cast<uint64_t*>(s + (NRES + 4) * kTile);
   m.str_bar = m.res_bar + 1;
-  m.col_lse = reinterpret_cast<float*>(s + 6 * kTile + 64);
+  m.col_lse = reinterpret_cast<float*>(s + (NRES + 4) * kTile + 64);
   m.col_delta = m.col_lse + 64;
   return m;
 }
@@ -98,12 +129,18 @@ struct TileSrc {
   const CUtensorMap* map;
   int head;
 };
-__device__ __forceinline__ void issue_pair(const Smem& m, int buf, TileSrc s0, TileSrc s1, int row) {
-  mbar_arrive_expect_tx(&m.str_bar[buf], 2 * kTile);
-  tma_load_3d(s0.map, &m.str_bar[buf], m.str[buf][0], 0, s0.head, row);
-  tma_load_3d(s1.map, &m.str_bar[buf], m.str[buf][1], 0, s1.head, row);
+template <int NP>
+__device__ __forceinline__ void load_tile(TileSrc s, uint64_t* bar, uint8_t* dst, int row) {
+#pragma unroll
+  for (int pn = 0; pn < NP; ++pn) tma_load_3d(s.map, bar, dst + pn * kPanel, 64 * pn, s.head, row);
 }
-template <int NRES>
+template <int NP>
+__device__ __forceinline__ void issue_pair(const Smem& m, int buf, TileSrc s0, TileSrc s1, int row) {
+  mbar_arrive_expect_tx(&m.str_bar[buf], 2 * NP * kPanel);
+  load_tile<NP>(s0, &m.str_bar[buf], m.str[buf][0], row);
+  load_tile<NP>(s1, &m.str_bar[buf], m.str[buf][1], row);
+}
+template <int NRES, int NP>
 __device__ __forceinline__ void prologue(const Smem& m, TileSrc r0, TileSrc r1, int res_row, TileSrc s0, TileSrc s1, int row0, int nblk) {
   if (threadIdx.x == 0) {
     mbar_init(m.res_bar, 1);
@@ -115,10 +152,10 @@ __device__ __forceinline__ void prologue(const Smem& m, TileSrc r0, TileSrc r1, 
   pdl_wait();
   if (warp_id() == 0) {
     if (elect_one()) {
-      mbar_arrive_expect_tx(m.res_bar, NRES * kTile);
-      tma_load_3d(r0.map, m.res_bar, m.res[0], 0, r0.head, res_row);
-      if (NRES == 2) tma_load_3d(r1.map, m.res_bar, m.res[1], 0, r1.head, res_row);
-      for (int j = 0; j < 2 && j < nblk; ++j) issue_pair(m, j, s0, s1, row0 + j * BQ);
+      mbar_arrive_expect_tx(m.res_bar, NRES * NP * kPanel);
+      load_tile<NP>(r0, m.res_bar, m.res[0], res_row);
+      if (NRES == 2) load_tile<NP>(r1, m.res_bar, m.res[1], res_row);
+      for (int j = 0; j < 2 && j < nblk; ++j) issue_pair<NP>(m, j, s0, s1, row0 + j * BQ);
     }
     __syncwarp();
   }
@@ -134,6 +171,7 @@ struct FwdArgs {
 };
 
 // =============================================================================================== forward
+template <int NP>
 __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const FwdArgs p) {
   if (threadIdx.x == 0) pdl_launch_dependents();
   const int nqb = (p.T + BQ - 1) / BQ;
@@ -141,12 +179,14 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
   const int h = blockIdx.y, b = blockIdx.z;
   const int q0 = qb * BQ, rowbase = b * p.T;
   const int nkb = qb + 1;
-  const Smem m = smem_layout();
+  const int nks = (p.hd + 15) / 16;
+  const Smem m = smem_layout<1, NP>();
   // resident: Q; streamed: K, V
-  prologue<1>(m, {&map_qkv, h}, {&map_qkv, h}, rowbase + q0, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase, nkb);
+  prologue<1, NP>(m, {&map_qkv, h}, {&map_qkv, h}, rowbase + q0, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase, nkb);
   const uint32_t sq = smem_u32(m.res[0]);
-  float o[32], mrow[2] = {kNegInf, kNegInf}, lrow[2] = {0.f, 0.f};
-  zero32(o);
+  float o[NP][32], mrow[2] = {kNegInf, kNegInf}, lrow[2] = {0.f, 0.f};
+#pragma unroll
+  for (int pn = 0; pn < NP; ++pn) zero32(o[pn]);
   const int r_lo = q0 + frag_row(0);  // this thread's two query rows: r_lo and r_lo + 8
   for (int j = 0; j < nkb; ++j) {
     const int buf = j & 1;
@@ -154,7 +194,7 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
     float s[32];
     zero32(s);
     wgmma_fence();
-    mma_tiles_kk(s, sq, smem_u32(m.str[buf][0]));
+    mma_tiles_kk<NP>(s, sq, smem_u32(m.str[buf][0]), nks);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(s);
@@ -179,7 +219,8 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
       const int hr = (i >> 1) & 1;
       s[i] = fast_exp2(s[i] - mx[hr]);
       ls[hr] += s[i];
-      o[i] *= corr[hr];
+#pragma unroll
+      for (int pn = 0; pn < NP; ++pn) o[pn][i] *= corr[hr];
     }
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
@@ -187,13 +228,14 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
       mrow[hr] = mx[hr];
     }
     wgmma_fence();
-    mma_regs_tile(o, s, smem_u32(m.str[buf][1]));
+    mma_regs_tile<NP>(o, s, smem_u32(m.str[buf][1]), NP);
     wgmma_commit();
     wgmma_wait<0>();
-    fence_regs(o);
+#pragma unroll
+    for (int pn = 0; pn < NP; ++pn) fence_regs(o[pn]);
     __syncthreads();  // every warp is done with this buffer
     if (warp_id() == 0 && j + 2 < nkb) {
-      if (elect_one()) issue_pair(m, buf, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + (j + 2) * BQ);
+      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + (j + 2) * BQ);
       __syncwarp();
     }
   }
@@ -203,12 +245,16 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
     lrow[hr] += __shfl_xor_sync(0xffffffffu, lrow[hr], 2);
   }
 #pragma unroll
-  for (int i = 0; i < 32; i += 2) {
-    const int hr = (i >> 1) & 1;
-    const int q = r_lo + 8 * hr, c = frag_col(i);
-    if (q >= p.T || c >= p.hd) continue;
-    const float inv = 1.f / lrow[hr];
-    *reinterpret_cast<uint32_t*>(p.out + (long long)(rowbase + q) * p.ld_out + h * p.hd + c) = pack_bf16x2(o[i] * inv, o[i + 1] * inv);
+  for (int pn = 0; pn < NP; ++pn) {
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int hr = (i >> 1) & 1;
+      const int q = r_lo + 8 * hr, c = 64 * pn + frag_col(i);
+      if (q >= p.T || c >= p.hd) continue;
+      const float inv = 1.f / lrow[hr];
+      *reinterpret_cast<uint32_t*>(p.out + (long long)(rowbase + q) * p.ld_out + h * p.hd + c) =
+          pack_bf16x2(o[pn][i] * inv, o[pn][i + 1] * inv);
+    }
   }
   if ((threadIdx.x & 3) == 0) {
 #pragma unroll
@@ -261,18 +307,31 @@ __device__ __forceinline__ void store_rows(bf16* base, long long ld, int row0, i
     *reinterpret_cast<uint32_t*>(base + (long long)row0 * ld + (long long)r * ld + col_ofs + c) = pack_bf16x2(d[i] * sc, d[i + 1] * sc);
   }
 }
+// output panels j < nout of a CTA that owns head columns 64·pn0 ..: panel j lands at column 64·(pn0 + j) of the head at col_ofs
+template <int NO>
+__device__ __forceinline__ void store_panels(bf16* base, long long ld, int row0, int rows_valid, int col_ofs, int hd, int pn0, int nout,
+                                             const float (&d)[NO][32], float sc) {
+#pragma unroll
+  for (int j = 0; j < NO; ++j)
+    if (j < nout) store_rows(base, ld, row0, rows_valid, col_ofs + 64 * (pn0 + j), hd - 64 * (pn0 + j), d[j], sc);
+}
 
 // =============================================================================================== backward: dQ
+template <int NP>
 __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv,
                                                                const __grid_constant__ CUtensorMap map_do, const BwdArgs p) {
+  constexpr int NO = dq_out_panels(NP), NSPLIT = splits(NP, dq_out_panels(NP));
   if (threadIdx.x == 0) pdl_launch_dependents();
   const int nqb = (p.T + BQ - 1) / BQ;
-  const int qb = nqb - 1 - blockIdx.x;
+  const int qb = nqb - 1 - blockIdx.x / NSPLIT;
+  const int pn0 = (blockIdx.x % NSPLIT) * NO;  // first output panel of this CTA
+  const int nout = NP % NO == 0 ? NO : min(NO, NP - pn0);
   const int h = blockIdx.y, b = blockIdx.z;
   const int q0 = qb * BQ, rowbase = b * p.T;
   const int nkb = qb + 1;
-  const Smem m = smem_layout();
-  prologue<2>(m, {&map_qkv, h}, {&map_do, h}, rowbase + q0, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase, nkb);
+  const int nks = (p.hd + 15) / 16;
+  const Smem m = smem_layout<2, NP>();
+  prologue<2, NP>(m, {&map_qkv, h}, {&map_do, h}, rowbase + q0, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase, nkb);
   const long long bh = (long long)b * p.nh + h;
   const int r_lo = q0 + frag_row(0);
   float lse[2], dlt[2];
@@ -282,8 +341,9 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
     lse[hr] = p.lse[bh * p.T + q];
     dlt[hr] = p.delta[bh * p.T + q];
   }
-  float dq[32];
-  zero32(dq);
+  float dq[NO][32];
+#pragma unroll
+  for (int j = 0; j < NO; ++j) zero32(dq[j]);
   for (int j = 0; j < nkb; ++j) {
     const int buf = j & 1;
     mbar_wait(&m.str_bar[buf], (j >> 1) & 1);
@@ -291,8 +351,8 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
     zero32(s);
     zero32(dp);
     wgmma_fence();
-    mma_tiles_kk(s, smem_u32(m.res[0]), smem_u32(m.str[buf][0]));   // S = Q·Kᵀ
-    mma_tiles_kk(dp, smem_u32(m.res[1]), smem_u32(m.str[buf][1]));  // dP = dO·Vᵀ
+    mma_tiles_kk<NP>(s, smem_u32(m.res[0]), smem_u32(m.str[buf][0]), nks);   // S = Q·Kᵀ
+    mma_tiles_kk<NP>(dp, smem_u32(m.res[1]), smem_u32(m.str[buf][1]), nks);  // dP = dO·Vᵀ
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(s);
@@ -305,35 +365,44 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
       s[i] = pr * (dp[i] - dlt[hr]);  // dS (w.r.t. the scaled scores)
     }
     wgmma_fence();
-    mma_regs_tile(dq, s, smem_u32(m.str[buf][0]));  // dQ += dS·K
+    mma_regs_tile<NO>(dq, s, smem_u32(m.str[buf][0]) + pn0 * kPanel, nout);  // dQ += dS·K
     wgmma_commit();
     wgmma_wait<0>();
-    fence_regs(dq);
+#pragma unroll
+    for (int jo = 0; jo < NO; ++jo) fence_regs(dq[jo]);
     __syncthreads();
     if (warp_id() == 0 && j + 2 < nkb) {
-      if (elect_one()) issue_pair(m, buf, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + (j + 2) * BQ);
+      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + (j + 2) * BQ);
       __syncwarp();
     }
   }
-  store_rows(p.dqkv + (long long)rowbase * p.ld_dqkv, p.ld_dqkv, q0, p.T, h * p.hd, p.hd, dq, p.scale);
+  store_panels<NO>(p.dqkv + (long long)rowbase * p.ld_dqkv, p.ld_dqkv, q0, p.T, h * p.hd, p.hd, pn0, nout, dq, p.scale);
 }
 
 // =============================================================================================== backward: dK, dV
+template <int NP>
 __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap map_qkv,
                                                                 const __grid_constant__ CUtensorMap map_do, const BwdArgs p) {
+  constexpr int NO = dkv_out_panels(NP), NSPLIT = splits(NP, dkv_out_panels(NP));
   if (threadIdx.x == 0) pdl_launch_dependents();
   const int nkb = (p.T + BQ - 1) / BQ;
-  const int kb = blockIdx.x;  // key block; query blocks kb .. nkb-1
+  const int kb = blockIdx.x / NSPLIT;  // key block; query blocks kb .. nkb-1
+  const int pn0 = (blockIdx.x % NSPLIT) * NO;
+  const int nout = NP % NO == 0 ? NO : min(NO, NP - pn0);
   const int h = blockIdx.y, b = blockIdx.z;
   const int k0 = kb * BQ, rowbase = b * p.T;
   const int nblk = nkb - kb;
-  const Smem m = smem_layout();
-  prologue<2>(m, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + k0, {&map_qkv, h}, {&map_do, h}, rowbase + k0, nblk);
+  const int nks = (p.hd + 15) / 16;
+  const Smem m = smem_layout<2, NP>();
+  prologue<2, NP>(m, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + k0, {&map_qkv, h}, {&map_do, h}, rowbase + k0, nblk);
   const long long bh = (long long)b * p.nh + h;
   const int key_lo = k0 + frag_row(0);
-  float dk[32], dv[32];
-  zero32(dk);
-  zero32(dv);
+  float dk[NO][32], dv[NO][32];
+#pragma unroll
+  for (int j = 0; j < NO; ++j) {
+    zero32(dk[j]);
+    zero32(dv[j]);
+  }
   for (int jj = 0; jj < nblk; ++jj) {
     const int buf = jj & 1;
     const int qs = (kb + jj) * BQ;
@@ -348,8 +417,8 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
     zero32(st);
     zero32(dpt);
     wgmma_fence();
-    mma_tiles_kk(st, smem_u32(m.res[0]), smem_u32(m.str[buf][0]));   // Sᵀ = K·Qᵀ
-    mma_tiles_kk(dpt, smem_u32(m.res[1]), smem_u32(m.str[buf][1]));  // dPᵀ = V·dOᵀ
+    mma_tiles_kk<NP>(st, smem_u32(m.res[0]), smem_u32(m.str[buf][0]), nks);   // Sᵀ = K·Qᵀ
+    mma_tiles_kk<NP>(dpt, smem_u32(m.res[1]), smem_u32(m.str[buf][1]), nks);  // dPᵀ = V·dOᵀ
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(st);
@@ -363,21 +432,24 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
       st[i] = pr;                                       // Pᵀ
     }
     wgmma_fence();
-    mma_regs_tile(dv, st, smem_u32(m.str[buf][1]));   // dV += Pᵀ·dO
-    mma_regs_tile(dk, dpt, smem_u32(m.str[buf][0]));  // dK += dSᵀ·Q
+    mma_regs_tile<NO>(dv, st, smem_u32(m.str[buf][1]) + pn0 * kPanel, nout);   // dV += Pᵀ·dO
+    mma_regs_tile<NO>(dk, dpt, smem_u32(m.str[buf][0]) + pn0 * kPanel, nout);  // dK += dSᵀ·Q
     wgmma_commit();
     wgmma_wait<0>();
-    fence_regs(dv);
-    fence_regs(dk);
+#pragma unroll
+    for (int j = 0; j < NO; ++j) {
+      fence_regs(dv[j]);
+      fence_regs(dk[j]);
+    }
     __syncthreads();
     if (warp_id() == 0 && jj + 2 < nblk) {
-      if (elect_one()) issue_pair(m, buf, {&map_qkv, h}, {&map_do, h}, rowbase + qs + 2 * BQ);
+      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, h}, {&map_do, h}, rowbase + qs + 2 * BQ);
       __syncwarp();
     }
   }
   bf16* base = p.dqkv + (long long)rowbase * p.ld_dqkv;
-  store_rows(base, p.ld_dqkv, k0, p.T, (p.nh + h) * p.hd, p.hd, dk, p.scale);
-  store_rows(base, p.ld_dqkv, k0, p.T, (2 * p.nh + h) * p.hd, p.hd, dv, 1.0f);
+  store_panels<NO>(base, p.ld_dqkv, k0, p.T, (p.nh + h) * p.hd, p.hd, pn0, nout, dk, p.scale);
+  store_panels<NO>(base, p.ld_dqkv, k0, p.T, (2 * p.nh + h) * p.hd, p.hd, pn0, nout, dv, 1.0f);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -417,8 +489,47 @@ CUtensorMap head_map(const void* ptr, long long ld, long long rows, int hd, int 
 
 void check_shape(int B, int T, int nh, int hd) {
   if (B <= 0 || T <= 0 || nh <= 0) throw std::runtime_error("attention: empty problem");
-  if (hd % 8 != 0 || hd > 64) throw std::runtime_error("attention: head_dim must be a multiple of 8 and <= 64");
+  if (hd <= 0 || hd % 8 != 0 || hd > kMaxHeadDim)
+    throw std::runtime_error("attention: head_dim must be a multiple of 8 and <= 256, got " + std::to_string(hd));
 }
+
+template <int NP>
+void fwd_np(const AttnDesc& d, const CUtensorMap& map, cudaStream_t stream) {
+  constexpr int smem = smem_bytes(1, NP);
+  static const bool configured =
+      (check(cudaFuncSetAttribute(attn_fwd_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "cudaFuncSetAttribute(attn_fwd)"), true);
+  (void)configured;
+  FwdArgs p;
+  p.out = reinterpret_cast<bf16*>(d.out); p.ld_out = d.ld_out; p.lse = d.lse;
+  p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
+  p.scale_log2 = d.scale * 1.4426950408889634f;
+  const dim3 grid((unsigned)((d.T + BQ - 1) / BQ), (unsigned)d.nh, (unsigned)d.B);
+  launch_k(attn_fwd_kernel<NP>, grid, kThreads, smem, stream, map, p);
+  RB_CHECK_LAUNCH("attn_fwd_kernel");
+}
+
+template <int NP>
+void bwd_np(const AttnBwdDesc& d, const CUtensorMap& map_qkv, const CUtensorMap& map_do, cudaStream_t stream) {
+  constexpr int smem = smem_bytes(2, NP);
+  static const bool configured =
+      (check(cudaFuncSetAttribute(attn_bwd_dq_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "cudaFuncSetAttribute(attn_dq)"),
+       check(cudaFuncSetAttribute(attn_bwd_dkv_kernel<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "cudaFuncSetAttribute(attn_dkv)"),
+       true);
+  (void)configured;
+  BwdArgs p;
+  p.lse = d.lse; p.delta = d.delta; p.dqkv = reinterpret_cast<bf16*>(d.dqkv); p.ld_dqkv = d.ld_dqkv;
+  p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
+  p.scale = d.scale; p.scale_log2 = d.scale * 1.4426950408889634f;
+  const unsigned nblk = (unsigned)((d.T + BQ - 1) / BQ);
+  const dim3 grid_dkv(nblk * splits(NP, dkv_out_panels(NP)), (unsigned)d.nh, (unsigned)d.B);
+  launch_k(attn_bwd_dkv_kernel<NP>, grid_dkv, kThreads, smem, stream, map_qkv, map_do, p);
+  RB_CHECK_LAUNCH("attn_bwd_dkv_kernel");
+  const dim3 grid_dq(nblk * splits(NP, dq_out_panels(NP)), (unsigned)d.nh, (unsigned)d.B);
+  launch_k(attn_bwd_dq_kernel<NP>, grid_dq, kThreads, smem, stream, map_qkv, map_do, p);
+  RB_CHECK_LAUNCH("attn_bwd_dq_kernel");
+}
+
+int panels(int hd) { return (hd + 63) / 64; }
 
 }  // namespace
 
@@ -426,18 +537,12 @@ void attention_fwd(const AttnDesc& d, cudaStream_t stream) {
   check_shape(d.B, d.T, d.nh, d.hd);
   const long long rows = (long long)d.B * d.T;
   CUtensorMap map = head_map(d.qkv, d.ld_qkv, rows, d.hd, 3 * d.nh);
-  static bool configured = false;
-  if (!configured) {
-    check(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem), "cudaFuncSetAttribute(attn_fwd)");
-    configured = true;
+  switch (panels(d.hd)) {
+    case 1: fwd_np<1>(d, map, stream); break;
+    case 2: fwd_np<2>(d, map, stream); break;
+    case 3: fwd_np<3>(d, map, stream); break;
+    default: fwd_np<4>(d, map, stream); break;
   }
-  FwdArgs p;
-  p.out = reinterpret_cast<bf16*>(d.out); p.ld_out = d.ld_out; p.lse = d.lse;
-  p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
-  p.scale_log2 = d.scale * 1.4426950408889634f;
-  const dim3 grid((unsigned)((d.T + BQ - 1) / BQ), (unsigned)d.nh, (unsigned)d.B);
-  launch_k(attn_fwd_kernel, grid, kThreads, kSmem, stream, map, p);
-  RB_CHECK_LAUNCH("attn_fwd_kernel");
 }
 
 void attention_bwd(const AttnBwdDesc& d, cudaStream_t stream) {
@@ -445,12 +550,6 @@ void attention_bwd(const AttnBwdDesc& d, cudaStream_t stream) {
   const long long rows = (long long)d.B * d.T;
   CUtensorMap map_qkv = head_map(d.qkv, d.ld_qkv, rows, d.hd, 3 * d.nh);
   CUtensorMap map_do = head_map(d.dout, d.ld_dout, rows, d.hd, d.nh);
-  static bool configured = false;
-  if (!configured) {
-    check(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem), "cudaFuncSetAttribute(attn_dq)");
-    check(cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem), "cudaFuncSetAttribute(attn_dkv)");
-    configured = true;
-  }
   {
     const long long total = rows * d.nh;
     const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 8);
@@ -458,16 +557,15 @@ void attention_bwd(const AttnBwdDesc& d, cudaStream_t stream) {
              d.ld_dout, d.delta, d.B, d.T, d.nh, d.hd);
     RB_CHECK_LAUNCH("attn_delta_kernel");
   }
-  BwdArgs p;
-  p.lse = d.lse; p.delta = d.delta; p.dqkv = reinterpret_cast<bf16*>(d.dqkv); p.ld_dqkv = d.ld_dqkv;
-  p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
-  p.scale = d.scale; p.scale_log2 = d.scale * 1.4426950408889634f;
-  const dim3 grid((unsigned)((d.T + BQ - 1) / BQ), (unsigned)d.nh, (unsigned)d.B);
-  launch_k(attn_bwd_dkv_kernel, grid, kThreads, kSmem, stream, map_qkv, map_do, p);
-  RB_CHECK_LAUNCH("attn_bwd_dkv_kernel");
-  launch_k(attn_bwd_dq_kernel, grid, kThreads, kSmem, stream, map_qkv, map_do, p);
-  RB_CHECK_LAUNCH("attn_bwd_dq_kernel");
+  switch (panels(d.hd)) {
+    case 1: bwd_np<1>(d, map_qkv, map_do, stream); break;
+    case 2: bwd_np<2>(d, map_qkv, map_do, stream); break;
+    case 3: bwd_np<3>(d, map_qkv, map_do, stream); break;
+    default: bwd_np<4>(d, map_qkv, map_do, stream); break;
+  }
 }
+
+int attention_smem_bytes(int hd) { return smem_bytes(2, panels(hd)); }
 
 long long attention_ds_pitch(int T) { return ((long long)T + 63) / 64 * 64; }
 long long attention_ds_workspace_elems(int B, int T, int nh) {

@@ -8,7 +8,8 @@ namespace rb {
 // qkv: bf16 [B*T, 3*nh*hd] (q | k | v, heads contiguous inside each third, RoPE already applied), row stride ld_qkv.
 // out: bf16 [B*T, nh*hd] (row stride ld_out).  lse: fp32 [B, nh, T], log2-domain log-sum-exp of the scaled scores
 //      (p = exp2(s * scale * log2(e) - lse)), consumed by the backward kernels.
-// Requirements: hd % 8 == 0, hd <= 64 (a 64-wide TMA box over a narrower head is zero filled).
+// Requirements: hd % 8 == 0, hd <= 256.  A head is read as ceil(hd / 64) TMA boxes 64 columns wide; the columns of the last box
+// past hd are zero filled.
 struct AttnDesc {
   const void* qkv = nullptr;
   long long ld_qkv = 0;
@@ -41,6 +42,8 @@ struct AttnBwdDesc {
 };
 void attention_bwd(const AttnBwdDesc& d, cudaStream_t stream);
 long long attention_ds_pitch(int T);
+// dynamic shared memory per CTA of the largest attention kernel launched for head size hd (bytes)
+int attention_smem_bytes(int hd);
 long long attention_ds_workspace_elems(int B, int T, int nh);
 
 }  // namespace rb

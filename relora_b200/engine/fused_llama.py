@@ -265,13 +265,13 @@ class FusedLlamaStepper:
         if not self.fp8:
             self.fp8_bwd = False
         attention = os.environ.get("RELORA_B200_ATTENTION", attention)
-        native_ok = self.hd % 8 == 0 and self.hd <= 64
-        if attention == "native" and not native_ok:
-            raise RuntimeError(f"--attention native supports head_dim <= 64 (multiple of 8), got {self.hd}")
-        # auto: this repo's wgmma kernels (csrc/attention.cu) wherever they apply -- the hot path then contains no library
-        # attention call; `--attention sdpa` selects torch SDPA (cuDNN; bench/attn_bench.py times both) and is what larger head
-        # dims fall back to
-        self.native_attn = attention == "native" or (attention == "auto" and native_ok)
+        # auto: this repo's wgmma kernels (csrc/attention.cu) for head_dim <= 64 -- the hot path then contains no library
+        # attention call -- and torch SDPA (cuDNN) above; native: the kernels up to head_dim 256; sdpa: torch SDPA
+        # (bench/attn_bench.py times both)
+        self.native_attn = fused.attention_backend(self.hd, attention) == "native"
+        if attention == "native" and not self.native_attn:
+            raise RuntimeError(f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM} (multiple of 8), "
+                               f"got {self.hd}")
         self.side = torch.cuda.Stream(device=dev) if overlap_wgrad else None
         self.fused_dx = os.environ.get("RELORA_B200_FUSED_DX", "1") != "0"
         # stacked output width from which dx uses two kernels (frozen-path GEMM on 256-wide tiles + a mask-and-add pass) instead of

@@ -208,8 +208,8 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
     if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
         logger.warning(f"--frozen_dtype {args.frozen_dtype} needs the fused executor (Llama + ReLoRA on CUDA/bf16); "
                        "the module path runs the frozen weights in the model dtype")
-    if getattr(args, "attention", "auto") == "sdpa":
+    if getattr(args, "attention", "auto") in ("sdpa", "native"):
         import os as _os
 
-        _os.environ["RELORA_B200_ATTENTION"] = "sdpa"  # the module path reads the switch where it calls attention
+        _os.environ["RELORA_B200_ATTENTION"] = args.attention  # the module path reads the switch where it calls attention
     return ModuleStepper(model, info, **kw)

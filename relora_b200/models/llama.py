@@ -199,12 +199,12 @@ class LlamaAttention(nn.Module):
 
 
 def _use_native_attention(q: torch.Tensor, head_dim: int) -> bool:
-    """CUDA + bf16 + head_dim <= 64 (multiple of 8): the wgmma kernels; RELORA_B200_ATTENTION=sdpa forces the library call."""
-    if not q.is_cuda or os.environ.get("RELORA_B200_ATTENTION", "auto") == "sdpa":
+    """The wgmma kernels where ops.fused.attention_backend picks them (RELORA_B200_ATTENTION, CUDA + bf16, head size)."""
+    if not q.is_cuda:
         return False
     from ..ops import dispatch, fused
 
-    return dispatch.use_fused(q) and fused.native_attention_supported(q, head_dim)
+    return dispatch.use_fused(q) and fused.attention_backend(head_dim, q=q) == "native"
 
 
 class LlamaDecoderLayer(nn.Module):

@@ -188,7 +188,7 @@ class GPTNeoXAttention(nn.Module):
 
     def _forward_native(self, qkv, B, T):
         """CUDA / bf16 training path: partial rotary in place on the fused projection output (csrc/neox.cu), then causal attention
-        on the wgmma kernels when the head size allows (<= 64), torch SDPA otherwise.  Positions are 0..T-1 (no cache)."""
+        on the wgmma kernels where ops.fused.attention_backend picks them, torch SDPA otherwise.  Positions are 0..T-1 (no cache)."""
         from ..ops import fused
 
         nh, hd, rd = self.num_attention_heads, self.head_size, self.rotary_ndims
@@ -197,7 +197,7 @@ class GPTNeoXAttention(nn.Module):
         q = qkv[..., :hd].permute(0, 2, 1, 3)
         k = qkv[..., hd : 2 * hd].permute(0, 2, 1, 3)
         v = qkv[..., 2 * hd :].permute(0, 2, 1, 3)
-        if fused.native_attention_supported(q, hd) and os.environ.get("RELORA_B200_ATTENTION", "auto") != "sdpa":
+        if fused.attention_backend(hd, q=q) == "native":
             out = fused.causal_attention(q, k, v)
         else:
             out = F.scaled_dot_product_attention(q, k, v, attn_mask=None, dropout_p=0.0, is_causal=T > 1)

@@ -344,9 +344,26 @@ def relora_linear_module(module, x: torch.Tensor) -> torch.Tensor:
 
 
 # ----------------------------------------------------------------------------- causal attention (module path)
-def native_attention_supported(q: torch.Tensor, head_dim: int) -> bool:
-    """The wgmma attention kernels (csrc/attention.cu): CUDA bf16, head_dim a multiple of 8 and <= 64."""
-    return q.is_cuda and q.dtype == _BF16 and head_dim % 8 == 0 and head_dim <= 64
+NATIVE_ATTENTION_MAX_HEAD_DIM = 256  # what the wgmma kernels (csrc/attention.cu) accept
+AUTO_ATTENTION_MAX_HEAD_DIM = 64     # where `--attention auto` uses them
+
+
+def attention_backend(head_dim: int, mode: Optional[str] = None, q: Optional[torch.Tensor] = None) -> str:
+    """Which causal-attention implementation runs: ``"native"`` (the wgmma kernels of csrc/attention.cu) or ``"sdpa"``
+    (torch SDPA, cuDNN).  ``mode`` is the ``--attention`` choice; by default ``RELORA_B200_ATTENTION``, else ``auto``.
+
+    * ``sdpa``: always SDPA.
+    * ``auto``: native for ``head_dim % 8 == 0 and head_dim <= 64``, SDPA otherwise.
+    * ``native``: native for ``head_dim % 8 == 0 and head_dim <= 256``, SDPA otherwise (the fused executor raises there).
+
+    With ``q`` given, native also needs q on CUDA in bf16."""
+    mode = mode or os.environ.get("RELORA_B200_ATTENTION", "auto")
+    if mode not in ("auto", "native", "sdpa"):
+        raise ValueError(f"attention mode must be auto, native or sdpa, got {mode!r}")
+    if mode == "sdpa" or (q is not None and not (q.is_cuda and q.dtype == _BF16)):
+        return "sdpa"
+    limit = NATIVE_ATTENTION_MAX_HEAD_DIM if mode == "native" else AUTO_ATTENTION_MAX_HEAD_DIM
+    return "native" if head_dim % 8 == 0 and 0 < head_dim <= limit else "sdpa"
 
 
 class _CausalAttentionFn(torch.autograd.Function):
