@@ -162,12 +162,15 @@ __device__ __forceinline__ void prologue(const Smem& m, TileSrc r0, TileSrc r1, 
   mbar_wait(m.res_bar, 0);
 }
 
+// Head map of the packed qkv buffer, in head-columns of hd: q, k, v of head h sit at h·hs, h·hs + ws, h·hs + 2·ws.
+// Default layout [(q|k|v), nh, hd]: hs = 1, ws = nh.  Interleaved (GPT-NeoX query_key_value) [nh, (q|k|v), hd]: hs = 3, ws = 1.
 struct FwdArgs {
   bf16* out;
   long long ld_out;
   float* lse;
   int B, T, nh, hd;
   float scale_log2;
+  int hs, ws;
 };
 
 // =============================================================================================== forward
@@ -182,7 +185,8 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
   const int nks = (p.hd + 15) / 16;
   const Smem m = smem_layout<1, NP>();
   // resident: Q; streamed: K, V
-  prologue<1, NP>(m, {&map_qkv, h}, {&map_qkv, h}, rowbase + q0, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase, nkb);
+  const int hq = h * p.hs, hk = hq + p.ws, hv = hq + 2 * p.ws;
+  prologue<1, NP>(m, {&map_qkv, hq}, {&map_qkv, hq}, rowbase + q0, {&map_qkv, hk}, {&map_qkv, hv}, rowbase, nkb);
   const uint32_t sq = smem_u32(m.res[0]);
   float o[NP][32], mrow[2] = {kNegInf, kNegInf}, lrow[2] = {0.f, 0.f};
 #pragma unroll
@@ -235,7 +239,7 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
     for (int pn = 0; pn < NP; ++pn) fence_regs(o[pn]);
     __syncthreads();  // every warp is done with this buffer
     if (warp_id() == 0 && j + 2 < nkb) {
-      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + (j + 2) * BQ);
+      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, hk}, {&map_qkv, hv}, rowbase + (j + 2) * BQ);
       __syncwarp();
     }
   }
@@ -297,6 +301,7 @@ struct BwdArgs {
   long long ld_dqkv;
   int B, T, nh, hd;
   float scale, scale_log2;
+  int hs, ws;  // head map of qkv / dqkv (see FwdArgs)
 };
 
 __device__ __forceinline__ void store_rows(bf16* base, long long ld, int row0, int rows_valid, int col_ofs, int hd, const float (&d)[32], float sc) {
@@ -331,7 +336,8 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
   const int nkb = qb + 1;
   const int nks = (p.hd + 15) / 16;
   const Smem m = smem_layout<2, NP>();
-  prologue<2, NP>(m, {&map_qkv, h}, {&map_do, h}, rowbase + q0, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase, nkb);
+  const int hq = h * p.hs, hk = hq + p.ws, hv = hq + 2 * p.ws;
+  prologue<2, NP>(m, {&map_qkv, hq}, {&map_do, h}, rowbase + q0, {&map_qkv, hk}, {&map_qkv, hv}, rowbase, nkb);
   const long long bh = (long long)b * p.nh + h;
   const int r_lo = q0 + frag_row(0);
   float lse[2], dlt[2];
@@ -372,11 +378,11 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
     for (int jo = 0; jo < NO; ++jo) fence_regs(dq[jo]);
     __syncthreads();
     if (warp_id() == 0 && j + 2 < nkb) {
-      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + (j + 2) * BQ);
+      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, hk}, {&map_qkv, hv}, rowbase + (j + 2) * BQ);
       __syncwarp();
     }
   }
-  store_panels<NO>(p.dqkv + (long long)rowbase * p.ld_dqkv, p.ld_dqkv, q0, p.T, h * p.hd, p.hd, pn0, nout, dq, p.scale);
+  store_panels<NO>(p.dqkv + (long long)rowbase * p.ld_dqkv, p.ld_dqkv, q0, p.T, hq * p.hd, p.hd, pn0, nout, dq, p.scale);
 }
 
 // =============================================================================================== backward: dK, dV
@@ -394,7 +400,8 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
   const int nblk = nkb - kb;
   const int nks = (p.hd + 15) / 16;
   const Smem m = smem_layout<2, NP>();
-  prologue<2, NP>(m, {&map_qkv, p.nh + h}, {&map_qkv, 2 * p.nh + h}, rowbase + k0, {&map_qkv, h}, {&map_do, h}, rowbase + k0, nblk);
+  const int hq = h * p.hs, hk = hq + p.ws, hv = hq + 2 * p.ws;
+  prologue<2, NP>(m, {&map_qkv, hk}, {&map_qkv, hv}, rowbase + k0, {&map_qkv, hq}, {&map_do, h}, rowbase + k0, nblk);
   const long long bh = (long long)b * p.nh + h;
   const int key_lo = k0 + frag_row(0);
   float dk[NO][32], dv[NO][32];
@@ -443,13 +450,13 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
     }
     __syncthreads();
     if (warp_id() == 0 && jj + 2 < nblk) {
-      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, h}, {&map_do, h}, rowbase + qs + 2 * BQ);
+      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, hq}, {&map_do, h}, rowbase + qs + 2 * BQ);
       __syncwarp();
     }
   }
   bf16* base = p.dqkv + (long long)rowbase * p.ld_dqkv;
-  store_panels<NO>(base, p.ld_dqkv, k0, p.T, (p.nh + h) * p.hd, p.hd, pn0, nout, dk, p.scale);
-  store_panels<NO>(base, p.ld_dqkv, k0, p.T, (2 * p.nh + h) * p.hd, p.hd, pn0, nout, dv, 1.0f);
+  store_panels<NO>(base, p.ld_dqkv, k0, p.T, hk * p.hd, p.hd, pn0, nout, dk, p.scale);
+  store_panels<NO>(base, p.ld_dqkv, k0, p.T, hv * p.hd, p.hd, pn0, nout, dv, 1.0f);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -503,6 +510,7 @@ void fwd_np(const AttnDesc& d, const CUtensorMap& map, cudaStream_t stream) {
   p.out = reinterpret_cast<bf16*>(d.out); p.ld_out = d.ld_out; p.lse = d.lse;
   p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
   p.scale_log2 = d.scale * 1.4426950408889634f;
+  p.hs = d.interleaved ? 3 : 1; p.ws = d.interleaved ? 1 : d.nh;
   const dim3 grid((unsigned)((d.T + BQ - 1) / BQ), (unsigned)d.nh, (unsigned)d.B);
   launch_k(attn_fwd_kernel<NP>, grid, kThreads, smem, stream, map, p);
   RB_CHECK_LAUNCH("attn_fwd_kernel");
@@ -520,6 +528,7 @@ void bwd_np(const AttnBwdDesc& d, const CUtensorMap& map_qkv, const CUtensorMap&
   p.lse = d.lse; p.delta = d.delta; p.dqkv = reinterpret_cast<bf16*>(d.dqkv); p.ld_dqkv = d.ld_dqkv;
   p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
   p.scale = d.scale; p.scale_log2 = d.scale * 1.4426950408889634f;
+  p.hs = d.interleaved ? 3 : 1; p.ws = d.interleaved ? 1 : d.nh;
   const unsigned nblk = (unsigned)((d.T + BQ - 1) / BQ);
   const dim3 grid_dkv(nblk * splits(NP, dkv_out_panels(NP)), (unsigned)d.nh, (unsigned)d.B);
   launch_k(attn_bwd_dkv_kernel<NP>, grid_dkv, kThreads, smem, stream, map_qkv, map_do, p);

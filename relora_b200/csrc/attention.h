@@ -18,6 +18,9 @@ struct AttnDesc {
   float* lse = nullptr;
   int B = 0, T = 0, nh = 0, hd = 0;
   float scale = 1.0f;  // 1/sqrt(hd)
+  // false: qkv is [(q|k|v), nh, hd] per row (above).  true: [nh, (q|k|v), hd] per row, the head-interleaved layout of GPT-NeoX's
+  // query_key_value projection (q, k, v of head h at head-columns 3h, 3h+1, 3h+2).
+  bool interleaved = false;
 };
 void attention_fwd(const AttnDesc& d, cudaStream_t stream);
 
@@ -36,6 +39,7 @@ struct AttnBwdDesc {
   long long ld_dqkv = 0;
   int B = 0, T = 0, nh = 0, hd = 0;
   float scale = 1.0f;
+  bool interleaved = false;  // layout of qkv and dqkv (see AttnDesc)
   // optional bf16 workspace of attention_ds_workspace_elems(B, T, nh) elements; not read by the sm_90 kernels (the dQ kernel
   // recomputes S and dP), kept so callers that size it need no change
   void* ds_workspace = nullptr;

@@ -260,19 +260,19 @@ void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Te
 }
 
 // causal flash attention over the packed (post-RoPE) qkv buffer [B*T, 3*nh*hd]
-void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64_t T, int64_t nh, int64_t hd, double scale) {
+void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64_t T, int64_t nh, int64_t hd, double scale, bool interleaved) {
   chk_bf16(qkv, "qkv"); chk_bf16(out, "out"); chk_2d_rowmajor(qkv, "qkv"); chk_2d_rowmajor(out, "out");
   TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == 3 * nh * hd, "qkv must be [B*T, 3*nh*hd]");
   TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd, "out must be [B*T, nh*hd]");
   TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
   rb::AttnDesc d;
   d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0); d.lse = lse.data_ptr<float>();
-  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.hd = (int)hd; d.scale = (float)scale;
+  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
   c10::cuda::CUDAGuard guard(qkv.device());
   rb::attention_fwd(d, cur_stream());
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& delta, Tensor& dqkv, int64_t B,
-                   int64_t T, int64_t nh, int64_t hd, double scale, const OptTensor& ds_workspace) {
+                   int64_t T, int64_t nh, int64_t hd, double scale, const OptTensor& ds_workspace, bool interleaved) {
   chk_bf16(qkv, "qkv"); chk_bf16(out, "out"); chk_bf16(dout, "dout"); chk_bf16(dqkv, "dqkv");
   chk_2d_rowmajor(qkv, "qkv"); chk_2d_rowmajor(out, "out"); chk_2d_rowmajor(dout, "dout"); chk_2d_rowmajor(dqkv, "dqkv");
   TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == 3 * nh * hd && dqkv.size(0) == B * T && dqkv.size(1) == 3 * nh * hd, "qkv / dqkv must be [B*T, 3*nh*hd]");
@@ -283,7 +283,7 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0);
   d.dout = dout.data_ptr(); d.ld_dout = dout.stride(0); d.lse = lse.data_ptr<float>(); d.delta = delta.data_ptr<float>();
   d.dqkv = dqkv.data_ptr(); d.ld_dqkv = dqkv.stride(0);
-  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.hd = (int)hd; d.scale = (float)scale;
+  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
   if (ds_workspace.has_value()) {
     chk_bf16(*ds_workspace, "ds_workspace");
     TORCH_CHECK(ds_workspace->is_contiguous() && ds_workspace->numel() >= rb::attention_ds_workspace_elems((int)B, (int)T, (int)nh),
@@ -407,39 +407,116 @@ void gemm_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tensor& 
 }
 
 // ---------------------------------------------------------------------------------------------- GPT-NeoX / Pythia block
-void layernorm_fwd(const Tensor& x, const Tensor& w, const OptTensor& b, Tensor& y, Tensor& mean, Tensor& rstd, double eps) {
+void chk_ln_vec(const OptTensor& t, int64_t H, const char* name) {
+  if (!t.has_value()) return;
+  chk_bf16(*t, name);
+  TORCH_CHECK(t->is_contiguous() && t->numel() == H, name, " must be contiguous [H]");
+}
+void chk_f32_vec(const OptTensor& t, int64_t n, const char* name) {
+  if (!t.has_value()) return;
+  TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == n, name, " must be fp32 contiguous [", n, "]");
+}
+void chk_rows(const OptTensor& t, const Tensor& like, const char* name) {
+  if (!t.has_value()) return;
+  chk_bf16(*t, name);
+  TORCH_CHECK(t->is_contiguous() && t->sizes() == like.sizes(), name, " must be contiguous and shaped like x");
+}
+void* ptr_or_null(const OptTensor& t) { return t.has_value() ? t->data_ptr() : nullptr; }
+float* f32_or_null(const OptTensor& t) { return t.has_value() ? t->data_ptr<float>() : nullptr; }
+
+rb::LnDrop ln_drop(const OptTensor& seed, double p) {
+  rb::LnDrop d;
+  d.seed_ptr = u32ptr(seed);
+  d.thr16 = (uint32_t)llround(p * 65536.0);
+  d.inv_keep = (float)(1.0 / (1.0 - p));
+  return d;
+}
+
+// y = LN(x; w, b).  Executor options: y2 = LN(x; w2, b2) from the same statistics, and dropout copies xd (of y, mask key `keys[0]`) /
+// xd2 (of y2, `keys[1]`) with probability p from the device seed.
+void layernorm_fwd(const Tensor& x, const Tensor& w, const OptTensor& b, Tensor& y, Tensor& mean, Tensor& rstd, double eps, const OptTensor& w2,
+                   const OptTensor& b2, const OptTensor& y2, const OptTensor& xd, const OptTensor& xd2, const OptTensor& seed,
+                   std::vector<int64_t> keys, double p) {
   chk_bf16(x, "x"); chk_bf16(w, "weight"); chk_bf16(y, "y");
   TORCH_CHECK(x.is_contiguous() && y.is_contiguous() && w.is_contiguous() && x.dim() == 2 && w.numel() == x.size(1));
   TORCH_CHECK(mean.scalar_type() == at::kFloat && rstd.scalar_type() == at::kFloat && mean.numel() == x.size(0) && rstd.numel() == x.size(0));
-  if (b.has_value()) { chk_bf16(*b, "bias"); TORCH_CHECK(b->is_contiguous() && b->numel() == x.size(1)); }
+  const int64_t H = x.size(1);
+  if (b.has_value()) { chk_bf16(*b, "bias"); TORCH_CHECK(b->is_contiguous() && b->numel() == H); }
+  chk_ln_vec(w2, H, "w2"); chk_ln_vec(b2, H, "b2");
+  chk_rows(y2, x, "y2"); chk_rows(xd, x, "xd"); chk_rows(xd2, x, "xd2");
+  TORCH_CHECK(y2.has_value() == w2.has_value(), "y2 and w2 go together");
+  TORCH_CHECK(!xd2.has_value() || y2.has_value(), "xd2 needs y2");
+  const size_t nkeys = (xd.has_value() || xd2.has_value()) ? 2 : 0;
+  TORCH_CHECK(nkeys == 0 || (keys.size() == 2 && seed.has_value() && p >= 0.0 && p < 1.0), "dropout copies need the seed, two keys and p");
+  rb::LnFwdOut n1, n2;
+  n1.w = w.data_ptr(); n1.b = ptr_or_null(b); n1.y = y.data_ptr(); n1.xd = ptr_or_null(xd);
+  n2.w = ptr_or_null(w2); n2.b = ptr_or_null(b2); n2.y = ptr_or_null(y2); n2.xd = ptr_or_null(xd2);
+  if (nkeys) { n1.key = (uint32_t)keys[0]; n2.key = (uint32_t)keys[1]; }
   c10::cuda::CUDAGuard guard(x.device());
-  const bool ok = rb::layernorm_fwd(x.data_ptr(), w.data_ptr(), b.has_value() ? b->data_ptr() : nullptr, y.data_ptr(), mean.data_ptr<float>(),
-                                    rstd.data_ptr<float>(), (int)x.size(0), (int)x.size(1), (float)eps, cur_stream());
+  const bool ok = rb::layernorm_fwd_dual(x.data_ptr(), n1, n2, mean.data_ptr<float>(), rstd.data_ptr<float>(), (int)x.size(0), (int)H, (float)eps,
+                                         nkeys ? ln_drop(seed, p) : rb::LnDrop{}, cur_stream());
   TORCH_CHECK(ok, "layernorm_fwd: hidden size must be a multiple of 8 and <= 4096");
 }
+
+// Module form: dx = LNᵀ(dy).  Executor form (any of dres / dy2 / dres_sum given): dx = dres + LNᵀ(dy) [+ LN2ᵀ(dy2)], γ / β gradients of
+// both norms, dres_sum (and dres_sum2) += Σ rows of dres.  All fp32 gradients accumulate.
 void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& w, const Tensor& mean, const Tensor& rstd, Tensor& dx, Tensor& dw,
-                   const OptTensor& db) {
+                   const OptTensor& db, const OptTensor& dres, const OptTensor& dy2, const OptTensor& w2, const OptTensor& dw2,
+                   const OptTensor& db2, const OptTensor& dres_sum, const OptTensor& dres_sum2) {
   chk_bf16(dy, "dy"); chk_bf16(x, "x"); chk_bf16(w, "weight"); chk_bf16(dx, "dx");
   TORCH_CHECK(dy.is_contiguous() && x.is_contiguous() && dx.is_contiguous() && w.is_contiguous() && x.dim() == 2);
   TORCH_CHECK(dw.scalar_type() == at::kFloat && dw.is_contiguous() && dw.numel() == x.size(1));
   if (db.has_value()) TORCH_CHECK(db->scalar_type() == at::kFloat && db->is_contiguous() && db->numel() == x.size(1));
   c10::cuda::CUDAGuard guard(x.device());
-  const bool ok = rb::layernorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), dx.data_ptr(),
-                                    dw.data_ptr<float>(), db.has_value() ? db->data_ptr<float>() : nullptr, (int)x.size(0), (int)x.size(1),
-                                    cur_stream());
+  const int64_t H = x.size(1);
+  bool ok;
+  if (!dres.has_value() && !dy2.has_value() && !dres_sum.has_value()) {
+    ok = rb::layernorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), dx.data_ptr(),
+                           dw.data_ptr<float>(), db.has_value() ? db->data_ptr<float>() : nullptr, (int)x.size(0), (int)H, cur_stream());
+  } else {
+    chk_rows(dres, x, "dres"); chk_rows(dy2, x, "dy2"); chk_ln_vec(w2, H, "w2");
+    chk_f32_vec(dw2, H, "dw2"); chk_f32_vec(db2, H, "db2"); chk_f32_vec(dres_sum, H, "dres_sum"); chk_f32_vec(dres_sum2, H, "dres_sum2");
+    TORCH_CHECK(dy2.has_value() == w2.has_value() && dy2.has_value() == dw2.has_value(), "dy2, w2 and dw2 go together");
+    TORCH_CHECK(!dres_sum.has_value() || dres.has_value(), "dres_sum needs dres");
+    TORCH_CHECK(!dres_sum2.has_value() || dres_sum.has_value(), "dres_sum2 needs dres_sum");
+    rb::LnBwdNorm n1, n2;
+    n1.dy = dy.data_ptr(); n1.w = w.data_ptr(); n1.dw = dw.data_ptr<float>(); n1.db = f32_or_null(db);
+    n2.dy = ptr_or_null(dy2); n2.w = ptr_or_null(w2); n2.dw = f32_or_null(dw2); n2.db = f32_or_null(db2);
+    ok = rb::layernorm_bwd_dual(x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), n1, n2, ptr_or_null(dres), dx.data_ptr(),
+                                f32_or_null(dres_sum), f32_or_null(dres_sum2), (int)x.size(0), (int)H, cur_stream());
+  }
   TORCH_CHECK(ok, "layernorm_bwd: hidden size must be a multiple of 8 and <= 2048");
 }
-void gelu_fwd(const Tensor& z, Tensor& a, bool tanh_approx) {
+// a = GELU(z); xd (optional): dropout copy of a with mask key `key` (rows of z.size(-1) elements)
+void gelu_fwd(const Tensor& z, Tensor& a, bool tanh_approx, const OptTensor& xd, const OptTensor& seed, int64_t key, double p) {
   chk_bf16(z, "z"); chk_bf16(a, "a");
   TORCH_CHECK(z.is_contiguous() && a.is_contiguous() && z.numel() == a.numel());
+  chk_rows(xd, z, "xd");
+  TORCH_CHECK(!xd.has_value() || (seed.has_value() && p >= 0.0 && p < 1.0), "the dropout copy needs the seed and p");
   c10::cuda::CUDAGuard guard(z.device());
-  rb::gelu_fwd(z.data_ptr(), a.data_ptr(), z.numel(), tanh_approx, cur_stream());
+  rb::gelu_fwd(z.data_ptr(), a.data_ptr(), z.numel(), tanh_approx, cur_stream(), ptr_or_null(xd), (int)z.size(-1), (uint32_t)key,
+               xd.has_value() ? ln_drop(seed, p) : rb::LnDrop{});
 }
-void gelu_bwd(const Tensor& da, const Tensor& z, Tensor& dz, bool tanh_approx) {
+// dz = da · GELU'(z); dbias (optional, fp32 [N]) += Σ rows of dz
+void gelu_bwd(const Tensor& da, const Tensor& z, Tensor& dz, bool tanh_approx, const OptTensor& dbias) {
   chk_bf16(da, "da"); chk_bf16(z, "z"); chk_bf16(dz, "dz");
   TORCH_CHECK(da.is_contiguous() && z.is_contiguous() && dz.is_contiguous() && z.numel() == da.numel() && z.numel() == dz.numel());
   c10::cuda::CUDAGuard guard(z.device());
+  if (dbias.has_value()) {
+    const int64_t N = z.size(-1);
+    chk_f32_vec(dbias, N, "dbias");
+    rb::gelu_bwd_colsum(da.data_ptr(), z.data_ptr(), dz.data_ptr(), dbias->data_ptr<float>(), (int)(z.numel() / N), (int)N, tanh_approx, cur_stream());
+    return;
+  }
   rb::gelu_bwd(da.data_ptr(), z.data_ptr(), dz.data_ptr(), z.numel(), tanh_approx, cur_stream());
+}
+// out (fp32 [N]) += Σ rows of x [M, N]
+void colsum(const Tensor& x, Tensor& out) {
+  chk_bf16(x, "x"); chk_2d_rowmajor(x, "x");
+  TORCH_CHECK(x.is_contiguous(), "x must be contiguous");
+  chk_f32_vec(out, x.size(1), "out");
+  c10::cuda::CUDAGuard guard(x.device());
+  rb::colsum(x.data_ptr(), out.data_ptr<float>(), (int)x.size(0), (int)x.size(1), cur_stream());
 }
 void neox_rope(Tensor& qkv, int64_t T, int64_t nh, int64_t hd, int64_t rot, const Tensor& cos, const Tensor& sin, int64_t pos0, bool inverse) {
   chk_bf16(qkv, "qkv"); chk_2d_rowmajor(qkv, "qkv");
@@ -621,9 +698,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fp8_prep", &fp8_prep, py::arg("state"), py::arg("w_scale"), py::arg("inv_sx"), py::arg("alpha_main"), py::arg("alpha_inv"), py::arg("margin"),
         py::arg("n_e4m3") = -1);
   m.def("attention_smem_bytes", [](int64_t hd) { return rb::attention_smem_bytes((int)hd); });
-  m.def("attention_fwd", &attention_fwd);
+  m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("out"), py::arg("lse"), py::arg("B"), py::arg("T"), py::arg("nh"), py::arg("hd"),
+        py::arg("scale"), py::arg("interleaved") = false);
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("delta"), py::arg("dqkv"),
-        py::arg("B"), py::arg("T"), py::arg("nh"), py::arg("hd"), py::arg("scale"), py::arg("ds_workspace") = py::none());
+        py::arg("B"), py::arg("T"), py::arg("nh"), py::arg("hd"), py::arg("scale"), py::arg("ds_workspace") = py::none(),
+        py::arg("interleaved") = false);
   m.def("attention_ds_workspace_elems", &rb::attention_ds_workspace_elems);
   m.def("lora_dx", &lora_dx, py::arg("dy"), py::arg("w"), py::arg("du"), py::arg("a"), py::arg("out"), py::arg("seed"), py::arg("keys"),
         py::arg("p"), py::arg("base") = py::none());
@@ -638,10 +717,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mx_dequantize_weight", &mx_dequantize_weight);
   m.def("gemm_mx", &gemm_mx, py::arg("a"), py::arg("sfa"), py::arg("b"), py::arg("sfb"), py::arg("out"), py::arg("M"), py::arg("N"), py::arg("K"),
         py::arg("b_mn_major") = false, py::arg("a2") = py::none(), py::arg("b2") = py::none(), py::arg("residual") = py::none());
-  m.def("layernorm_fwd", &layernorm_fwd);
-  m.def("layernorm_bwd", &layernorm_bwd);
-  m.def("gelu_fwd", &gelu_fwd);
-  m.def("gelu_bwd", &gelu_bwd);
+  m.def("layernorm_fwd", &layernorm_fwd, py::arg("x"), py::arg("w"), py::arg("b"), py::arg("y"), py::arg("mean"), py::arg("rstd"), py::arg("eps"),
+        py::arg("w2") = py::none(), py::arg("b2") = py::none(), py::arg("y2") = py::none(), py::arg("xd") = py::none(), py::arg("xd2") = py::none(),
+        py::arg("seed") = py::none(), py::arg("keys") = std::vector<int64_t>{}, py::arg("p") = 0.0);
+  m.def("layernorm_bwd", &layernorm_bwd, py::arg("dy"), py::arg("x"), py::arg("w"), py::arg("mean"), py::arg("rstd"), py::arg("dx"), py::arg("dw"),
+        py::arg("db"), py::arg("dres") = py::none(), py::arg("dy2") = py::none(), py::arg("w2") = py::none(), py::arg("dw2") = py::none(),
+        py::arg("db2") = py::none(), py::arg("dres_sum") = py::none(), py::arg("dres_sum2") = py::none());
+  m.def("gelu_fwd", &gelu_fwd, py::arg("z"), py::arg("a"), py::arg("tanh_approx"), py::arg("xd") = py::none(), py::arg("seed") = py::none(),
+        py::arg("key") = 0, py::arg("p") = 0.0);
+  m.def("gelu_bwd", &gelu_bwd, py::arg("da"), py::arg("z"), py::arg("dz"), py::arg("tanh_approx"), py::arg("dbias") = py::none());
+  m.def("colsum", &colsum);
   m.def("neox_rope", &neox_rope);
   m.def("embedding_fwd", &embedding_fwd);
   m.def("embedding_bwd", &embedding_bwd);

@@ -58,8 +58,41 @@ bool layernorm_fwd(const void* x, const void* w, const void* b, void* y, float* 
 // dw / db (fp32, may be nullptr for db) are accumulated (+=)
 bool layernorm_bwd(const void* dy, const void* x, const void* w, const float* mean, const float* rstd, void* dx, float* dw, float* db, int M,
                    int H, cudaStream_t s);
-void gelu_fwd(const void* z, void* a, long long n, bool tanh_approx, cudaStream_t s);
+// LoRA-dropout of a kernel output: mask stream mix_seed(*seed_ptr, key) (common.cuh:keep_drop), keep probability inv_keep⁻¹
+struct LnDrop {
+  const uint32_t* seed_ptr = nullptr;
+  uint32_t thr16 = 0;
+  float inv_keep = 1.f;
+};
+// one LayerNorm output of layernorm_fwd_dual: y = LN(x; w, b) (b may be nullptr) and, when xd != nullptr, its dropout copy under `key`
+struct LnFwdOut {
+  const void* w = nullptr;
+  const void* b = nullptr;
+  void* y = nullptr;
+  void* xd = nullptr;
+  uint32_t key = 0;
+};
+// Up to two LayerNorms of the same x in one pass (n2.y == nullptr: one), sharing the fp32 mean / rstd.  H <= 2048, H % 8 == 0.
+bool layernorm_fwd_dual(const void* x, const LnFwdOut& n1, const LnFwdOut& n2, float* mean, float* rstd, int M, int H, float eps,
+                        const LnDrop& drop, cudaStream_t s);
+// one LayerNorm of layernorm_bwd_dual: output gradient dy, weight w; dw / db (fp32, db may be nullptr) accumulated (+=)
+struct LnBwdNorm {
+  const void* dy = nullptr;
+  const void* w = nullptr;
+  float* dw = nullptr;
+  float* db = nullptr;
+};
+// dx = dres + LN1ᵀ(dy1) [+ LN2ᵀ(dy2) when n2.dy != nullptr]; dres may be nullptr.  dsum1 / dsum2 (fp32, optional) += Σ rows of dres.
+bool layernorm_bwd_dual(const void* x, const float* mean, const float* rstd, const LnBwdNorm& n1, const LnBwdNorm& n2, const void* dres,
+                        void* dx, float* dsum1, float* dsum2, int M, int H, cudaStream_t s);
+// xd (optional): dropout copy of the output under `key`, rows of N elements
+void gelu_fwd(const void* z, void* a, long long n, bool tanh_approx, cudaStream_t s, void* xd = nullptr, int N = 0, uint32_t key = 0,
+              const LnDrop& drop = LnDrop{});
 void gelu_bwd(const void* da, const void* z, void* dz, long long n, bool tanh_approx, cudaStream_t s);
+// gelu_bwd on [M, N] that also adds Σ rows of dz into dbias (fp32, 16-byte aligned)
+void gelu_bwd_colsum(const void* da, const void* z, void* dz, float* dbias, int M, int N, bool tanh_approx, cudaStream_t s);
+// out[N] (fp32, 16-byte aligned) += Σ rows of x [M, N] (bf16, contiguous)
+void colsum(const void* x, float* out, int M, int N, cudaStream_t s);
 // partial rotary embedding in place on the fused query_key_value output [rows, nh, 3*hd] (q | k | v per head); fp32 tables [n_pos, rot]
 // holding the cos / sin of the first rot/2 frequencies twice (HF layout: emb = cat(freqs, freqs)); inverse = backward direction
 void neox_rope(void* qkv, long long ld, long long rows, int T, int nh, int hd, int rot, const float* cos, const float* sin, int pos0,

@@ -23,19 +23,17 @@ from __future__ import annotations
 
 import math
 import os
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Tuple
 
 import torch
-import torch.distributed as dist
 import torch.nn.functional as F_
 
 from ..models.llama import LlamaForCausalLM
 from ..ops import fused, native
 from ..parallel.dist import DistInfo
-from ..parallel.flat import FlatAdamW, FlatParamStore
-from ..parallel.grad_sync import GradSync, broadcast_params
+from ..parallel.grad_sync import broadcast_params
 from ..relora import ReLoRaLinear, ReLoRaModel
-from .stepper import UpdateInfo
+from .fused_common import FusedStepperBase
 
 BF = torch.bfloat16
 
@@ -74,7 +72,7 @@ class _Layer:
                  "keys_gu", "key_d", "mods", "merge")
 
 
-class FusedLlamaStepper:
+class FusedLlamaStepper(FusedStepperBase):
     def __init__(self, model: ReLoRaModel, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, symm_factory=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
@@ -145,22 +143,7 @@ class FusedLlamaStepper:
         extra = [(n, p) for n, p in model.named_parameters() if p.requires_grad and id(p) not in seen]
         if extra:
             raise RuntimeError(f"unexpected trainable parameters for the fused executor: {[n for n, _ in extra]}")
-        # ---- transport: NVLink peer-memory kernels when symmetric memory is available, NCCL otherwise
-        self.comm = None
-        if info.world_size > 1 and transport in ("p2p", "auto"):
-            from ..parallel.symm import SymmComm, symmetric_memory_available
-
-            if symmetric_memory_available():
-                try:
-                    self.comm = SymmComm()
-                except Exception as e:  # no P2P access, allocation failure, ...
-                    if transport == "p2p":
-                        raise
-                    from ..obs import logger
-
-                    logger.warning(f"peer-memory collectives unavailable ({type(e).__name__}: {e}); using NCCL")
-            elif transport == "p2p":
-                raise RuntimeError("--comm p2p needs torch symmetric memory over an NCCL process group")
+        self._init_transport(info, transport)
         padded: Dict[int, Tuple[int, int]] = {}
         if fp != f:
             for layer in layers:
@@ -168,19 +151,8 @@ class FusedLlamaStepper:
                 padded[id(mlp.gate_proj.lora_B.weight)] = (fp, r)
                 padded[id(mlp.up_proj.lora_B.weight)] = (fp, r)
                 padded[id(mlp.down_proj.lora_A.weight)] = (r, fp)
-        self.store = FlatParamStore(named, world_size=info.world_size, grad_dtype=torch.float32, bind_grads=False,
-                                    allocator=self.comm.allocator() if self.comm is not None else None,
-                                    storage_shapes=padded)
-        self.trainable_params = [p for _, p in named]
-        self.trainable_names = [n for n, _ in named]
-        self.lora_params = [p for n, p in named if "lora_" in n]
-
-        def pv(p, rows_mult=1):  # stacked view over `rows_mult` adjacent parameters (params and grads)
-            o, n = self.store.segment(p)
-            ps = self.store.storage.get(id(p), tuple(p.shape))  # padded block shape where one exists
-            shape = (ps[0] * rows_mult, ps[1]) if p.dim() == 2 else (ps[0] * rows_mult,)
-            tot = n * rows_mult
-            return self.store.params[o:o + tot].view(shape), self.store.grads[o:o + tot].view(shape)
+        self._init_store(named, padded)
+        pv = self._stacked_view  # stacked view over `rows_mult` adjacent parameters (params and grads)
 
         self.layers: List[_Layer] = []
         for layer in layers:
@@ -222,24 +194,7 @@ class FusedLlamaStepper:
         self.sin = rot.sin_cached[0, 0].to(BF).contiguous()
 
         # ---------------------------------------------------------------- optimizer / comm
-        self.sync = GradSync(self.store, info, transport="nccl", zero=zero and self.comm is None)
-        shard = self.sync.shard if (zero and self.comm is None) else None
-        self._stage = None
-        if self.comm is not None:
-            # fused update: gradients travel as bf16 through a symmetric buffer, each rank owns 1/world of the
-            # optimizer state (ZeRO-1 dataflow) and writes its updated parameters into every replica
-            self.sync.transport = "p2p"
-            self.param_buf = self.comm.buffer_of(self.store.params)
-            self.grad_buf = self.comm.alloc(self.store.numel, BF)
-            self.gred = torch.empty(self.store.numel // info.world_size, dtype=torch.float32, device=dev)
-            shard = self.store.shard_bounds(info.rank, info.world_size)
-        self.optimizer = FlatAdamW(self.store, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, shard=shard,
-                                   native=native or fused.NativeOptim())
-        self.seed = fused.seed_state.get(dev)
-        self._shape = None
-        self._graph = None
-        self._replays = 0
-        self._launches_per_micro = 0
+        self._init_optimizer(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, zero=zero, native=native)
         self._attn_saved: List = []
         # ---- fp8 frozen-weight path: E4M3 copies of the stacked weights + per-site activation scales (csrc/fp8.cu)
         self.fp8 = bool(fp8) or os.environ.get("RELORA_B200_FP8", "0") == "1"
@@ -277,7 +232,6 @@ class FusedLlamaStepper:
         # stacked output width from which dx uses two kernels (frozen-path GEMM on 256-wide tiles + a mask-and-add pass) instead of
         # the one-kernel form; the thresholds (4096 bf16, 2048 with fp8 input-gradient GEMMs) have not been re-tuned on the H100.
         self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0")) or (2048 if self.fp8_bwd else 4096)
-        self._wg_done: Dict[str, torch.cuda.Event] = {}
         # --deterministic: the stacked dA / dB weight-gradient GEMMs run without split-K (one CTA owns an output tile for the whole token
         # reduction: fixed summation order instead of fp32 atomics from several CTAs).  Remaining order-dependent reductions are the
         # [h]-sized norm-weight gradients (block partials combined with vector atomics).
@@ -378,28 +332,6 @@ class FusedLlamaStepper:
             return (None, None, None)
         return (self.x8_h if K == self.h else self.x8_f, self.inv_sx[l, s_i:s_i + 1], self.act_state[l, s_i, 1:2])
 
-    def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False):
-        """u = s·xd_g·A_gᵀ (grouped) ; out = [xn | u]·[W | B]ᵀ (+ residual).
-
-        fp8 path (``site = (layer, index)``): xn is quantised to E4M3 with the site's delayed scale and multiplied with the E4M3
-        copy of W on the kind::f8f6f4 tensor-core path; the bf16 LoRA term shares the accumulator, so u is produced pre-divided
-        by the product scale s_x·s_w, which the epilogue multiplies back."""
-        g, r, M = fused.gemm, self.r, self.M_
-        drop = self.p > 0 and xd.shape[1] == G * K
-        if self.fp8 and site is not None:
-            l, s_i = site
-            x8 = self.x8_h if K == self.h else self.x8_f
-            if not prequant:  # the producer of xn did not emit the E4M3 copy itself
-                self.C.fp8_quantize_act(xn, x8, self.inv_sx[l, s_i:s_i + 1], self.act_state[l, s_i, 1:2])
-        if self.fp8 and site is not None and not self._fp8_calibrating:
-            g(xd, A, u, M=M, N=G * r, K1=K, n_per_group=r, a1_group_kofs=K if drop else 0, alpha=self.scale,
-              alpha_dev=self.alpha_inv[l, s_i:s_i + 1])
-            g(x8, self.W8[s_i][l], out, M=M, N=G * Ng, K1=K, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, residual=residual,
-              fp8=True, alpha_dev=self.alpha_main[l, s_i:s_i + 1])
-            return
-        g(xd, A, u, M=M, N=G * r, K1=K, n_per_group=r, a1_group_kofs=K if drop else 0, alpha=self.scale)
-        g(xn, W, out, M=M, N=G * Ng, K1=K, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, residual=residual)
-
     def _forward(self, train: bool):
         C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
         p = self.p if train else 0.0
@@ -455,93 +387,6 @@ class FusedLlamaStepper:
         x_last = self.x_in[self.L] if train else self.x_in[self.L % 2]
         C.rmsnorm_fwd(x_last, self.w_norm, self.xf, self.rstd_f, self.eps, None, None, [], 0.0)
         return x_last
-
-    def _loss_and_head_backward(self, train: bool):
-        """Chunked LM head + CE.  In training also dxf and dW_head (so logits never persist)."""
-        C, g, M, h, V = self.C, fused.gemm, self.M_, self.h, self.V
-        n_valid = self.B_ * (self.T_ - 1)
-        self.loss_sum.zero_()
-        self.count.zero_()
-        grad_scale = 1.0 / (n_valid * self.ga)
-        for s in range(0, M, self.ce_chunk):
-            m = min(self.ce_chunk, M - s)
-            hc = self.xf[s:s + m]
-            lg = self.logits[:m]
-            g(hc, self.W_head, lg, M=m, N=V, K1=h)
-            C.cross_entropy_fwd_bwd(lg, self.labels[s:s + m], V, grad_scale, -100, self.loss_sum, self.count)
-            if train:
-                g(lg, self.W_head, self.dxf[s:s + m], M=m, N=h, K1=V, b1_mn=True)
-                g(lg, hc, self.gW_head, M=V, N=h, K1=m, a1_mn=True, b1_mn=True, accumulate=True)
-        torch.div(self.loss_sum[0], float(n_valid), out=self.loss_out)
-
-    def _lora_group_bwd(self, dy, S_B, S_W, S_A, gA, gB, xd, u, keys, *, G, K, Ng, base_out, out, tag, site=None):
-        """Backward of one stacked LoRA group.  dy [M, G·Ng] -> out [M, K] (grad of the group's input).
-
-        The two weight-gradient GEMMs only read (dy, du, xd, u), so they are forked onto a side stream and fill the
-        SMs that the skinny du / parts GEMMs and kernel tails of the main chain leave idle; ``self._wg_done[tag]``
-        is the event the main stream waits on before it overwrites one of their inputs (see ``_backward``)."""
-        C, g, M, r, s = self.C, fused.gemm, self.M_, self.r, self.scale
-        du = self.du_bufs[tag]
-        # du_g = s · dy_g · B_g          (B stacked [G·Ng, r], read MN-major; K window g·Ng)
-        g(dy, S_B, du, M=M, N=G * r, K1=Ng, b1_mn=True, n_per_group=r, a1_group_kofs=Ng if G > 1 else 0,
-          b1_group_kofs=Ng if G > 1 else 0, b1_local_n=True, alpha=s)
-        drop = self.p > 0
-        shared_x = (not drop) or xd.shape[1] != G * K
-
-        def wgrads():  # fp32, accumulated across micro-batches, split-K over tokens
-            g(du, xd, gA, M=G * r, N=K, K1=M, a1_mn=True, b1_mn=True, accumulate=True, split_k=self.wgrad_split_k,
-              m_per_group=r if G > 1 else 0, b1_mn_ofs_per_mgroup=0 if shared_x else K)
-            # fp8 path: the saved u is u / (s_x·s_w); the product scale is multiplied back here
-            g(dy, u, gB, M=G * Ng, N=r, K1=M, a1_mn=True, b1_mn=True, accumulate=True, split_k=self.wgrad_split_k,
-              m_per_group=Ng if G > 1 else 0, b1_mn_ofs_per_mgroup=r if G > 1 else 0,
-              alpha_dev=self.alpha_main[site[0], site[1]:site[1] + 1] if (self.fp8 and site is not None) else None)
-
-        if self.side is not None:
-            fork = torch.cuda.Event()
-            fork.record()
-            self.side.wait_event(fork)
-            with torch.cuda.stream(self.side):
-                wgrads()
-                done = torch.cuda.Event()
-                done.record()
-            self._wg_done[tag] = done
-        if self.fused_dx:
-            sd, ks, pp = (self.seed, list(keys), self.p) if drop else (None, [0] * G, 0.0)
-            if G * Ng >= self.dx_split_k:
-                # long reductions: the frozen-path product runs on the 256-wide / CTA-pair GEMM (1.3-1.5x the per-FLOP rate of
-                # the 128-wide multi-accumulator tiles), then one light pass adds the masked low-rank terms
-                if self.fp8_bwd and site is not None:
-                    # E5M2 copy of the output gradient (delayed scale) x E4M3 copy of Wᵀ on the kind::f8f6f4 path
-                    l_, s_i = site
-                    dy8 = self.dy8[G * Ng]
-                    C.fp8_quantize_act(dy, dy8, self._inv_sx2[1, l_, s_i:s_i + 1], self._act_state2[1, l_, s_i, 1:2], True)
-                if self.fp8_bwd and site is not None and self._fp8_bwd_calibrated:
-                    g(dy8, self.W8T[s_i][l_], base_out, M=M, N=K, K1=G * Ng, fp8=2, alpha_dev=self._alpha_main2[1, l_, s_i:s_i + 1])
-                else:
-                    g(dy, S_W, base_out, M=M, N=K, K1=G * Ng, b1_mn=True)
-                C.lora_dx(None, None, du, S_A, out, sd, ks, pp, base_out)
-            else:
-                # one kernel: out = dy·W + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)  (masked LoRA terms folded into the register accumulator)
-                C.lora_dx(dy, S_W, du, S_A, out, sd, ks, pp)
-        else:
-            # frozen path: base = dy · W     (W stacked [G·Ng, K], read MN-major)
-            g(dy, S_W, base_out, M=M, N=K, K1=G * Ng, b1_mn=True)
-            # low-rank path per group: part_g = du_g · A_g
-            parts = self.parts.view(-1)[: M * G * K].view(M, G * K)
-            g(du, S_A, parts, M=M, N=G * K, K1=r, b1_mn=True, n_per_group=K, a1_group_kofs=r if G > 1 else 0,
-              b1_group_kofs=r if G > 1 else 0, b1_local_n=True)
-            if drop:
-                C.dropout_combine(base_out, parts, out, self.seed, keys, self.p)
-            else:
-                torch.add(base_out, parts.view(M, G, K).sum(1) if G > 1 else parts, out=out)
-        if self.side is None:
-            wgrads()
-
-    def _join(self, tag):
-        """Main stream waits for the side-stream weight gradients tagged ``tag`` (no-op if none are pending)."""
-        ev = self._wg_done.pop(tag, None)
-        if ev is not None:
-            torch.cuda.current_stream().wait_event(ev)
 
     def _backward(self):
         C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
@@ -609,8 +454,7 @@ class FusedLlamaStepper:
         self._fp8_calibrated = True
 
     def _micro_body(self):
-        self.labels.view(self.B_, self.T_)[:, :-1].copy_(self.ids[:, 1:])
-        self.labels.view(self.B_, self.T_)[:, -1].fill_(-100)
+        self._set_labels()
         if self.fp8:  # rotate the activation amax state, derive this micro-step's scales
             self.C.fp8_prep(self._act_state2, self._w_scale2, self._inv_sx2, self._alpha_main2, self._alpha_inv2, self.fp8_margin,
                             4 * self.L)
@@ -622,59 +466,11 @@ class FusedLlamaStepper:
         self.C.seed_advance(self.seed)
 
     # ------------------------------------------------------------------ public stepper interface
-    @torch.no_grad()
-    def micro_step(self, input_ids: torch.Tensor) -> torch.Tensor:
-        B, T = input_ids.shape
-        if self._shape != (B, T):
-            self._alloc(B, T)
-            self._graph = None
-        self.ids.copy_(input_ids, non_blocking=True)
+    def _before_micro(self):
         if self.fp8 and not self._fp8_calibrated:
             self._fp8_calibrate()
-        if not self.use_graphs:
-            self._micro_body()
-            return self.loss_out.clone()
-        if self._graph is None:
-            self._capture()
-        else:
-            self._graph.replay()
-            self._replays += 1
-        return self.loss_out.clone()
 
-    def _capture(self):
-        # warm-up (allocator, cuBLAS/flash workspaces, tensor-map cache) on a side stream, then capture
-        grads_backup = self.store.grads.clone()
-        seed_backup = self.seed.clone()
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            self._micro_body()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        self.store.grads.copy_(grads_backup)
-        self.seed.copy_(seed_backup)
-        n0 = self.C.launch_count()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            self._micro_body()
-        self._launches_per_micro = self.C.launch_count() - n0
-        # capture does not execute: run the captured work once for this micro-batch
-        self.store.grads.copy_(grads_backup)
-        self.seed.copy_(seed_backup)
-        del grads_backup
-        graph.replay()
-        self._replays += 1
-        self._graph = graph
-
-    @torch.no_grad()
-    def eval_loss(self, input_ids: torch.Tensor) -> torch.Tensor:
-        B, T = input_ids.shape
-        if self._shape != (B, T):
-            self._alloc(B, T)
-            self._graph = None
-        self.ids.copy_(input_ids)
-        self.labels.view(B, T)[:, :-1].copy_(self.ids[:, 1:])
-        self.labels.view(B, T)[:, -1].fill_(-100)
+    def _eval_body(self):
         if self.fp8 and not self._fp8_calibrated:
             # evaluation before the first training step: bootstrap the activation scales exactly like micro_step does
             self._fp8_calibrate()
@@ -682,74 +478,10 @@ class FusedLlamaStepper:
                             4 * self.L)
         self._forward(False)
         self._loss_and_head_backward(False)
-        return self.loss_out.clone()
-
-    @property
-    def folds_loss_reduce(self) -> bool:
-        """True when ``update(local_loss=...)`` combines loss / skip over ranks inside the NVLink kernel chain (no NCCL call)."""
-        return self.comm is not None
-
-    @torch.no_grad()
-    def update(self, skip: Optional[torch.Tensor] = None, error_if_nonfinite: bool = False,
-               local_loss: Optional[torch.Tensor] = None) -> UpdateInfo:
-        opt = self.optimizer
-        world = self.info.world_size
-        if self.comm is not None:
-            from .stepper import peer_memory_update
-
-            return peer_memory_update(self, grads_f32=self.store.grads, skip=skip, error_if_nonfinite=error_if_nonfinite,
-                                      local_loss=local_loss)
-        grads = None
-        if world > 1 and not self.sync.zero:
-            # NCCL baseline: gradients cross the wire as bf16 (like the reference's bf16 DDP buckets), once per update
-            if self._stage is None:
-                self._stage = torch.empty(self.store.numel, dtype=BF, device=self.device)
-            self.C.cast_f32_to_bf16(self.store.grads, self._stage, 1.0)
-            dist.all_reduce(self._stage, op=dist.ReduceOp.SUM)
-            grads = self._stage
-            sq = torch.zeros(1, dtype=torch.float32, device=self.device)
-            self.C.sumsq(grads, sq)
-            total = sq[0].sqrt() / world
-            coef = torch.clamp(self.clip / (total + 1e-6), max=1.0) if self.clip and self.clip > 0 else torch.ones_like(total)
-            coef = torch.where(torch.isfinite(total), coef, torch.full_like(coef, float("nan")))  # non-finite norm: skip the update
-            scale = coef / world
-        else:
-            self.sync.reduce()
-            total, scale = self.sync.grad_norm_and_scale(self.clip)
-        if error_if_nonfinite and not bool(torch.isfinite(total)):
-            raise RuntimeError(f"The total norm of order 2.0 for gradients is non-finite ({float(total)}), so it cannot be clipped.")
-        opt.step(grad_scale=scale, skip=skip, grads=grads)
-        self.sync.gather_params()
-        opt.zero_grad()
-        return UpdateInfo(total, False)
 
     @torch.no_grad()
     def merge_and_reinit(self):
         """W += s·B@A on the stacked buffers (wgmma GEMM accumulating into W in fp32), then hash re-init."""
-        from ..ops import reference as ref
-
-        g, r = fused.gemm, self.r
-        for S in self.layers:
-            for m, (Bm, Am, Wm) in zip(S.mods, S.merge):
-                g(Bm, Am, Wm, M=Wm.shape[0], N=Wm.shape[1], K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
-                sd = ref.mix_seed(self.model.seed, self.model.n_restarts, m.module_index)
-                self.C.fill_uniform_hash(m.lora_A.weight.data, sd, 1.0 / math.sqrt(m.in_features))
-                m.lora_B.weight.data.zero_()
-        self.model.n_restarts += 1
+        self._merge_modules([blk for S in self.layers for blk in zip(S.mods, S.merge)])
         if self.fp8:
             self._quantize_weights()
-
-    def launches_in_window(self, n_steps: int) -> int:
-        """Kernel launches of this extension since ``reset_launch_count`` (graph replays included)."""
-        return int(self.C.launch_count() + self._replays_since_reset() * self._launches_per_micro)
-
-    def _replays_since_reset(self) -> int:
-        return self._replays - getattr(self, "_replay_mark", 0)
-
-    def mark_launch_window(self):
-        self._replay_mark = self._replays
-        self.C.reset_launch_count()
-
-    def set_lr(self, lr: float) -> None:
-        for grp in self.optimizer.param_groups:
-            grp["lr"] = lr

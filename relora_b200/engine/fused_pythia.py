@@ -1,0 +1,397 @@
+"""Whole-model fused executor for Pythia (GPT-NeoX) + ReLoRA on H100.
+
+The Llama executor's design (:mod:`.fused_llama`) applied to the GPT-NeoX block:
+
+* every projection is ONE wgmma GEMM with the LoRA up-projection folded into the K loop and the bias (and, for ``dense`` and
+  ``dense_4h_to_h``, the residual) added in the epilogue: ``y = [x | s·xd·Aᵀ]·[W | B]ᵀ + b (+ residual)``;
+* one LayerNorm pass writes ``LN1(x)`` and, under parallel residual, ``LN2(x)`` from shared fp32 statistics, each with its LoRA-
+  dropout copy; the backward forms ``dx = dres + LN1ᵀ(dy1) + LN2ᵀ(dy2)`` in one pass together with the γ / β gradients and the
+  bias gradient of the projections whose output gradient ``dres`` is;
+* GELU writes the dropout copy of its output, its backward the bias gradient of ``dense_h_to_4h``; a column sum of ``dqkv`` is the
+  ``query_key_value`` bias gradient;
+* attention runs on the head-interleaved ``query_key_value`` output in place (wgmma kernels, or SDPA on strided views);
+* chunked LM head + CE, one flat fp32 gradient buffer, one CUDA graph per micro-batch (dropout seeds on the device).
+
+The frozen weights stay where the modules keep them; the trainable parameters (LoRA factors, biases, LayerNorms, embeddings) are
+views of the flat store, so checkpoints keep the HF GPT-NeoX keys.  Numerics tests compare this executor with the module path on
+identical weights and dropout masks.
+
+Parallel residual:   x_next = x + dense(attn(LN1 x)) + b_o + mlp(LN2 x) + b_4
+Sequential residual: x1 = x + dense(attn(LN1 x)) + b_o ;  x_next = x1 + mlp(LN2 x1) + b_4
+"""
+from __future__ import annotations
+
+import math
+import os
+from typing import List, Tuple
+
+import torch
+import torch.nn as nn
+import torch.nn.functional as F_
+
+from ..models.pythia import GPTNeoXForCausalLM
+from ..ops import fused
+from ..parallel.dist import DistInfo
+from ..parallel.grad_sync import broadcast_params
+from ..relora import ReLoRaModel
+from .fused_common import FusedStepperBase
+
+BF = torch.bfloat16
+MAX_HIDDEN = 2048  # the executor LayerNorm backward keeps its block partials of five [H] vectors in 48 KB of shared memory
+
+
+def supports(model, args=None) -> Tuple[bool, str]:
+    """(True, "ok") when the Pythia executor can train ``model``, else (False, why).  The configuration is checked before the device,
+    so the reason does not depend on where the model lives."""
+    if not isinstance(model, ReLoRaModel):
+        return False, "full-rank training uses the module path"
+    inner = model.wrapped_model
+    if not isinstance(inner, GPTNeoXForCausalLM):
+        return False, "not a GPT-NeoX (Pythia) model"
+    if model.lora_only or model.trainable_scaling or model._config.quantize is not None:
+        return False, "lora_only / trainable scaling / quantized frozen weights use the module path"
+    if args is not None and getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return False, "fp8 frozen weights are not supported for Pythia"
+    cfg = inner.config
+    if float(getattr(cfg, "hidden_dropout", 0.0)) != 0.0 or float(getattr(cfg, "attention_dropout", 0.0)) != 0.0:
+        return False, "hidden / attention dropout must be 0"
+    layer0 = inner.gpt_neox.layers[0]
+    if not isinstance(layer0.mlp.act, nn.GELU):
+        return False, "only the GELU activation is fused"
+    h, f, nh, r = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, model.r
+    if h % 128 or r % 128 or f % 128:
+        return False, f"hidden ({h}), intermediate ({f}) and rank ({r}) must be multiples of 128"
+    if h > MAX_HIDDEN:
+        return False, f"hidden ({h}) must be <= {MAX_HIDDEN} (LayerNorm kernel limit)"
+    hd = h // nh
+    if hd % 8:
+        return False, "head_dim must be a multiple of 8"
+    if layer0.attention.rotary_ndims % 2:
+        return False, "the number of rotary dims must be even"
+    at, mlp = layer0.attention, layer0.mlp
+    if any(m.bias is None for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)):
+        return False, "projections without bias use the module path"
+    p = next(inner.parameters())
+    if not p.is_cuda or p.dtype != BF:
+        return False, "needs CUDA + bfloat16"
+    return True, "ok"
+
+
+class _Layer:
+    """Views of one GPT-NeoX layer's parameters and gradients."""
+
+    __slots__ = ("W_qkv", "W_o", "W_h", "W_4", "A_qkv", "B_qkv", "b_qkv", "A_o", "B_o", "b_o", "A_h", "B_h", "b_h", "A_4", "B_4", "b_4",
+                 "w1", "c1", "w2", "c2", "gA_qkv", "gB_qkv", "gb_qkv", "gA_o", "gB_o", "gb_o", "gA_h", "gB_h", "gb_h", "gA_4", "gB_4",
+                 "gb_4", "gw1", "gc1", "gw2", "gc2", "key_qkv", "key_o", "key_h", "key_4", "mods")
+
+
+class FusedPythiaStepper(FusedStepperBase):
+    def __init__(self, model: ReLoRaModel, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
+                 weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
+                 transport: str = "nccl", native=None, symm_factory=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
+                 overlap_wgrad: bool = True, attention: str = "auto"):
+        ok, why = supports(model)
+        if not ok:
+            raise RuntimeError(why)
+        self.model, self.info = model, info
+        self.inner: GPTNeoXForCausalLM = model.wrapped_model
+        self.C = fused._C()
+        self.ga = grad_accumulation
+        self.clip = clip_grad_norm
+        self.use_graphs = cuda_graphs
+        self.ce_chunk = ce_chunk
+        cfg = self.inner.config
+        self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
+        self.hd = self.h // self.nh
+        self.r = model.r
+        self.L = cfg.num_hidden_layers
+        self.p = float(model.lora_dropout)
+        self.scale = float(model.lora_alpha) / model.r
+        self.device = info.device
+        self.fp8 = self.fp8_bwd = False
+        broadcast_params(model)
+        neox = self.inner.gpt_neox
+        layers = neox.layers
+        self.parallel = bool(layers[0].use_parallel_residual)
+        self.tanh = layers[0].mlp.act.approximate == "tanh"
+        self.eps = [(l.input_layernorm.eps, l.post_attention_layernorm.eps) for l in layers]
+        self.eps_f = neox.final_layer_norm.eps
+        at0 = layers[0].attention
+        self.rot = at0.rotary_ndims
+        self.rotary = at0.rotary_emb
+
+        # ---------------------------------------------------------------- flat trainable store
+        named: List[Tuple[str, torch.nn.Parameter]] = []
+        name_of = {id(p): n for n, p in model.named_parameters()}
+
+        def add(p):
+            named.append((name_of[id(p)], p))
+
+        for layer in layers:
+            at, mlp = layer.attention, layer.mlp
+            for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h):
+                add(m.lora_A.weight); add(m.lora_B.weight); add(m.bias)
+            for ln in (layer.input_layernorm, layer.post_attention_layernorm):
+                add(ln.weight); add(ln.bias)
+        add(neox.embed_in.weight)
+        add(neox.final_layer_norm.weight); add(neox.final_layer_norm.bias)
+        add(self.inner.embed_out.weight)
+        seen = {id(p) for _, p in named}
+        extra = [(n, p) for n, p in model.named_parameters() if p.requires_grad and id(p) not in seen]
+        if extra:
+            raise RuntimeError(f"unexpected trainable parameters for the fused executor: {[n for n, _ in extra]}")
+        self._init_transport(info, transport)
+        self._init_store(named)
+        pv = self._stacked_view
+
+        self.layers: List[_Layer] = []
+        for layer in layers:
+            at, mlp = layer.attention, layer.mlp
+            S = _Layer()
+            for tag, m in (("qkv", at.query_key_value), ("o", at.dense), ("h", mlp.dense_h_to_4h), ("4", mlp.dense_4h_to_h)):
+                setattr(S, "W_" + tag, m.weight.data)  # frozen weight, [out, in] contiguous as the module keeps it
+                A, gA = pv(m.lora_A.weight)
+                B, gB = pv(m.lora_B.weight)
+                b, gb = pv(m.bias)
+                for k, v in (("A_", A), ("gA_", gA), ("B_", B), ("gB_", gB), ("b_", b), ("gb_", gb)):
+                    setattr(S, k + tag, v)
+                setattr(S, "key_" + tag, m.module_index + 1)  # LoRA-dropout mask stream of the module path
+                assert A.data_ptr() == m.lora_A.weight.data_ptr() and b.data_ptr() == m.bias.data_ptr()
+            S.w1, S.gw1 = pv(layer.input_layernorm.weight)
+            S.c1, S.gc1 = pv(layer.input_layernorm.bias)
+            S.w2, S.gw2 = pv(layer.post_attention_layernorm.weight)
+            S.c2, S.gc2 = pv(layer.post_attention_layernorm.bias)
+            S.mods = (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)
+            self.layers.append(S)
+        self.W_emb, self.gW_emb = pv(neox.embed_in.weight)
+        self.w_norm, self.gw_norm = pv(neox.final_layer_norm.weight)
+        self.c_norm, self.gc_norm = pv(neox.final_layer_norm.bias)
+        self.W_head, self.gW_head = pv(self.inner.embed_out.weight)
+
+        # ---------------------------------------------------------------- optimizer / comm
+        self._init_optimizer(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, zero=zero, native=native)
+        self._attn_saved: List = []
+        attention = os.environ.get("RELORA_B200_ATTENTION", attention)
+        self.native_attn = fused.attention_backend(self.hd, attention) == "native"
+        if attention == "native" and not self.native_attn:
+            raise RuntimeError(f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM} (multiple of 8), "
+                               f"got {self.hd}")
+        self.side = torch.cuda.Stream(device=self.device) if overlap_wgrad else None
+        self.fused_dx = True
+        self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0")) or 4096
+        self.wgrad_split_k = 0
+        self.deterministic_embedding = os.environ.get("RELORA_B200_ATOMIC_EMBEDDING", "0") != "1"
+
+    # ------------------------------------------------------------------ buffers
+    def _alloc(self, B: int, T: int):
+        dev, h, f, r, L = self.device, self.h, self.f, self.r, self.L
+        M = B * T
+        e = lambda *s: torch.empty(*s, dtype=BF, device=dev)  # noqa: E731
+        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
+        self.B_, self.T_, self.M_ = B, T, M
+        self.ids = torch.zeros(B, T, dtype=torch.long, device=dev)
+        self.labels = torch.zeros(M, dtype=torch.long, device=dev)
+        # saved for the backward, one slot per layer ([0] only in evaluation)
+        self.x_in = e(L + 1, M, h)
+        self.mean1, self.rstd1 = f32(L, M), f32(L, M)
+        self.xd1, self.xd2 = e(L, M, h), e(L, M, h)  # LoRA inputs of query_key_value / dense_h_to_4h (the norms' outputs when p = 0)
+        self.qkv = e(L, M, 3 * h)                    # post-rotary, head-interleaved
+        self.xd_o = e(L, M, h)                       # attention output (dropout copy when p > 0): LoRA input of dense
+        self.z = e(L, M, f)                          # pre-GELU
+        self.xd_4 = e(L, M, f)                       # GELU output (dropout copy when p > 0): LoRA input of dense_4h_to_h
+        self.u_qkv, self.u_o, self.u_h, self.u_4 = e(L, M, r), e(L, M, r), e(L, M, r), e(L, M, r)
+        if not self.parallel:
+            self.x1 = e(L, M, h)
+            self.mean2, self.rstd2 = f32(L, M), f32(L, M)
+        if self.native_attn:
+            self.attn_o = e(L, M, h)
+            self.lse = f32(L, B, self.nh, T)
+            self.delta = f32(B, self.nh, T)
+        # transients
+        self.xn1, self.xn2, self.attn_t, self.x1_t = e(M, h), e(M, h), e(M, h), e(M, h)
+        self.a = e(M, f)
+        self.mean_f, self.rstd_f = f32(M), f32(M)
+        self.xf, self.dxf = e(M, h), e(M, h)
+        self.dx_a, self.dx_b, self.dxn1, self.dxn2, self.dattn, self.tmp_h = e(M, h), e(M, h), e(M, h), e(M, h), e(M, h), e(M, h)
+        self.dqkv = e(M, 3 * h)
+        self.da, self.dz, self.tmp_f = e(M, f), e(M, f), e(M, f)
+        self.du_bufs = {"4": e(M, r), "h": e(M, r), "o": e(M, r), "qkv": e(M, r)}
+        ldv = (self.V + 7) // 8 * 8
+        self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
+        self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.count = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
+        # rotary tables of the module (linear / dynamic-NTK scaling, T beyond max_position_embeddings), fp32 [T, rot]
+        if self.rot > 0:
+            cos, sin = self.rotary(self.x_in, seq_len=T)
+            self.cos = cos[0, 0, :T].float().contiguous()
+            self.sin = sin[0, 0, :T].float().contiguous()
+        self._shape = (B, T)
+
+    # ------------------------------------------------------------------ forward
+    def _attention(self, qkv: torch.Tensor, train: bool, sl: int, out: torch.Tensor):
+        B, T, nh, hd = self.B_, self.T_, self.nh, self.hd
+        if self.native_attn:
+            self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd), interleaved=True)
+            return out
+        v5 = qkv.view(B, T, nh, 3, hd)
+        q, k, v = (v5[:, :, :, i].transpose(1, 2) for i in range(3))
+        if train:
+            q, k, v = (t.detach().requires_grad_() for t in (q, k, v))
+            with torch.enable_grad():
+                o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True)
+            self._attn_saved.append((o, q, k, v))
+        else:
+            o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True)
+        out.view(B, T, nh, hd).copy_(o.detach().transpose(1, 2))
+        return out
+
+    def _norms(self, x, S, l, sl, train, p, both: bool, second_of=None):
+        """LN1(x) (and LN2(x) when ``both``) or, with ``second_of``, LN2 of that input alone; returns the normed outputs and the LoRA
+        inputs (dropout copies in training with p > 0)."""
+        C, seed = self.C, self.seed
+        keep = train and self.p == 0  # the normed output itself is the saved LoRA input
+        outs = []
+        specs = [(S.w2, S.c2, self.xd2, self.xn2, S.key_h)] if second_of is not None else \
+            [(S.w1, S.c1, self.xd1, self.xn1, S.key_qkv)] + ([(S.w2, S.c2, self.xd2, self.xn2, S.key_h)] if both else [])
+        for w, c, xd_buf, xn_t, key in specs:
+            xn = xd_buf[sl] if keep else xn_t
+            xd = xd_buf[sl] if (train and p > 0) else None
+            outs.append((w, c, xn, xd, key))
+        if second_of is not None:
+            mean, rstd, eps = self.mean2[sl], self.rstd2[sl], self.eps[l][1]
+        else:
+            mean, rstd, eps = self.mean1[sl], self.rstd1[sl], self.eps[l][0]
+        (w1, c1, y1, d1, k1) = outs[0]
+        kw = {}
+        if len(outs) == 2:
+            (w2, c2, y2, d2, k2) = outs[1]
+            kw = dict(w2=w2, b2=c2, y2=y2, xd2=d2)
+        else:
+            k2, d2 = 0, None
+        if d1 is not None or d2 is not None:
+            kw.update(xd=d1, seed=seed, keys=[k1, k2], p=p)
+        C.layernorm_fwd(x, w1, c1, y1, mean, rstd, eps, **kw)
+        return [(o[2], o[3] if o[3] is not None else o[2]) for o in outs]
+
+    def _forward(self, train: bool):
+        C, M, h, f = self.C, self.M_, self.h, self.f
+        p = self.p if train else 0.0
+        seed = self.seed
+        C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
+        self._attn_saved.clear()
+        for l, S in enumerate(self.layers):
+            sl = l if train else 0
+            x = self.x_in[l] if train else self.x_in[l % 2]
+            x_next = self.x_in[l + 1] if train else self.x_in[(l + 1) % 2]
+            qkv = self.qkv[sl]
+            normed = self._norms(x, S, l, sl, train, p, both=self.parallel)
+            xn1, xd1 = normed[0]
+            # ---- attention: qkv = [xn1 | u]·[W | B]ᵀ + b, rotary in place, attention on the interleaved layout
+            self._lora_group_fwd(xn1, xd1, S.A_qkv, S.B_qkv, S.W_qkv, self.u_qkv[sl], qkv, G=1, K=h, Ng=3 * h, bias=S.b_qkv)
+            if self.rot > 0:
+                C.neox_rope(qkv, self.T_, self.nh, self.hd, self.rot, self.cos, self.sin, 0, False)
+            attn = self._attention(qkv, train, sl, self.attn_o[sl] if self.native_attn else (self.xd_o[sl] if train and self.p == 0 else self.attn_t))
+            if p > 0:
+                xd_o = self.xd_o[sl]
+                C.dropout_expand(attn, xd_o, seed, [S.key_o], p)
+            else:
+                xd_o = attn
+                if train and attn.data_ptr() != self.xd_o[sl].data_ptr():
+                    self.xd_o[sl].copy_(attn)
+            x1 = self.x1[sl] if (train and not self.parallel) else self.x1_t
+            self._lora_group_fwd(attn, xd_o, S.A_o, S.B_o, S.W_o, self.u_o[sl], x1, G=1, K=h, Ng=h, residual=x, bias=S.b_o)
+            # ---- MLP: z = [xn2 | u]·[W | B]ᵀ + b, GELU (+ dropout copy), x_next = [a | u]·[W | B]ᵀ + b + x1
+            if self.parallel:
+                xn2, xd2 = normed[1]
+            else:
+                xn2, xd2 = self._norms(x1, S, l, sl, train, p, both=False, second_of=x1)[0]
+            z = self.z[sl]
+            self._lora_group_fwd(xn2, xd2, S.A_h, S.B_h, S.W_h, self.u_h[sl], z, G=1, K=h, Ng=f, bias=S.b_h)
+            a = self.xd_4[sl] if (train and self.p == 0) else self.a
+            if p > 0:
+                xd_4 = self.xd_4[sl]
+                C.gelu_fwd(z, a, self.tanh, xd=xd_4, seed=seed, key=S.key_4, p=p)
+            else:
+                C.gelu_fwd(z, a, self.tanh)
+                xd_4 = a
+            self._lora_group_fwd(a, xd_4, S.A_4, S.B_4, S.W_4, self.u_4[sl], x_next, G=1, K=f, Ng=h, residual=x1, bias=S.b_4)
+        x_last = self.x_in[self.L] if train else self.x_in[self.L % 2]
+        C.layernorm_fwd(x_last, self.w_norm, self.c_norm, self.xf, self.mean_f, self.rstd_f, self.eps_f)
+        return x_last
+
+    # ------------------------------------------------------------------ backward
+    def _backward(self):
+        C, h, f = self.C, self.h, self.f
+        B, T, nh, hd = self.B_, self.T_, self.nh, self.hd
+        dx, dx_other = self.dx_a, self.dx_b
+        C.layernorm_bwd(self.dxf, self.x_in[self.L], self.w_norm, self.mean_f, self.rstd_f, dx, self.gw_norm, self.gc_norm)
+        for l in range(self.L - 1, -1, -1):
+            S = self.layers[l]
+            # ---- MLP: x_next = a·W_4ᵀ + u_4·B_4ᵀ + b_4 + x1   (output gradient dx)
+            self._lora_group_bwd(dx, S.B_4, S.W_4, S.A_4, S.gA_4, S.gB_4, self.xd_4[l], self.u_4[l], [S.key_4],
+                                 G=1, K=f, Ng=h, base_out=self.tmp_f, out=self.da, tag="4")
+            self._join("h")  # the previous layer's dense_h_to_4h weight gradients read dz / du
+            C.gelu_bwd(self.da, self.z[l], self.dz, self.tanh, dbias=S.gb_h)
+            self._lora_group_bwd(self.dz, S.B_h, S.W_h, S.A_h, S.gA_h, S.gB_h, self.xd2[l], self.u_h[l], [S.key_h],
+                                 G=1, K=h, Ng=f, base_out=self.tmp_h, out=self.dxn2, tag="h")
+            if self.parallel:
+                d_attn_out = dx  # dense's output gradient is the block's
+            else:
+                # x_next = x1 + mlp(LN2 x1) + b_4:  dx1 = dx + LN2ᵀ(dxn2); Σ dx is the bias gradient of dense_4h_to_h
+                C.layernorm_bwd(self.dxn2, self.x1[l], S.w2, self.mean2[l], self.rstd2[l], dx_other, S.gw2, S.gc2, dres=dx,
+                                dres_sum=S.gb_4)
+                dx, dx_other = dx_other, dx
+                d_attn_out = dx
+            # ---- attention: x1 = attn·W_oᵀ + u_o·B_oᵀ + b_o + x
+            self._lora_group_bwd(d_attn_out, S.B_o, S.W_o, S.A_o, S.gA_o, S.gB_o, self.xd_o[l], self.u_o[l], [S.key_o],
+                                 G=1, K=h, Ng=h, base_out=self.tmp_h, out=self.dattn, tag="o")
+            if self.native_attn:
+                self._join("qkv")  # the previous layer's query_key_value weight gradients read dqkv / du
+                C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
+                                1.0 / math.sqrt(hd), interleaved=True)
+            else:
+                o, q, k, v = self._attn_saved[l]
+                dq, dk, dv = torch.autograd.grad(o, (q, k, v), self.dattn.view(B, T, nh, hd).transpose(1, 2))
+                self._join("qkv")
+                d5 = self.dqkv.view(B, T, nh, 3, hd)
+                for i, d in enumerate((dq, dk, dv)):
+                    d5[:, :, :, i].copy_(d.transpose(1, 2))
+            if self.rot > 0:
+                C.neox_rope(self.dqkv, T, nh, hd, self.rot, self.cos, self.sin, 0, True)  # back through the rotation of q, k
+            C.colsum(self.dqkv, S.gb_qkv)
+            self._lora_group_bwd(self.dqkv, S.B_qkv, S.W_qkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd1[l], self.u_qkv[l], [S.key_qkv],
+                                 G=1, K=h, Ng=3 * h, base_out=self.tmp_h, out=self.dxn1, tag="qkv")
+            self._join("o")  # this layer's dense / dense_4h_to_h weight gradients read the buffer written next
+            if self.parallel:
+                # dx = dx_next + LN1ᵀ(dxn1) + LN2ᵀ(dxn2); Σ dx_next is the bias gradient of both dense and dense_4h_to_h
+                C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[l], self.rstd1[l], dx_other, S.gw1, S.gc1, dres=dx,
+                                dy2=self.dxn2, w2=S.w2, dw2=S.gw2, db2=S.gc2, dres_sum=S.gb_o, dres_sum2=S.gb_4)
+            else:
+                C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[l], self.rstd1[l], dx_other, S.gw1, S.gc1, dres=dx,
+                                dres_sum=S.gb_o)
+            dx, dx_other = dx_other, dx
+        if self.deterministic_embedding:
+            sorted_ids, perm = torch.sort(self.ids.view(-1), stable=True)
+            C.embedding_bwd_sorted(sorted_ids, perm, dx, self.gW_emb, -1)
+        else:
+            C.embedding_bwd(self.ids.view(-1), dx, self.gW_emb, -1)
+        for tag in ("4", "h", "o", "qkv"):
+            self._join(tag)
+        self._attn_saved.clear()
+
+    def _micro_body(self):
+        self._set_labels()
+        self._forward(True)
+        self._loss_and_head_backward(True)
+        self._backward()
+        self.C.seed_advance(self.seed)
+
+    def _eval_body(self):
+        self._forward(False)
+        self._loss_and_head_backward(False)
+
+    @torch.no_grad()
+    def merge_and_reinit(self):
+        """W += s·B@A per module (wgmma GEMM accumulating into W in fp32), then the hash re-init of the module path."""
+        self._merge_modules([(m, (m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data)) for S in self.layers for m in S.mods])

@@ -9,7 +9,8 @@ transport and exposes two calls:
 This mirrors one iteration of the reference hot loop (``torchrun_main.py:783-826``) with the
 gradient all-reduce hoisted out of the accumulation loop.  :class:`ModuleStepper` drives any
 ``nn.Module`` whose forward returns ``.loss`` (CPU/gloo and the generic GPU path);
-:class:`relora_b200.engine.fused_llama.FusedLlamaStepper` is the H100 executor (whole-layer fused
+:class:`relora_b200.engine.fused_llama.FusedLlamaStepper` and
+:class:`relora_b200.engine.fused_pythia.FusedPythiaStepper` are the H100 executors (whole-layer fused
 kernels, CUDA graphs) with the same interface.
 """
 from __future__ import annotations
@@ -198,7 +199,16 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
                                      fp8_backward=getattr(args, "frozen_dtype", None) == "fp8_full",
                                      deterministic=bool(getattr(args, "deterministic", False)), **kw)
         if engine == "fused":
-            raise RuntimeError(f"--engine fused requested but not applicable: {why}")
+            # Pythia (GPT-NeoX) has its own executor; `auto` keeps it on the module path
+            from ..models.pythia import GPTNeoXForCausalLM
+            from .fused_pythia import FusedPythiaStepper, supports as pythia_supports
+
+            ok, why_p = pythia_supports(model, args)
+            if ok:
+                return FusedPythiaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
+                                          attention=getattr(args, "attention", "auto"), **kw)
+            inner = getattr(model, "wrapped_model", model)
+            raise RuntimeError(f"--engine fused requested but not applicable: {why_p if isinstance(inner, GPTNeoXForCausalLM) else why}")
     if info.device.type != "cuda":
         kw["transport"] = "nccl"  # CPU: the process group's own reduction (gloo)
     # the fp8 tensor-core path and the wgmma attention kernels belong to the fused executor: say so instead of silently
