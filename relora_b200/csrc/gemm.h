@@ -20,7 +20,8 @@ struct Operand {
 // K-window of A1 starts at g*a1_group_kofs and the K-window of A2 at g*a2_group_kofs (B rows are the output
 // columns themselves).  With a2_group_kofs = r this evaluates, per group,
 //     y_g = x · W_gᵀ + u_g · B_gᵀ        (u = [u_0 | u_1 | ...] holds the down-projections side by side)
-// in one pass over x and one write of y.
+// in one pass over x and one write of y.  When both A1 and B1 take per-group K windows, K1 must be a multiple of the
+// k-block (64 elements, fp8: 128).
 struct GemmDesc {
   Operand a1, b1, a2, b2;
   int M = 0, N = 0, K1 = 0, K2 = 0;
@@ -35,6 +36,7 @@ struct GemmDesc {
   long long ldc = 0;
   bool out_f32 = false;     // output dtype: bf16 (default) or fp32
   bool accumulate = false;  // out += result (fp32 outputs: gradient accumulation)
+  // residual and bias: bf16 outputs only (refused with an fp32 output)
   const void* residual = nullptr;  // bf16 [M, N], added in fp32 before rounding
   long long ldr = 0;
   const void* bias = nullptr;      // bf16 [N], added in fp32 (after alpha, before the residual)

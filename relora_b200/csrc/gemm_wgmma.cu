@@ -564,6 +564,7 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   p.out = d.out; p.ldc = d.ldc; p.residual = reinterpret_cast<const bf16*>(d.residual); p.ldr = d.ldr;
   p.bias = reinterpret_cast<const bf16*>(d.bias);
   if (d.bias != nullptr && d.out_f32) throw std::runtime_error("gemm: bias is only fused for bf16 outputs");
+  if (d.residual != nullptr && d.out_f32) throw std::runtime_error("gemm: residual is only fused for bf16 outputs");
   p.alpha = d.alpha; p.alpha_dev = d.alpha_dev; p.fp8 = d.fp8 ? (d.fp8_a_e5m2 ? 2 : 1) : 0; p.out_f32 = d.out_f32 ? 1 : 0; p.accumulate = d.accumulate ? 1 : 0;
   p.num_m_tiles = ceil_div(d.M, BLOCK_M);
   const int groups = ceil_div(d.N, p.n_per_group);
@@ -571,6 +572,11 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   if (groups > 1 && (p.n_per_group % 64) != 0) throw std::runtime_error("gemm: n_per_group must be a multiple of 64");
   p.tiles_per_group = ceil_div(p.n_per_group, BLOCK_N);
   p.num_n_tiles = groups * p.tiles_per_group;
+  // The last k-block of a K window narrower than a whole number of k-blocks runs into the next group's window, which lies
+  // inside the tensor map, so TMA does not zero-fill it.  With only one of A1 / B1 windowed the other one's map ends at K1 and
+  // the overhang multiplies zeros; with both windowed it would add the next group's terms.
+  if (groups > 1 && d.a1_group_kofs != 0 && d.b1_group_kofs != 0 && d.K1 % (d.fp8 ? 2 * BLOCK_K : BLOCK_K) != 0)
+    throw std::runtime_error("gemm: with per-group K windows on both A1 and B1, K1 must be a multiple of the k-block (64, fp8: 128)");
 
   // K extents of the global tensors include the per-group windows
   const long long a1_k_total = (long long)d.K1 + (long long)(groups - 1) * d.a1_group_kofs;

@@ -188,6 +188,186 @@ def adamw_step(
     exp_avg_sq.copy_(v.to(exp_avg_sq.dtype))
 
 
+# ----------------------------------------------------------------------------- wgmma GEMM (csrc/gemm.h)
+# fp64 evaluations of the GemmDesc / LoraDxDesc contracts, written from their documentation.  Each returns the exact result and
+# an element-wise magnitude bound (sum of |terms|) that scales the accumulation-error tolerance of assert_gemm_close.
+_F64 = torch.float64
+
+# Accumulation-error coefficients of assert_gemm_close, as a fraction of the element's magnitude bound.  Set from the worst
+# element observed on an H100 80GB HBM3 (sm_90a wgmma) over the mode sweep in tests/test_gemm_modes_gpu.py, with headroom:
+# |err| / bound of fp32 outputs reached 2.0e-7 for bf16 operands (split-K atomics included) and 3.2e-4 for fp8 operands, whose
+# tensor-core path accumulates with fewer mantissa bits.
+GEMM_C_ACC_BF16 = 2.0 ** -16
+GEMM_C_ACC_FP8 = 2.0 ** -10
+
+
+def _window(t: torch.Tensor, r0: int, nr: int, c0: int, nc: int, what: str) -> torch.Tensor:
+    """``t[r0:r0+nr, c0:c0+nc]``; a window that leaves the operand is an error, not a silent truncation."""
+    if r0 < 0 or c0 < 0 or r0 + nr > t.shape[0] or c0 + nc > t.shape[1]:
+        raise IndexError(f"{what}: window rows [{r0}, {r0 + nr}) x cols [{c0}, {c0 + nc}) outside the {tuple(t.shape)} operand")
+    return t[r0:r0 + nr, c0:c0 + nc]
+
+
+def _gemm_operand(t: torch.Tensor, mn_major: bool, fp8_dtype=None) -> torch.Tensor:
+    """fp64 ``[rows, K]`` view of an operand: K-major element (i, k) is ``t[i, k]``, MN-major it is ``t[k, i]``."""
+    if fp8_dtype is not None:
+        t = t.view(fp8_dtype)
+    t = t.to(_F64)
+    return t.t() if mn_major else t
+
+
+def gemm_ref(
+    a1: torch.Tensor,
+    b1: torch.Tensor,
+    out: Optional[torch.Tensor] = None,
+    *,
+    M: Optional[int] = None,
+    N: Optional[int] = None,
+    K1: Optional[int] = None,
+    a2: Optional[torch.Tensor] = None,
+    b2: Optional[torch.Tensor] = None,
+    K2: int = 0,
+    a1_mn: bool = False,
+    b1_mn: bool = False,
+    n_per_group: int = 0,
+    a1_group_kofs: int = 0,
+    a2_group_kofs: int = 0,
+    residual: Optional[torch.Tensor] = None,
+    alpha: float = 1.0,
+    accumulate: bool = False,
+    out_dtype: torch.dtype = torch.bfloat16,
+    block_n: int = 0,
+    split_k: int = 1,
+    b1_group_kofs: int = 0,
+    b1_local_n: bool = False,
+    m_per_group: int = 0,
+    b1_mn_ofs_per_mgroup: int = 0,
+    bias: Optional[torch.Tensor] = None,
+    pair: int = -1,
+    fp8: int = 0,
+    alpha_dev: Optional[torch.Tensor] = None,
+) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp64 ``(result, bound)`` of :func:`relora_b200.ops.fused.gemm` called with the same arguments (``out``: its content
+    before the call; read only when ``accumulate`` is set, otherwise only its dtype matters).
+
+    Per output element (m, n), with n in column group g = n // n_per_group and local column nl = n - g·n_per_group:
+
+        D = alpha·alpha_dev · ( Σ_k A1[m, g·a1_group_kofs + k] · B1[j, g·b1_group_kofs + k]      (k < K1)
+                              + Σ_k A2[m, g·a2_group_kofs + k] · B2[n, k] )                    (k < K2)
+        j = (nl if b1_local_n else n) + (m // m_per_group) · b1_mn_ofs_per_mgroup
+
+    bf16 output: out = D + bias[n] + residual[m, n] (+ out if accumulate), rounded once; fp32 output: out = D (+ out).
+    ``fp8``: A1 / B1 are one-byte tensors decoded as E4M3 (A1 as E5M2 with ``fp8=2``).  ``block_n``, ``split_k`` and
+    ``pair`` choose the schedule and do not change the result.  ``bound`` is the same sum over |terms|."""
+    if M is None:
+        M = a1.shape[1] if a1_mn else a1.shape[0]
+    if K1 is None:
+        K1 = a1.shape[0] if a1_mn else a1.shape[1]
+    if N is None:
+        N = b1.shape[1] if b1_mn else b1.shape[0]
+    if a2 is not None and K2 == 0:
+        K2 = b2.shape[1]
+    odt = out.dtype if out is not None else out_dtype
+    if odt == torch.float32 and (bias is not None or residual is not None):
+        raise ValueError("gemm: bias and residual are only fused for bf16 outputs")
+    if accumulate and out is None:
+        raise ValueError("gemm: accumulate needs the previous output")
+    f8a = (torch.float8_e5m2 if fp8 == 2 else torch.float8_e4m3fn) if fp8 else None
+    A1 = _gemm_operand(a1, a1_mn, f8a)
+    B1 = _gemm_operand(b1, b1_mn, torch.float8_e4m3fn if fp8 else None)
+    A2 = _gemm_operand(a2, False) if K2 > 0 else None
+    B2 = _gemm_operand(b2, False) if K2 > 0 else None
+    npg = n_per_group if n_per_group > 0 else N
+    mpg = m_per_group if m_per_group > 0 else M
+    ref = torch.zeros(M, N, dtype=_F64, device=a1.device)
+    bound = torch.zeros_like(ref)
+    for g in range((N + npg - 1) // npg):
+        n0, nw = g * npg, min(npg, N - g * npg)
+        for m0 in range(0, M, mpg):
+            mw = min(mpg, M - m0)
+            j0 = (0 if b1_local_n else n0) + (m0 // mpg) * b1_mn_ofs_per_mgroup
+            a = _window(A1, m0, mw, g * a1_group_kofs, K1, "A1")
+            b = _window(B1, j0, nw, g * b1_group_kofs, K1, "B1")
+            ref[m0:m0 + mw, n0:n0 + nw] += a @ b.t()
+            bound[m0:m0 + mw, n0:n0 + nw] += a.abs() @ b.abs().t()
+        if K2 > 0:
+            a = _window(A2, 0, M, g * a2_group_kofs, K2, "A2")
+            b = _window(B2, n0, nw, 0, K2, "B2")
+            ref[:, n0:n0 + nw] += a @ b.t()
+            bound[:, n0:n0 + nw] += a.abs() @ b.abs().t()
+    scale = float(alpha) * (float(alpha_dev.reshape(-1)[0]) if alpha_dev is not None else 1.0)
+    ref *= scale
+    bound *= abs(scale)
+    for extra in (None if bias is None else bias.reshape(-1)[:N].to(_F64).expand(M, N),
+                  None if residual is None else residual[:M, :N].to(_F64),
+                  out[:M, :N].to(_F64) if accumulate else None):
+        if extra is not None:
+            ref += extra
+            bound += extra.abs()
+    return ref, bound
+
+
+def lora_dx_ref(dy, w, du: torch.Tensor, a: torch.Tensor, seed, keys, p: float, base: Optional[torch.Tensor] = None):
+    """fp64 ``(result, bound)`` of the extension's ``lora_dx(dy, w, du, a, out, seed, keys, p, base)``:
+
+        out = dy·W + 1/(1-p) · Σ_g keep_g ⊙ (du_g·A_g),    keep_g = dropout_keep_mask(mix_seed(seed, keys[g]), M, N, p)
+
+    with ``du = [du_0 | du_1 | ...]`` ([M, G·r]) and ``A = [A_0; A_1; ...]`` ([G·r, N]); with ``base`` given (the ``Kb == 0``
+    form) ``base`` replaces dy·W.  ``seed``: the device seed tensor or an int (None reads as 0)."""
+    G = len(keys)
+    M, N = du.shape[0], a.shape[1]
+    r = du.shape[1] // G
+    s = 0 if seed is None else (int(seed.reshape(-1)[0].item()) if torch.is_tensor(seed) else int(seed)) & _M32
+    ref = torch.zeros(M, N, dtype=_F64, device=du.device)
+    bound = torch.zeros_like(ref)
+    for g in range(G):
+        x, y = du[:, g * r:(g + 1) * r].to(_F64), a[g * r:(g + 1) * r].to(_F64)
+        part, pb = x @ y, x.abs() @ y.abs()
+        if p > 0:
+            keep = dropout_keep_mask(mix_seed(s, keys[g]), M, N, p, device=du.device)
+            part, pb = part * keep, pb * keep
+        ref += part
+        bound += pb
+    inv_keep = 1.0 / (1.0 - p)
+    ref *= inv_keep
+    bound *= inv_keep
+    if base is not None:
+        ref += base[:M, :N].to(_F64)
+        bound += base[:M, :N].to(_F64).abs()
+    else:
+        x, y = dy.to(_F64), w.to(_F64)
+        ref += x @ y
+        bound += x.abs() @ y.abs()
+    return ref, bound
+
+
+def assert_gemm_close(out: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, *, fp8: bool = False) -> float:
+    """Element-wise check of a GEMM output against :func:`gemm_ref` / :func:`lora_dx_ref`:
+
+        |out - ref| <= c_out·|ref| + c_acc·bound
+
+    ``c_out`` is the output rounding (2⁻⁸ for bf16, 2⁻²³ for fp32), ``c_acc`` the accumulation error per unit of the
+    magnitude bound (:data:`GEMM_C_ACC_BF16`, or :data:`GEMM_C_ACC_FP8` for the fp8 tensor-core path).  A NaN fails.
+    Returns the worst ratio of error to tolerance (<= 1 when it passes); the failure message names where it occurs."""
+    M, N = ref.shape
+    o = out[:M, :N].to(_F64)
+    c_out = 2.0 ** -8 if out.dtype == torch.bfloat16 else 2.0 ** -23
+    c_acc = GEMM_C_ACC_FP8 if fp8 else GEMM_C_ACC_BF16
+    err = (o - ref).abs()
+    tol = c_out * ref.abs() + c_acc * bound
+    ratio = torch.where(tol > 0, err / tol.clamp(min=1e-300), torch.where(err == 0, 0.0, math.inf))
+    ratio = torch.nan_to_num(ratio, nan=math.inf, posinf=math.inf)
+    flat = int(torch.argmax(ratio))
+    i, j = divmod(flat, N)
+    worst = float(ratio[i, j])
+    if not worst <= 1.0:
+        n_bad = int((ratio > 1.0).sum())
+        raise AssertionError(
+            f"GEMM output out of tolerance at {n_bad} of {M * N} elements; worst ratio {worst:.3g} at (row {i}, col {j}): "
+            f"out={float(o[i, j]):.6g} ref={float(ref[i, j]):.6g} bound={float(bound[i, j]):.6g} (c_out={c_out:.3g}, c_acc={c_acc:.3g})")
+    return worst
+
+
 # ----------------------------------------------------------------------------- merge
 def merge_delta(weight: torch.Tensor, lora_a: torch.Tensor, lora_b: torch.Tensor, scale: float) -> torch.Tensor:
     """W + s·B@A accumulated in fp32, rounded to ``weight.dtype`` (reference relora.py:275-276)."""
