@@ -6,7 +6,8 @@ Every launch of this repo's extension inside one micro-step (+ the optimizer upd
 (GEMM shape / operand majors / grouping, or the elementwise kernel's name), timed by the CUDA profiler (kineto kernel
 durations, no graph, launches matched to tags by order) and compared against its roofline:
 
-    t_min = max(flops / bf16_peak, bytes / hbm_bw)      (MEASURED_PEAKS.json; fallbacks 1590 TFLOP/s, 6.5 TB/s)
+    t_min = max(flops / bf16_peak, bytes / hbm_bw)      (MEASURED_PEAKS.json; fallbacks: H100 SXM data sheet,
+                                                           989 TFLOP/s dense BF16, 3.35 TB/s HBM3)
 
 ``bytes`` is the compulsory traffic (each operand once); ``frac`` = t_min / t_measured.  Library kernels (cuDNN
 attention) are listed with their measured time only.
@@ -33,9 +34,9 @@ from relora_b200.parallel.dist import DistInfo  # noqa: E402
 def peaks():
     try:
         d = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return float(d.get("bf16_tflops", 1590.0)) * 1e12, float(d.get("hbm_gbs", 6500.0)) * 1e9
+        return float(d.get("bf16_tflops", 989.0)) * 1e12, float(d.get("hbm_gbs", 3350.0)) * 1e9
     except Exception:
-        return 1590e12, 6500e9
+        return 989e12, 3350e9
 
 
 def tensor_bytes(args, kwargs):

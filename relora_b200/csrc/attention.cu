@@ -16,8 +16,8 @@
 // K = 16 steps that hold data when the head spans several panels; products that produce head_dim columns run one
 // register-A wgmma chain per panel, and the padded columns of the last panel are computed but never stored.  The
 // probabilities / score gradients never leave registers: the accumulator fragment of one wgmma is, packed to bf16, the register A operand of the next.  The streamed
-// operand pair is double buffered.  Each consumer issues one k-block of wgmma and waits for it before the dependent math;
-// the overlap this forgoes has not been measured on the H100.
+// operand pair is double buffered.  Each product (or the pair of independent products S, dP) is issued as one wgmma batch,
+// and the warpgroup waits for it only where softmax or the next product reads the result.
 //
 // Register budget.  The output accumulators take 32 fp32 registers per panel per thread, on top of the two 32-register
 // score fragments of the backward kernels.  Where the whole head does not fit one warpgroup without spilling (dQ at NP = 4,
@@ -70,28 +70,52 @@ __device__ __forceinline__ void frag_to_a(const float (&d)[32], int kk, uint32_t
   a[2] = pack_bf16x2(d[8 * kk + 4], d[8 * kk + 5]);
   a[3] = pack_bf16x2(d[8 * kk + 6], d[8 * kk + 7]);
 }
+template <int NSTEPS>
+__device__ __forceinline__ void mma_steps_kk(float (&d)[32], uint32_t a, uint32_t b) {
+#pragma unroll
+  for (int ks = 0; ks < NSTEPS; ++ks) {
+    const uint32_t ofs = (ks >> 2) * kPanel + (ks & 3) * 32;
+    wgmma_bf16_ss_n64<0, 0>(d, desc_kmajor(a + ofs), desc_kmajor(b + ofs));
+  }
+}
 // d += A · Bᵀ with A, B both [64 x 64·NP] K-major tiles (reduction over head_dim); only the first nks K = 16 steps hold data.
-// A single-panel head issues all four steps unconditionally (zero-filled columns add nothing), which keeps the head_dim <= 64
-// kernels free of the per-step branches.
+// A single-panel head issues all four steps unconditionally (zero-filled columns add nothing).  Wider heads pick the step
+// count with one uniform branch into straight-line runs: a wgmma under a condition of its own makes ptxas serialise every
+// wgmma of the batch.
 template <int NP>
 __device__ __forceinline__ void mma_tiles_kk(float (&d)[32], uint32_t a, uint32_t b, int nks) {
+  if constexpr (NP == 1) {
+    mma_steps_kk<4>(d, a, b);
+  } else {
+    switch (nks - 4 * (NP - 1)) {
+      case 1: mma_steps_kk<4 * NP - 3>(d, a, b); break;
+      case 2: mma_steps_kk<4 * NP - 2>(d, a, b); break;
+      case 3: mma_steps_kk<4 * NP - 1>(d, a, b); break;
+      default: mma_steps_kk<4 * NP>(d, a, b); break;
+    }
+  }
+}
+// P (rows x 64, an accumulator fragment) as the register A operands of the four K = 16 steps of mma_regs_tile.  Call it
+// before wgmma_fence(): packing between the wgmma of one batch would make ptxas serialise them.
+__device__ __forceinline__ void pack_a(const float (&p)[32], uint32_t (&a)[4][4]) {
 #pragma unroll
-  for (int ks = 0; ks < 4 * NP; ++ks) {
-    const uint32_t ofs = (ks >> 2) * kPanel + (ks & 3) * 32;
-    if (NP == 1 || ks < nks) wgmma_bf16_ss_n64<0, 0>(d, desc_kmajor(a + ofs), desc_kmajor(b + ofs));
+  for (int kk = 0; kk < 4; ++kk) {
+    frag_to_a(p, kk, a[kk]);
+    fence_regs(a[kk]);
   }
 }
 // d[j] += P · T_j for the first nout of NO consecutive panels T_j starting at t, read MN-major (reduction over their rows);
-// P in registers (rows x 64)
-template <int NO>
-__device__ __forceinline__ void mma_regs_tile(float (&d)[NO][32], const float (&p)[32], uint32_t t, int nout) {
+// P packed by pack_a.  N counts the panels of the straight-line run; a smaller nout is peeled off by uniform branches
+// (as in mma_tiles_kk).
+template <int NO, int N = NO>
+__device__ __forceinline__ void mma_regs_tile(float (&d)[NO][32], const uint32_t (&a)[4][4], uint32_t t, int nout) {
+  if constexpr (N > 1) {
+    if (nout < N) return mma_regs_tile<NO, N - 1>(d, a, t, nout);
+  }
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) {
-    uint32_t a[4];
-    frag_to_a(p, kk, a);
 #pragma unroll
-    for (int j = 0; j < NO; ++j)
-      if (j < nout) wgmma_bf16_rs_n64<1>(d[j], a, desc_mnmajor(t + j * kPanel + kk * 2048));
+    for (int j = 0; j < N; ++j) wgmma_bf16_rs_n64<1>(d[j], a[kk], desc_mnmajor(t + j * kPanel + kk * 2048));
   }
 }
 __device__ __forceinline__ void zero32(float (&d)[32]) {
@@ -231,8 +255,12 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
       lrow[hr] = lrow[hr] * corr[hr] + ls[hr];
       mrow[hr] = mx[hr];
     }
+    uint32_t pa[4][4];
+    pack_a(s, pa);
+#pragma unroll
+    for (int pn = 0; pn < NP; ++pn) fence_regs(o[pn]);  // the rescaled accumulator is written before the batch
     wgmma_fence();
-    mma_regs_tile<NP>(o, s, smem_u32(m.str[buf][1]), NP);
+    mma_regs_tile<NP>(o, pa, smem_u32(m.str[buf][1]), NP);
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
@@ -370,8 +398,10 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
       const float pr = ok ? fast_exp2(s[i] * p.scale_log2 - lse[hr]) : 0.f;
       s[i] = pr * (dp[i] - dlt[hr]);  // dS (w.r.t. the scaled scores)
     }
+    uint32_t pa[4][4];
+    pack_a(s, pa);
     wgmma_fence();
-    mma_regs_tile<NO>(dq, s, smem_u32(m.str[buf][0]) + pn0 * kPanel, nout);  // dQ += dS·K
+    mma_regs_tile<NO>(dq, pa, smem_u32(m.str[buf][0]) + pn0 * kPanel, nout);  // dQ += dS·K
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
@@ -438,9 +468,12 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
       dpt[i] = pr * (dpt[i] - m.col_delta[frag_col(i)]);  // dSᵀ
       st[i] = pr;                                       // Pᵀ
     }
+    uint32_t pa[4][4], dsa[4][4];
+    pack_a(st, pa);
+    pack_a(dpt, dsa);
     wgmma_fence();
-    mma_regs_tile<NO>(dv, st, smem_u32(m.str[buf][1]) + pn0 * kPanel, nout);   // dV += Pᵀ·dO
-    mma_regs_tile<NO>(dk, dpt, smem_u32(m.str[buf][0]) + pn0 * kPanel, nout);  // dK += dSᵀ·Q
+    mma_regs_tile<NO>(dv, pa, smem_u32(m.str[buf][1]) + pn0 * kPanel, nout);   // dV += Pᵀ·dO
+    mma_regs_tile<NO>(dk, dsa, smem_u32(m.str[buf][0]) + pn0 * kPanel, nout);  // dK += dSᵀ·Q
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll

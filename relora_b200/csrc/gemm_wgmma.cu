@@ -86,20 +86,58 @@ __device__ __forceinline__ void mma_bf16_kblock(float (&acc)[BLOCK_N / 2], uint3
     else wgmma_bf16_ss_n64<A_MN, B_MN>(acc, da + kStepA * k, db + kStepB * k);
   }
 }
-template <int BLOCK_N>
-__device__ __forceinline__ void mma_fp8_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa, uint32_t sb, bool a_e5m2) {
+template <int BLOCK_N, bool A_E5M2>
+__device__ __forceinline__ void mma_fp8_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa, uint32_t sb) {
   const uint64_t da = desc_kmajor(sa), db = desc_kmajor(sb);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {  // rows of 128 bytes: four K = 32 steps
     if constexpr (BLOCK_N == 256) {
-      if (a_e5m2) wgmma_e5m2_ss_n256(acc, da + 2 * k, db + 2 * k);
+      if constexpr (A_E5M2) wgmma_e5m2_ss_n256(acc, da + 2 * k, db + 2 * k);
       else wgmma_e4m3_ss_n256(acc, da + 2 * k, db + 2 * k);
     } else {
-      if (a_e5m2) wgmma_e5m2_ss_n128(acc, da + 2 * k, db + 2 * k);
+      if constexpr (A_E5M2) wgmma_e5m2_ss_n128(acc, da + 2 * k, db + 2 * k);
       else wgmma_e4m3_ss_n128(acc, da + 2 * k, db + 2 * k);
     }
   }
 }
+
+// Consumer side of the shared-memory ring with one k-block of wgmma in flight: after issuing k-block kb as one batch the
+// warpgroup waits only for k-block kb - 1, then hands that k-block's stage back to the producer.  `held` is the stage the
+// batch still in flight reads (-1: none); drain() retires it.  Accumulator registers are only touched by the wgmma
+// instructions between drains, so no operand fences sit between in-flight batches.
+template <int kStages, int kStageBytes>
+struct MmaRing {
+  const uint32_t smem0;
+  uint64_t* const full_bar;
+  uint64_t* const empty_bar;
+  int stage = 0;
+  uint32_t phase = 0;
+  int held = -1;
+
+  // n k-blocks through mma(stage smem address)
+  template <typename Mma>
+  __device__ __forceinline__ void run(int n, Mma mma) {
+    for (int i = 0; i < n; ++i) {
+      mbar_wait(&full_bar[stage], phase);
+      wgmma_fence();
+      mma(smem0 + stage * kStageBytes);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (held >= 0) mbar_arrive(&empty_bar[held]);
+      held = stage;
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+  }
+  // wait for every issued batch, then release the last stage; the caller fences the accumulator before reading it
+  __device__ __forceinline__ void drain() {
+    wgmma_wait<0>();
+    if (held >= 0) mbar_arrive(&empty_bar[held]);
+    held = -1;
+  }
+};
 
 template <int BLOCK_N, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -189,8 +227,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
   const float alpha_eff = p.alpha * (p.alpha_dev != nullptr ? *p.alpha_dev : 1.0f);
   const bool out_vec = (p.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 7) == 0);
   const bool res_vec = p.residual != nullptr && (p.ldr % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0);
-  int stage = 0;
-  uint32_t phase = 0;
+  MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar};
+  const uint32_t a_ofs = cw * 8192;  // this warpgroup's 64 rows of the A tile (either major)
   float acc[BLOCK_N / 2];
   for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
     const int tile = work / p.split_k, split = work % p.split_k;
@@ -200,26 +238,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     const int n0 = (tn / p.tiles_per_group) * p.n_per_group + nl;
     const int n_lim = min(p.N, n0 + min(BLOCK_N, p.n_per_group - nl));  // a group's last tile may be ragged
     const int kb_begin = split * kb_per_split, kb_end = min(num_kb, kb_begin + kb_per_split);
+    if (kb_begin >= kb_end) continue;  // nothing to accumulate for this work item
+    const int kb_mid = max(kb_begin, min(kb1, kb_end));  // segment 1: [kb_begin, kb_mid), segment 2: [kb_mid, kb_end)
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem0 + stage * L::kStageBytes + cw * 8192;  // this warpgroup's 64 rows (either major)
-      const uint32_t sb = smem0 + stage * L::kStageBytes + L::kABytes;
-      wgmma_fence();
-      if (kb < kb1 && p.fp8) mma_fp8_kblock<BLOCK_N>(acc, sa, sb, p.fp8 == 2);
-      else if (kb < kb1) mma_bf16_kblock<BLOCK_N, A_MN, B_MN>(acc, sa, sb);
-      else mma_bf16_kblock<BLOCK_N, false, false>(acc, sa, sb);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(acc);
-      mbar_arrive(&empty_bar[stage]);
-      if (++stage == kStages) {
-        stage = 0;
-        phase ^= 1;
-      }
+    fence_regs(acc);
+    // The operand type is chosen once per segment, so each loop body is one straight batch of wgmma.
+    if (p.fp8 == 2) {
+      ring.run(kb_mid - kb_begin, [&](uint32_t s) { mma_fp8_kblock<BLOCK_N, true>(acc, s + a_ofs, s + L::kABytes); });
+    } else if (p.fp8) {
+      ring.run(kb_mid - kb_begin, [&](uint32_t s) { mma_fp8_kblock<BLOCK_N, false>(acc, s + a_ofs, s + L::kABytes); });
+    } else {
+      ring.run(kb_mid - kb_begin, [&](uint32_t s) { mma_bf16_kblock<BLOCK_N, A_MN, B_MN>(acc, s + a_ofs, s + L::kABytes); });
     }
-    if (kb_begin >= kb_end) continue;  // nothing was accumulated for this work item
+    ring.run(kb_end - kb_mid, [&](uint32_t s) { mma_bf16_kblock<BLOCK_N, false, false>(acc, s + a_ofs, s + L::kABytes); });
+    ring.drain();
+    fence_regs(acc);
     // ---- epilogue: each thread owns column pairs of two rows (accumulator fragment order)
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; i += 2) {
@@ -379,23 +413,13 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
   uint32_t seeds[3];
 #pragma unroll
   for (int g = 0; g < 3; ++g) seeds[g] = mix_seed(seed0, p.keys[g]);
-  int stage = 0;
-  uint32_t phase = 0;
+  MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar};
+  // n k-blocks into acc with one batch in flight, drained before the caller reads acc
   auto mma_blocks = [&](float (&acc)[BLOCK_N / 2], int n) {
-    for (int kb = 0; kb < n; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem0 + stage * L::kStageBytes + cw * 8192;
-      wgmma_fence();
-      mma_bf16_kblock<BLOCK_N, false, true>(acc, sa, smem0 + stage * L::kStageBytes + L::kABytes);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(acc);
-      mbar_arrive(&empty_bar[stage]);
-      if (++stage == kStages) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
+    fence_regs(acc);
+    ring.run(n, [&](uint32_t s) { mma_bf16_kblock<BLOCK_N, false, true>(acc, s + cw * 8192, s + L::kABytes); });
+    ring.drain();
+    fence_regs(acc);
   };
   float acc[BLOCK_N / 2], cmb[BLOCK_N / 2];
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {

@@ -27,7 +27,9 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// Spin-wait watchdog: a protocol bug traps (kernel error) instead of hanging the GPU.
+// Spin-wait watchdog: a protocol bug traps (kernel error) instead of hanging the GPU.  The trap path must stay free of
+// function calls (no printf): ptxas will not keep a wgmma batch in flight across a call, and every wgmma kernel polls
+// mbarriers, so a call here would serialise each wgmma of every GEMM and attention kernel (warning C7510).
 #ifndef SM90_WATCHDOG_NS
 #define SM90_WATCHDOG_NS 4000000000ull  // 4 s
 #endif
@@ -75,7 +77,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       if (t0 == 0) {
         t0 = now;
       } else if (now - t0 > SM90_WATCHDOG_NS) {
-        printf("sm90 watchdog: mbarrier wait timed out (block %d thread %d parity %u)\n", blockIdx.x, threadIdx.x, parity);
         __trap();
       }
     }
@@ -131,6 +132,11 @@ template <int N>
 __device__ __forceinline__ void fence_regs(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 template <uint32_t R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
