@@ -37,7 +37,7 @@ for K in (128, 256, 512, 768, 1536, 3072, 6144):
     rec["bn128_us"] = timeit(lambda: F.gemm(x, W, out, block_n=128, pair=0), flush) * 1e6
     rec["bn256_us"] = timeit(lambda: F.gemm(x, W, out, block_n=256, pair=0), flush) * 1e6
     rec["pair_us"] = timeit(lambda: F.gemm(x, W, out, block_n=256, pair=1), flush) * 1e6
-    # fp32 accumulate output: no TMA-store epilogue (direct 128-bit global read-modify-write)
+    # fp32 accumulate output: stored from registers (global read-modify-write), the epilogue of the weight gradients
     rec["bn256_f32acc_us"] = timeit(lambda: F.gemm(x, W, outf, block_n=256, pair=0, accumulate=True), flush) * 1e6
     rows.append(rec)
     print(json.dumps({k: (round(v, 1) if isinstance(v, float) else v) for k, v in rec.items()}), flush=True)

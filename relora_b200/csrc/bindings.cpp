@@ -482,8 +482,11 @@ void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& w, const Ten
     rb::LnBwdNorm n1, n2;
     n1.dy = dy.data_ptr(); n1.w = w.data_ptr(); n1.dw = dw.data_ptr<float>(); n1.db = f32_or_null(db);
     n2.dy = ptr_or_null(dy2); n2.w = ptr_or_null(w2); n2.dw = f32_or_null(dw2); n2.db = f32_or_null(db2);
+    Tensor total;  // Σ rows of dres, formed once when it goes to two outputs
+    if (dres_sum2.has_value()) total = at::empty({H}, x.options().dtype(at::kFloat));
     ok = rb::layernorm_bwd_dual(x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), n1, n2, ptr_or_null(dres), dx.data_ptr(),
-                                f32_or_null(dres_sum), f32_or_null(dres_sum2), (int)x.size(0), (int)H, cur_stream());
+                                f32_or_null(dres_sum), f32_or_null(dres_sum2), dres_sum2.has_value() ? total.data_ptr<float>() : nullptr,
+                                (int)x.size(0), (int)H, cur_stream());
   }
   TORCH_CHECK(ok, "layernorm_bwd: hidden size must be a multiple of 8 and <= 2048");
 }
@@ -685,6 +688,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "relora_b200 sm_90a kernels";
   m.def("gemm", &gemm, "wgmma GEMM with fused LoRA K-extension");
   m.def("gemm_clear_descriptor_cache", &rb::gemm_clear_descriptor_cache);
+  // host-side schedule of one gemm call (no launch): (block_n, tma_store, dynamic shared memory bytes)
+  m.def("gemm_plan", [](int64_t block_n, bool out_f32, int64_t out_addr, int64_t ldc, int64_t n, int64_t split_k) {
+    rb::GemmDesc d;
+    d.block_n = (int)block_n; d.out_f32 = out_f32; d.out = reinterpret_cast<void*>(out_addr); d.ldc = ldc; d.N = (int)n;
+    const int bn = rb::gemm_block_n(d);
+    return py::make_tuple(bn, rb::gemm_uses_tma_store(d, bn, (int)split_k), rb::gemm_smem_bytes(bn));
+  }, py::arg("block_n"), py::arg("out_f32"), py::arg("out_addr"), py::arg("ldc"), py::arg("n"), py::arg("split_k"));
   m.def("rmsnorm_fwd", &rmsnorm_fwd, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("rstd"), py::arg("eps"), py::arg("xd"), py::arg("seed"),
         py::arg("keys"), py::arg("p"), py::arg("q8") = py::none(), py::arg("q_inv_scale") = py::none(), py::arg("q_amax") = py::none());
   m.def("rmsnorm_bwd", &rmsnorm_bwd);

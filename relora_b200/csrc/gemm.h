@@ -58,6 +58,11 @@ struct GemmDesc {
 };
 
 void gemm_bf16(const GemmDesc& d, cudaStream_t stream);
+// Schedule choices of gemm_bf16 (host side): the tile width, whether the epilogue stores through shared memory with TMA,
+// and the dynamic shared memory of a tile width.
+int gemm_block_n(const GemmDesc& d);
+bool gemm_uses_tma_store(const GemmDesc& d, int block_n, int split_k);
+int gemm_smem_bytes(int block_n);
 
 // Input gradient of a stacked LoRA group with the dropout mask applied in the epilogue:
 //   out[M,N] = dy[M,Kb]·W[Kb,N] + inv_keep · Σ_g keep(seed_g; row, col) ⊙ (du_g[M,r]·A_g[r,N]),  g < groups <= 3

@@ -1,5 +1,6 @@
 // Persistent warp-specialised bf16 / fp8 GEMM for sm_90a: TMA -> shared memory (128B swizzle) -> wgmma with fp32
-// accumulators in registers -> epilogue straight from registers.
+// accumulators in registers -> epilogue.  bf16 outputs of the 128-wide tile leave through a shared-memory staging buffer
+// and TMA stores that drain while the next tile's k-loop runs; fp32, split-K and unaligned outputs are stored from registers.
 //
 //   D[M,N] = alpha * ( A1[M,K1]·B1[N,K1]ᵀ + A2[M,K2]·B2[N,K2]ᵀ ) (+ bias) (+ residual) (+ D)
 //
@@ -49,6 +50,7 @@ struct KernelArgs {
   int num_m_tiles, num_n_tiles;
   int tiles_per_group;  // N-tiles per output-column group (the last one of a group may be ragged)
   int split_k;  // >1: each output tile is computed by split_k CTAs over disjoint K ranges, combined with fp32 atomics
+  int tma_store;  // bf16 output through shared memory and TMA stores (map_out); else stored from registers
 };
 
 template <int BLOCK_N>
@@ -58,7 +60,11 @@ struct SmemLayout {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = (192 * 1024) / kStageBytes;  // 6 stages of 128-wide tiles, 4 of 256-wide tiles
   static constexpr int kTileBytes = kStages * kStageBytes;
-  static constexpr int kTotal = kTileBytes + 1024 + 1024;  // barriers, manual 1024-byte alignment
+  static constexpr int kRingTotal = kTileBytes + 1024 + 1024;  // ring, barriers, manual 1024-byte alignment (lora_dx)
+  // gemm_kernel: + the store staging of the bf16 epilogue, two 64 x 64 sub-tiles (8 KB, 128B-swizzled) per consumer
+  // warpgroup.  128-wide tiles only: with the 128 accumulator registers of a 256-wide tile the staging code spills.
+  static constexpr int kStoreBytes = BLOCK_N == 128 ? 2 * 2 * 64 * 64 * 2 : 0;
+  static constexpr int kTotal = kRingTotal + kStoreBytes;
 };
 static_assert(SmemLayout<256>::kTotal <= 232448 && SmemLayout<128>::kTotal <= 232448, "shared memory budget");
 
@@ -142,12 +148,13 @@ struct MmaRing {
 template <int BLOCK_N, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ CUtensorMap map_b1,
-            const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b2, const KernelArgs p) {
+            const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b2,
+            const __grid_constant__ CUtensorMap map_out, const KernelArgs p) {
   using L = SmemLayout<BLOCK_N>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kTileBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kTileBytes + L::kStoreBytes);
   uint64_t* empty_bar = full_bar + kStages;
 
   const uint32_t warp = warp_id();
@@ -160,6 +167,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
       tma_prefetch_desc(&map_a2);
       tma_prefetch_desc(&map_b2);
     }
+    if (p.tma_store) tma_prefetch_desc(&map_out);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 256);  // every consumer thread releases the slot
@@ -229,6 +237,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
   const bool res_vec = p.residual != nullptr && (p.ldr % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0);
   MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar};
   const uint32_t a_ofs = cw * 8192;  // this warpgroup's 64 rows of the A tile (either major)
+  const bool store_lead = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's TMA stores
+  const uint32_t stage_u32 = smem0 + L::kTileBytes;  // store staging, 1024-byte aligned (128B swizzle)
   float acc[BLOCK_N / 2];
   for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
     const int tile = work / p.split_k, split = work % p.split_k;
@@ -254,7 +264,66 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     ring.run(kb_end - kb_mid, [&](uint32_t s) { mma_bf16_kblock<BLOCK_N, false, false>(acc, s + a_ofs, s + L::kABytes); });
     ring.drain();
     fence_regs(acc);
-    // ---- epilogue: each thread owns column pairs of two rows (accumulator fragment order)
+    if (BLOCK_N == 128 && p.tma_store) {
+      // ---- bf16 epilogue through shared memory: each 64-column sub-tile of the warpgroup's 64 rows is written to a
+      // staging buffer in the TMA box layout and stored by one thread; the store drains while the next tile's k-loop runs.
+      // Same fp32 operations in the same order as the register path below, one rounding.  A group's ragged last tile
+      // stores only the sub-tiles inside the group (group widths are multiples of 64); the TMA unit clips rows and columns
+      // past the tensor.
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 64; ++j) {
+        if (n0 + j * 64 >= n_lim) break;
+        // buffer j % 2: wait until the store that last read it has done so (the previous tile's last store, issued a whole
+        // k-loop ago, or sub-tile j - 2)
+        if (store_lead) {
+          if (j == 0) bulk_wait_read<0>();
+          else bulk_wait_read<1>();
+        }
+        named_bar_sync(1 + cw, 128);
+        const uint32_t buf = stage_u32 + (cw * 2 + (j & 1)) * 8192;
+#pragma unroll
+        for (int q = 0; q < 32; q += 2) {
+          const int i = j * 32 + q;
+          const int r = frag_row(i);
+          const int row = m0 + cw * 64 + r, col = n0 + frag_col(i);
+          float v0 = acc[i] * alpha_eff, v1 = acc[i + 1] * alpha_eff;
+          if (row < p.M && col < n_lim) {
+            const bool pair_ok = col + 1 < n_lim;
+            if (p.bias != nullptr) {
+              v0 += __bfloat162float(p.bias[col]);
+              if (pair_ok) v1 += __bfloat162float(p.bias[col + 1]);
+            }
+            const long long ofs = (long long)row * p.ldc + col;
+            if (p.residual != nullptr) {
+              const bf16* rp = p.residual + (long long)row * p.ldr + col;
+              if (pair_ok && res_vec) {
+                const float2 rv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(rp));
+                v0 += rv.x;
+                v1 += rv.y;
+              } else {
+                v0 += __bfloat162float(rp[0]);
+                if (pair_ok) v1 += __bfloat162float(rp[1]);
+              }
+            }
+            if (p.accumulate) {
+              const bf16* op = reinterpret_cast<const bf16*>(p.out) + ofs;
+              v0 += __bfloat162float(op[0]);
+              if (pair_ok) v1 += __bfloat162float(op[1]);
+            }
+          }
+          // 16-byte chunk (q / 4) of row r, XOR-swizzled by r % 8: conflict-free, and the layout the TMA unit reads
+          st_shared_u32(buf + r * 128 + (((q >> 2) ^ (r & 7)) << 4) + (threadIdx.x & 3) * 4, pack_bf16x2(v0, v1));
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(1 + cw, 128);
+        if (store_lead) {
+          tma_store_2d(&map_out, buf, n0 + j * 64, m0 + cw * 64);
+          bulk_commit();
+        }
+      }
+      continue;
+    }
+    // ---- epilogue from registers: each thread owns column pairs of two rows (accumulator fragment order)
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; i += 2) {
       const int row = m0 + cw * 64 + frag_row(i);
@@ -312,6 +381,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
       }
     }
   }
+  if (store_lead && p.tma_store) bulk_wait_all();  // the staging buffers must outlive the stores that read them
 }
 
 // =============================================================================================
@@ -576,6 +646,14 @@ static CUtensorMap operand_map(const Operand& o, long long mn, long long k, int 
   return make_map_2d(o.ptr, mn, k, o.ld, 64, BLOCK_K);
 }
 
+// The TMA store needs a 16-byte aligned base and row pitch, and a row length of whole 16-byte chunks: past a ragged last
+// chunk it writes beyond column N.  fp32 outputs (weight gradients, accumulated or split-K with atomics) and 256-wide tiles
+// keep the register epilogue.
+bool gemm_uses_tma_store(const GemmDesc& d, int block_n, int split_k) {
+  return block_n == 128 && !d.out_f32 && split_k == 1 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && d.ldc % 8 == 0 &&
+         d.N % 8 == 0;
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN>
 static void launch(const GemmDesc& d, cudaStream_t stream) {
   using L = SmemLayout<BLOCK_N>;
@@ -636,10 +714,12 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
     throw std::runtime_error("gemm: split_k needs an fp32 accumulate output without residual");
   if (split < 1) split = 1;
   p.split_k = split;
+  p.tma_store = gemm_uses_tma_store(d, BLOCK_N, split) ? 1 : 0;
+  const CUtensorMap mout = p.tma_store ? make_map_2d(d.out, d.N, d.M, d.ldc, 64, 64) : ma1;
   const int work = tiles * split;
   const int grid = work < num_sms() ? work : num_sms();
   if (grid <= 0) return;
-  launch_k(kern, grid, kNumThreads, L::kTotal, stream, ma1, mb1, ma2, mb2, p);
+  launch_k(kern, grid, kNumThreads, L::kTotal, stream, ma1, mb1, ma2, mb2, mout, p);
   RB_CHECK_LAUNCH("gemm_kernel");
 }
 
@@ -654,17 +734,19 @@ static void dispatch_major(const GemmDesc& d, cudaStream_t s) {
   }
 }
 
+// Tile width: 128 unless the caller asks for 256 (block_n 0 = auto).  On an H100 80GB HBM3 at 700 W (bench/gemm_bench.py, M 12288, plain
+// bf16 GEMM with the register epilogue) the 256-wide tile ran at 192 - 387 TFLOP/s on the llama_1b shapes and 410 at 8192^3,
+// the 128-wide one at 466 - 548 and 440; with the fused LoRA branch the 256-wide tile took 2.0 - 2.5x as long on every
+// llama_250m / llama_1b projection.  The K sweep (bench/gemm_ksweep.py) puts the difference in the per-tile fixed cost:
+// 528 vs 260 us at K = 128, N = 5120.  Only the 128-wide tile has the TMA-store epilogue (the 256-wide one would spill).
+int gemm_block_n(const GemmDesc& d) { return d.block_n == 256 ? 256 : 128; }
+
+int gemm_smem_bytes(int block_n) { return block_n == 256 ? SmemLayout<256>::kTotal : SmemLayout<128>::kTotal; }
+
 void gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
   if (d.n_lora_acc != 0) throw std::runtime_error("gemm: dropout-combine epilogue not built into this kernel variant");
   if (d.M <= 0 || d.N <= 0) return;
-  int bn = d.block_n;
-  if (bn == 0) {
-    // wide tiles halve the shared-memory traffic per MMA; keep 128 when the group size demands it or there are too few tiles
-    const int npg = d.n_per_group > 0 ? d.n_per_group : d.N;
-    const bool groups_ok = (npg % 256 == 0) || (npg >= d.N) || (npg % 64 == 0 && npg >= 2048);  // ragged last tile: <= 6 % waste
-    bn = (d.N >= 512 && groups_ok && ceil_div(d.M, BLOCK_M) * ceil_div(d.N, 256) >= num_sms() / 2) ? 256 : 128;
-  }
-  if (bn == 256) dispatch_major<256>(d, stream);
+  if (gemm_block_n(d) == 256) dispatch_major<256>(d, stream);
   else dispatch_major<128>(d, stream);
 }
 
@@ -694,12 +776,12 @@ void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
   }
   static bool configured = false;
   if (!configured) {
-    check(cudaFuncSetAttribute(lora_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal), "cudaFuncSetAttribute(lora_dx)");
+    check(cudaFuncSetAttribute(lora_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kRingTotal), "cudaFuncSetAttribute(lora_dx)");
     configured = true;
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  launch_k(lora_dx_kernel, grid, kNumThreads, L::kTotal, stream, m_dy, m_w, m_du, m_a, p);
+  launch_k(lora_dx_kernel, grid, kNumThreads, L::kRingTotal, stream, m_dy, m_w, m_du, m_a, p);
   RB_CHECK_LAUNCH("lora_dx_kernel");
 }
 

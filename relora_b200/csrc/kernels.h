@@ -82,9 +82,10 @@ struct LnBwdNorm {
   float* dw = nullptr;
   float* db = nullptr;
 };
-// dx = dres + LN1ᵀ(dy1) [+ LN2ᵀ(dy2) when n2.dy != nullptr]; dres may be nullptr.  dsum1 / dsum2 (fp32, optional) += Σ rows of dres.
+// dx = dres + LN1ᵀ(dy1) [+ LN2ᵀ(dy2) when n2.dy != nullptr]; dres may be nullptr.  dsum1 / dsum2 (fp32, optional) += Σ rows of dres;
+// with dsum2, the sum is formed once in dsum_tmp (fp32 [H] scratch) and added to both, so equal inputs stay bit-equal.
 bool layernorm_bwd_dual(const void* x, const float* mean, const float* rstd, const LnBwdNorm& n1, const LnBwdNorm& n2, const void* dres,
-                        void* dx, float* dsum1, float* dsum2, int M, int H, cudaStream_t s);
+                        void* dx, float* dsum1, float* dsum2, float* dsum_tmp, int M, int H, cudaStream_t s);
 // xd (optional): dropout copy of the output under `key`, rows of N elements
 void gelu_fwd(const void* z, void* a, long long n, bool tanh_approx, cudaStream_t s, void* xd = nullptr, int N = 0, uint32_t key = 0,
               const LnDrop& drop = LnDrop{});

@@ -173,13 +173,14 @@ __global__ void __launch_bounds__(kRowsPerBlock * 32) layernorm_bwd_kernel(const
 
 // Executor form of the backward: dx = dres + LN1ᵀ(dy1) [+ LN2ᵀ(dy2)] for norms of the same x, the γ / β gradients of each norm and,
 // optionally, Σ rows of dres (the bias gradient of the projections whose output gradient dres is).  Block partials go through
-// shared memory, laid out [quantity][j][column vector] so that the lanes of a warp hit consecutive words.
+// shared memory, laid out [quantity][j][column vector] so that the lanes of a warp hit consecutive words.  With two Σ dres
+// outputs the blocks add their partials into `dsum1` as a zeroed total, which ln_add_total then adds to both outputs.
 template <int VPL>
 __global__ void __launch_bounds__(kRowsPerBlock * 32) layernorm_bwd_dual_kernel(const bf16* __restrict__ x, const float* __restrict__ mean,
                                                                                const float* __restrict__ rstd, const LnBwdNorm n1,
                                                                                const LnBwdNorm n2, const bf16* __restrict__ dres,
                                                                                bf16* __restrict__ dx, float* __restrict__ dsum1,
-                                                                               float* __restrict__ dsum2, int M, int H) {
+                                                                               int M, int H) {
   extern __shared__ float sacc[];  // [5][H]: dw1, db1, dw2, db2, Σ dres
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nvec = H / 8;
@@ -255,10 +256,19 @@ __global__ void __launch_bounds__(kRowsPerBlock * 32) layernorm_bwd_dual_kernel(
   for (int q = 0; q < nq; ++q) {
     if (dst[q] == nullptr) continue;
     for (int col = threadIdx.x; col < H; col += blockDim.x) {
-      const float v = sacc[q * H + (col & 7) * nvec + (col >> 3)];
-      atomicAdd(dst[q] + col, v);
-      if (q == 4 && dsum2 != nullptr) atomicAdd(dsum2 + col, v);
+      atomicAdd(dst[q] + col, sacc[q * H + (col & 7) * nvec + (col >> 3)]);
     }
+  }
+}
+
+// out1 += total; out2 += total: the two bias gradients that share Σ dres receive the same rounded sum, whatever order the
+// blocks' atomics added it up in
+__global__ void ln_add_total_kernel(const float* __restrict__ total, float* __restrict__ out1, float* __restrict__ out2, int H) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < H) {
+    const float t = total[c];
+    out1[c] += t;
+    out2[c] += t;
   }
 }
 
@@ -445,13 +455,19 @@ bool layernorm_bwd(const void* dy, const void* x, const void* w, const float* me
 }
 
 bool layernorm_bwd_dual(const void* x, const float* mean, const float* rstd, const LnBwdNorm& n1, const LnBwdNorm& n2, const void* dres,
-                        void* dx, float* dsum1, float* dsum2, int M, int H, cudaStream_t s) {
+                        void* dx, float* dsum1, float* dsum2, float* dsum_tmp, int M, int H, cudaStream_t s) {
   const int vpl = (H % 8 == 0) ? pick_vpl(H / 8) : 0;
   if (vpl == 0 || vpl > 8 || M <= 0) return false;
+  if (dsum2 != nullptr && (dsum1 == nullptr || dsum_tmp == nullptr)) throw std::runtime_error("layernorm_bwd: dsum2 needs dsum1 and dsum_tmp");
   const size_t smem = 5 * (size_t)H * sizeof(float);
   const int grid = std::min(ceil_div(M, kRowsPerBlock), 2 * num_sms());
   const bf16 *xp = (const bf16*)x, *rp = (const bf16*)dres;
-#define L(V) launch_k(layernorm_bwd_dual_kernel<V>, grid, kRowsPerBlock * 32, smem, s, xp, mean, rstd, n1, n2, rp, (bf16*)dx, dsum1, dsum2, M, H)
+  float* dsum = dsum1;
+  if (dsum2 != nullptr) {
+    check(cudaMemsetAsync(dsum_tmp, 0, (size_t)H * sizeof(float), s), "cudaMemsetAsync(layernorm_bwd total)");
+    dsum = dsum_tmp;
+  }
+#define L(V) launch_k(layernorm_bwd_dual_kernel<V>, grid, kRowsPerBlock * 32, smem, s, xp, mean, rstd, n1, n2, rp, (bf16*)dx, dsum, M, H)
   switch (vpl) {
     case 1: L(1); break;
     case 2: L(2); break;
@@ -461,6 +477,10 @@ bool layernorm_bwd_dual(const void* x, const float* mean, const float* rstd, con
   }
 #undef L
   RB_CHECK_LAUNCH("layernorm_bwd_dual");
+  if (dsum2 != nullptr) {
+    launch_k(ln_add_total_kernel, ceil_div(H, 256), 256, 0, s, (const float*)dsum_tmp, dsum1, dsum2, H);
+    RB_CHECK_LAUNCH("ln_add_total");
+  }
   return true;
 }
 

@@ -47,6 +47,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -117,6 +120,22 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* ba
         "l"(hint)
       : "memory");
 }
+// Shared -> global tensor store, tracked per issuing thread as a bulk async-group.  The source must have been written
+// before a fence_proxy_async_smem() of every writing thread and a barrier.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               :
+               : "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// wait until every bulk group of this thread has completed (its global writes included)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
 // wgmma: one warpgroup (128 threads) computes a 64-row slice; accumulators live in registers.

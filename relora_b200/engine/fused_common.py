@@ -153,8 +153,8 @@ class FusedStepperBase:
         if self.fused_dx:
             sd, ks, pp = (self.seed, list(keys), self.p) if drop else (None, [0] * G, 0.0)
             if G * Ng >= self.dx_split_k:
-                # long reductions: the frozen-path product runs on the 256-wide / CTA-pair GEMM (1.3-1.5x the per-FLOP rate of
-                # the 128-wide multi-accumulator tiles), then one light pass adds the masked low-rank terms
+                # long reductions: the frozen-path product runs on the GEMM, whose TMA-store epilogue overlaps the next
+                # tile's k-loop, then one light pass adds the masked low-rank terms
                 if self.fp8_bwd and site is not None:
                     # E5M2 copy of the output gradient (delayed scale) x E4M3 copy of Wᵀ on the kind::f8f6f4 path
                     l_, s_i = site
