@@ -113,17 +113,16 @@ def delete_old_checkpoints(save_dir: str, keep: Optional[int]) -> None:
 
 
 def load_model_weights(module: torch.nn.Module, directory: str, strict: bool = True) -> None:
-    """Load ``pytorch_model.bin`` (hard-coded name upstream; safetensors accepted as a fallback)."""
-    path = os.path.join(directory, "pytorch_model.bin")
-    if os.path.exists(path):
-        state = torch.load(path, map_location="cpu", weights_only=True)
-    else:
-        from safetensors.torch import load_file
+    """Load ``pytorch_model.bin`` (hard-coded name upstream), ``model.safetensors`` or a sharded checkpoint's ``*.index.json``.
+    Hugging Face Llama checkpoints carry no ``rotary_emb.inv_freq`` buffers: those keep the module's values."""
+    from ..models.llama import load_state_dict_files
 
-        state = load_file(os.path.join(directory, "model.safetensors"))
+    state = load_state_dict_files(directory)
     if hasattr(module, "load_hf_state_dict"):
         module.load_hf_state_dict(state, strict=strict)
     else:
+        own = module.state_dict()
+        state.update({k: v for k, v in own.items() if k.endswith("rotary_emb.inv_freq") and k not in state})
         module.load_state_dict(state, strict=strict)
 
 

@@ -7,7 +7,7 @@
 //
 //   attn_fwd_kernel      CTA = (64 queries, head, batch); per 64 keys:  S = Q·Kᵀ -> online softmax -> O += P·V
 //   attn_bwd_dq_kernel   CTA = (64 queries, head, batch); per 64 keys:  S, dP = dO·Vᵀ -> dS -> dQ += dS·K
-//   attn_bwd_dkv_kernel  CTA = (64 keys, head, batch); per 64 queries:  Sᵀ = K·Qᵀ, dPᵀ = V·dOᵀ -> Pᵀ, dSᵀ -> dV += Pᵀ·dO, dK += dSᵀ·Q
+//   attn_bwd_dkv_kernel  CTA = (64 keys, KV head, batch); per 64 queries of each query head of the group:  Sᵀ = K·Qᵀ, dPᵀ = V·dOᵀ -> Pᵀ, dSᵀ -> dV += Pᵀ·dO, dK += dSᵀ·Q
 //
 // Each kernel is instantiated for NP = ceil(head_dim / 64) in {1, 2, 3, 4}.  An operand tile is NP shared-memory panels of
 // [64 rows x 64 columns] bf16 (128 bytes per row, 128-byte swizzle), loaded by NP TMA boxes at column offsets 64·p; columns
@@ -186,15 +186,23 @@ __device__ __forceinline__ void prologue(const Smem& m, TileSrc r0, TileSrc r1, 
   mbar_wait(m.res_bar, 0);
 }
 
-// Head map of the packed qkv buffer, in head-columns of hd: q, k, v of head h sit at h·hs, h·hs + ws, h·hs + 2·ws.
-// Default layout [(q|k|v), nh, hd]: hs = 1, ws = nh.  Interleaved (GPT-NeoX query_key_value) [nh, (q|k|v), hd]: hs = 3, ws = 1.
+// Head map of the packed qkv buffer, in head-columns of hd: query head h sits at h·hs; it reads KV head kv = h / group, whose
+// k and v sit at kv·hs + wk and kv·hs + wv.  Default layout [q: nh | k: nkv | v: nkv] x hd: hs = 1, wk = nh, wv = nh + nkv,
+// group = nh / nkv (grouped-query attention; 1 for multi-head).  Interleaved (GPT-NeoX query_key_value) [nh, (q|k|v), hd]:
+// hs = 3, wk = 1, wv = 2, group = 1.
+struct HeadMap {
+  int hs, wk, wv, group;
+  __device__ __forceinline__ int q(int h) const { return h * hs; }
+  __device__ __forceinline__ int k(int kv) const { return kv * hs + wk; }
+  __device__ __forceinline__ int v(int kv) const { return kv * hs + wv; }
+};
 struct FwdArgs {
   bf16* out;
   long long ld_out;
   float* lse;
   int B, T, nh, hd;
   float scale_log2;
-  int hs, ws;
+  HeadMap hm;
 };
 
 // =============================================================================================== forward
@@ -209,7 +217,8 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(const __grid_constan
   const int nks = (p.hd + 15) / 16;
   const Smem m = smem_layout<1, NP>();
   // resident: Q; streamed: K, V
-  const int hq = h * p.hs, hk = hq + p.ws, hv = hq + 2 * p.ws;
+  const int kv = h / p.hm.group;
+  const int hq = p.hm.q(h), hk = p.hm.k(kv), hv = p.hm.v(kv);
   prologue<1, NP>(m, {&map_qkv, hq}, {&map_qkv, hq}, rowbase + q0, {&map_qkv, hk}, {&map_qkv, hv}, rowbase, nkb);
   const uint32_t sq = smem_u32(m.res[0]);
   float o[NP][32], mrow[2] = {kNegInf, kNegInf}, lrow[2] = {0.f, 0.f};
@@ -329,7 +338,7 @@ struct BwdArgs {
   long long ld_dqkv;
   int B, T, nh, hd;
   float scale, scale_log2;
-  int hs, ws;  // head map of qkv / dqkv (see FwdArgs)
+  HeadMap hm;  // of qkv / dqkv (see FwdArgs)
 };
 
 __device__ __forceinline__ void store_rows(bf16* base, long long ld, int row0, int rows_valid, int col_ofs, int hd, const float (&d)[32], float sc) {
@@ -364,7 +373,8 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
   const int nkb = qb + 1;
   const int nks = (p.hd + 15) / 16;
   const Smem m = smem_layout<2, NP>();
-  const int hq = h * p.hs, hk = hq + p.ws, hv = hq + 2 * p.ws;
+  const int kv = h / p.hm.group;
+  const int hq = p.hm.q(h), hk = p.hm.k(kv), hv = p.hm.v(kv);
   prologue<2, NP>(m, {&map_qkv, hq}, {&map_do, h}, rowbase + q0, {&map_qkv, hk}, {&map_qkv, hv}, rowbase, nkb);
   const long long bh = (long long)b * p.nh + h;
   const int r_lo = q0 + frag_row(0);
@@ -416,6 +426,11 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dq_kernel(const __grid_cons
 }
 
 // =============================================================================================== backward: dK, dV
+// CTA = (64 keys, KV head, batch).  Under grouped-query attention (GQA) the CTA streams the (Q, dO) blocks of each query head of its
+// group in turn and accumulates dK / dV over the whole group in registers: one writer per output element and a fixed summation
+// order, so no atomics and bit-reproducible results.  Stream item jj is query block kb + jb of query head h0 + g, with
+// jj = g·nblk + jb; the query head and first row are stepped as counters rather than divided out (the kernel runs at the edge of the
+// register file).
 template <int NP>
 __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap map_qkv,
                                                                 const __grid_constant__ CUtensorMap map_do, const BwdArgs p) {
@@ -425,14 +440,17 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
   const int kb = blockIdx.x / NSPLIT;  // key block; query blocks kb .. nkb-1
   const int pn0 = (blockIdx.x % NSPLIT) * NO;
   const int nout = NP % NO == 0 ? NO : min(NO, NP - pn0);
-  const int h = blockIdx.y, b = blockIdx.z;
+  const int kv = blockIdx.y, b = blockIdx.z;
   const int k0 = kb * BQ, rowbase = b * p.T;
   const int nblk = nkb - kb;
   const int nks = (p.hd + 15) / 16;
   const Smem m = smem_layout<2, NP>();
-  const int hq = h * p.hs, hk = hq + p.ws, hv = hq + 2 * p.ws;
-  prologue<2, NP>(m, {&map_qkv, hk}, {&map_qkv, hv}, rowbase + k0, {&map_qkv, hq}, {&map_do, h}, rowbase + k0, nblk);
-  const long long bh = (long long)b * p.nh + h;
+  const int h0 = kv * p.hm.group;  // first query head of the group
+  prologue<2, NP>(m, {&map_qkv, p.hm.k(kv)}, {&map_qkv, p.hm.v(kv)}, rowbase + k0, {&map_qkv, p.hm.q(h0)}, {&map_do, h0}, rowbase + k0, nblk);
+  if (nblk == 1 && p.hm.group > 1 && warp_id() == 0) {  // the prologue streamed only the first head's single block
+    if (elect_one()) issue_pair<NP>(m, 1, {&map_qkv, p.hm.q(h0 + 1)}, {&map_do, h0 + 1}, rowbase + k0);
+    __syncwarp();
+  }
   const int key_lo = k0 + frag_row(0);
   float dk[NO][32], dv[NO][32];
 #pragma unroll
@@ -440,9 +458,11 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
     zero32(dk[j]);
     zero32(dv[j]);
   }
-  for (int jj = 0; jj < nblk; ++jj) {
+  int hg = h0, qs = k0;  // query head and first query row of stream item jj
+  // the bound is re-derived from blockIdx and the kernel parameters, so it occupies no register across the loop
+  for (int jj = 0; hg < ((int)blockIdx.y + 1) * p.hm.group; ++jj) {
     const int buf = jj & 1;
-    const int qs = (kb + jj) * BQ;
+    const long long bh = (long long)b * p.nh + hg;
     if (threadIdx.x < BQ) {  // row statistics of this block's 64 queries, read by every thread below
       const int qc = min(qs + (int)threadIdx.x, p.T - 1);
       m.col_lse[threadIdx.x] = p.lse[bh * p.T + qc];
@@ -482,14 +502,26 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_dkv_kernel(const __grid_con
       fence_regs(dk[j]);
     }
     __syncthreads();
-    if (warp_id() == 0 && jj + 2 < nblk) {
-      if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, hq}, {&map_do, h}, rowbase + qs + 2 * BQ);
-      __syncwarp();
+    if (warp_id() == 0) {
+      int h2 = hg, q2 = qs + 2 * BQ;  // item jj + 2
+      while (q2 >= p.T) {
+        q2 -= nkb * BQ - k0;
+        ++h2;
+      }
+      if (h2 < ((int)blockIdx.y + 1) * p.hm.group) {
+        if (elect_one()) issue_pair<NP>(m, buf, {&map_qkv, p.hm.q(h2)}, {&map_do, h2}, rowbase + q2);
+        __syncwarp();
+      }
+    }
+    qs += BQ;
+    if (qs >= p.T) {
+      qs = k0;
+      ++hg;
     }
   }
   bf16* base = p.dqkv + (long long)rowbase * p.ld_dqkv;
-  store_panels<NO>(base, p.ld_dqkv, k0, p.T, hk * p.hd, p.hd, pn0, nout, dk, p.scale);
-  store_panels<NO>(base, p.ld_dqkv, k0, p.T, hv * p.hd, p.hd, pn0, nout, dv, 1.0f);
+  store_panels<NO>(base, p.ld_dqkv, k0, p.T, p.hm.k(blockIdx.y) * p.hd, p.hd, pn0, nout, dk, p.scale);
+  store_panels<NO>(base, p.ld_dqkv, k0, p.T, p.hm.v(blockIdx.y) * p.hd, p.hd, pn0, nout, dv, 1.0f);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -527,10 +559,17 @@ CUtensorMap head_map(const void* ptr, long long ld, long long rows, int hd, int 
   return m;
 }
 
-void check_shape(int B, int T, int nh, int hd) {
+void check_shape(int B, int T, int nh, int nkv, int hd, bool interleaved) {
   if (B <= 0 || T <= 0 || nh <= 0) throw std::runtime_error("attention: empty problem");
   if (hd <= 0 || hd % 8 != 0 || hd > kMaxHeadDim)
     throw std::runtime_error("attention: head_dim must be a multiple of 8 and <= 256, got " + std::to_string(hd));
+  if (nkv <= 0 || nh % nkv != 0)
+    throw std::runtime_error("attention: nh (" + std::to_string(nh) + ") must be a multiple of nkv (" + std::to_string(nkv) + ")");
+  if (interleaved && nkv != nh) throw std::runtime_error("attention: the interleaved qkv layout has no grouped-query form (nkv must equal nh)");
+}
+
+HeadMap head_map_of(int nh, int nkv, bool interleaved) {
+  return interleaved ? HeadMap{3, 1, 2, 1} : HeadMap{1, nh, nh + nkv, nh / nkv};
 }
 
 template <int NP>
@@ -543,7 +582,7 @@ void fwd_np(const AttnDesc& d, const CUtensorMap& map, cudaStream_t stream) {
   p.out = reinterpret_cast<bf16*>(d.out); p.ld_out = d.ld_out; p.lse = d.lse;
   p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
   p.scale_log2 = d.scale * 1.4426950408889634f;
-  p.hs = d.interleaved ? 3 : 1; p.ws = d.interleaved ? 1 : d.nh;
+  p.hm = head_map_of(d.nh, d.nkv, d.interleaved);
   const dim3 grid((unsigned)((d.T + BQ - 1) / BQ), (unsigned)d.nh, (unsigned)d.B);
   launch_k(attn_fwd_kernel<NP>, grid, kThreads, smem, stream, map, p);
   RB_CHECK_LAUNCH("attn_fwd_kernel");
@@ -561,9 +600,9 @@ void bwd_np(const AttnBwdDesc& d, const CUtensorMap& map_qkv, const CUtensorMap&
   p.lse = d.lse; p.delta = d.delta; p.dqkv = reinterpret_cast<bf16*>(d.dqkv); p.ld_dqkv = d.ld_dqkv;
   p.B = d.B; p.T = d.T; p.nh = d.nh; p.hd = d.hd;
   p.scale = d.scale; p.scale_log2 = d.scale * 1.4426950408889634f;
-  p.hs = d.interleaved ? 3 : 1; p.ws = d.interleaved ? 1 : d.nh;
+  p.hm = head_map_of(d.nh, d.nkv, d.interleaved);
   const unsigned nblk = (unsigned)((d.T + BQ - 1) / BQ);
-  const dim3 grid_dkv(nblk * splits(NP, dkv_out_panels(NP)), (unsigned)d.nh, (unsigned)d.B);
+  const dim3 grid_dkv(nblk * splits(NP, dkv_out_panels(NP)), (unsigned)d.nkv, (unsigned)d.B);
   launch_k(attn_bwd_dkv_kernel<NP>, grid_dkv, kThreads, smem, stream, map_qkv, map_do, p);
   RB_CHECK_LAUNCH("attn_bwd_dkv_kernel");
   const dim3 grid_dq(nblk * splits(NP, dq_out_panels(NP)), (unsigned)d.nh, (unsigned)d.B);
@@ -576,9 +615,9 @@ int panels(int hd) { return (hd + 63) / 64; }
 }  // namespace
 
 void attention_fwd(const AttnDesc& d, cudaStream_t stream) {
-  check_shape(d.B, d.T, d.nh, d.hd);
+  check_shape(d.B, d.T, d.nh, d.nkv, d.hd, d.interleaved);
   const long long rows = (long long)d.B * d.T;
-  CUtensorMap map = head_map(d.qkv, d.ld_qkv, rows, d.hd, 3 * d.nh);
+  CUtensorMap map = head_map(d.qkv, d.ld_qkv, rows, d.hd, d.nh + 2 * d.nkv);
   switch (panels(d.hd)) {
     case 1: fwd_np<1>(d, map, stream); break;
     case 2: fwd_np<2>(d, map, stream); break;
@@ -588,9 +627,9 @@ void attention_fwd(const AttnDesc& d, cudaStream_t stream) {
 }
 
 void attention_bwd(const AttnBwdDesc& d, cudaStream_t stream) {
-  check_shape(d.B, d.T, d.nh, d.hd);
+  check_shape(d.B, d.T, d.nh, d.nkv, d.hd, d.interleaved);
   const long long rows = (long long)d.B * d.T;
-  CUtensorMap map_qkv = head_map(d.qkv, d.ld_qkv, rows, d.hd, 3 * d.nh);
+  CUtensorMap map_qkv = head_map(d.qkv, d.ld_qkv, rows, d.hd, d.nh + 2 * d.nkv);
   CUtensorMap map_do = head_map(d.dout, d.ld_dout, rows, d.hd, d.nh);
   {
     const long long total = rows * d.nh;

@@ -5,7 +5,8 @@
 
 namespace rb {
 
-// qkv: bf16 [B*T, 3*nh*hd] (q | k | v, heads contiguous inside each third, RoPE already applied), row stride ld_qkv.
+// qkv: bf16 [B*T, (nh + 2*nkv)*hd] (q: nh heads | k: nkv heads | v: nkv heads, heads contiguous inside each part, RoPE already
+//      applied), row stride ld_qkv.  Query head h attends with KV head h / (nh / nkv): grouped-query attention when nkv < nh.
 // out: bf16 [B*T, nh*hd] (row stride ld_out).  lse: fp32 [B, nh, T], log2-domain log-sum-exp of the scaled scores
 //      (p = exp2(s * scale * log2(e) - lse)), consumed by the backward kernels.
 // Requirements: hd % 8 == 0, hd <= 256.  A head is read as ceil(hd / 64) TMA boxes 64 columns wide; the columns of the last box
@@ -17,14 +18,16 @@ struct AttnDesc {
   long long ld_out = 0;
   float* lse = nullptr;
   int B = 0, T = 0, nh = 0, hd = 0;
+  int nkv = 0;         // KV heads, nh % nkv == 0 (nkv == nh: multi-head attention)
   float scale = 1.0f;  // 1/sqrt(hd)
-  // false: qkv is [(q|k|v), nh, hd] per row (above).  true: [nh, (q|k|v), hd] per row, the head-interleaved layout of GPT-NeoX's
-  // query_key_value projection (q, k, v of head h at head-columns 3h, 3h+1, 3h+2).
+  // false: qkv is [q | k | v] per row (above).  true: [nh, (q|k|v), hd] per row, the head-interleaved layout of GPT-NeoX's
+  // query_key_value projection (q, k, v of head h at head-columns 3h, 3h+1, 3h+2); needs nkv == nh.
   bool interleaved = false;
 };
 void attention_fwd(const AttnDesc& d, cudaStream_t stream);
 
-// Backward: dqkv bf16 [B*T, 3*nh*hd] receives dq | dk | dv in the layout of qkv (gradient w.r.t. the post-RoPE q / k).
+// Backward: dqkv bf16 [B*T, (nh + 2*nkv)*hd] receives dq | dk | dv in the layout of qkv (gradient w.r.t. the post-RoPE q / k).
+// dK / dV of a KV head sum over its group's query heads inside one CTA (no atomics).
 // delta: fp32 workspace [B, nh, T] (row sums of dO * O), filled by this call.
 struct AttnBwdDesc {
   const void* qkv = nullptr;
@@ -38,6 +41,7 @@ struct AttnBwdDesc {
   void* dqkv = nullptr;
   long long ld_dqkv = 0;
   int B = 0, T = 0, nh = 0, hd = 0;
+  int nkv = 0;  // see AttnDesc
   float scale = 1.0f;
   bool interleaved = false;  // layout of qkv and dqkv (see AttnDesc)
   // optional bf16 workspace of attention_ds_workspace_elems(B, T, nh) elements; not read by the sm_90 kernels (the dQ kernel

@@ -259,23 +259,27 @@ void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Te
   rb::lora_dx(d, cur_stream());
 }
 
-// causal flash attention over the packed (post-RoPE) qkv buffer [B*T, 3*nh*hd]
-void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64_t T, int64_t nh, int64_t hd, double scale, bool interleaved) {
+// causal flash attention over the packed (post-RoPE) qkv buffer [B*T, (nh + 2*nkv)*hd]; nkv < 0 means nkv = nh
+void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64_t T, int64_t nh, int64_t hd, double scale, bool interleaved,
+                   int64_t nkv) {
+  if (nkv < 0) nkv = nh;
   chk_bf16(qkv, "qkv"); chk_bf16(out, "out"); chk_2d_rowmajor(qkv, "qkv"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == 3 * nh * hd, "qkv must be [B*T, 3*nh*hd]");
+  TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == (nh + 2 * nkv) * hd, "qkv must be [B*T, (nh+2*nkv)*hd]");
   TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd, "out must be [B*T, nh*hd]");
   TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
   rb::AttnDesc d;
   d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0); d.lse = lse.data_ptr<float>();
-  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
+  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.nkv = (int)nkv; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
   c10::cuda::CUDAGuard guard(qkv.device());
   rb::attention_fwd(d, cur_stream());
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& delta, Tensor& dqkv, int64_t B,
-                   int64_t T, int64_t nh, int64_t hd, double scale, const OptTensor& ds_workspace, bool interleaved) {
+                   int64_t T, int64_t nh, int64_t hd, double scale, const OptTensor& ds_workspace, bool interleaved, int64_t nkv) {
+  if (nkv < 0) nkv = nh;
   chk_bf16(qkv, "qkv"); chk_bf16(out, "out"); chk_bf16(dout, "dout"); chk_bf16(dqkv, "dqkv");
   chk_2d_rowmajor(qkv, "qkv"); chk_2d_rowmajor(out, "out"); chk_2d_rowmajor(dout, "dout"); chk_2d_rowmajor(dqkv, "dqkv");
-  TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == 3 * nh * hd && dqkv.size(0) == B * T && dqkv.size(1) == 3 * nh * hd, "qkv / dqkv must be [B*T, 3*nh*hd]");
+  TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == (nh + 2 * nkv) * hd && dqkv.size(0) == B * T && dqkv.size(1) == (nh + 2 * nkv) * hd,
+              "qkv / dqkv must be [B*T, (nh+2*nkv)*hd]");
   TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd && dout.size(0) == B * T && dout.size(1) == nh * hd, "out / dout must be [B*T, nh*hd]");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
   TORCH_CHECK(delta.is_cuda() && delta.scalar_type() == at::kFloat && delta.is_contiguous() && delta.numel() == B * nh * T, "delta must be fp32 [B, nh, T]");
@@ -283,7 +287,7 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0);
   d.dout = dout.data_ptr(); d.ld_dout = dout.stride(0); d.lse = lse.data_ptr<float>(); d.delta = delta.data_ptr<float>();
   d.dqkv = dqkv.data_ptr(); d.ld_dqkv = dqkv.stride(0);
-  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
+  d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.nkv = (int)nkv; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
   if (ds_workspace.has_value()) {
     chk_bf16(*ds_workspace, "ds_workspace");
     TORCH_CHECK(ds_workspace->is_contiguous() && ds_workspace->numel() >= rb::attention_ds_workspace_elems((int)B, (int)T, (int)nh),
@@ -305,17 +309,22 @@ void rope_inplace(Tensor& buf, int64_t T, int64_t n_rot_heads, int64_t hd, int64
                    sin.data_ptr(), backward, (int)pos0, cur_stream());
 }
 
+// dq [B, nh, T, hd]; dk, dv [B, nkv, T, hd] (nkv < 0 means nh), nh % nkv == 0 -> out [B*T, (nh + 2*nkv)*hd]
 void rope_pack_bwd(const Tensor& dq, const Tensor& dk, const Tensor& dv, Tensor& out, int64_t rotary_dim, const Tensor& cos,
-                   const Tensor& sin, int64_t pos0) {
+                   const Tensor& sin, int64_t pos0, int64_t nkv) {
   chk_bf16(dq, "dq"); chk_bf16(dk, "dk"); chk_bf16(dv, "dv"); chk_bf16(out, "out"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(dq.dim() == 4 && dq.stride(3) == 1 && dq.sizes() == dk.sizes() && dq.sizes() == dv.sizes(), "dq/dk/dv must be [B, nh, T, hd]");
-  TORCH_CHECK(dq.strides() == dk.strides() && dq.strides() == dv.strides(), "dq/dk/dv must share strides");
+  TORCH_CHECK(dq.dim() == 4 && dq.stride(3) == 1 && dk.dim() == 4 && dk.sizes() == dv.sizes(), "dq must be [B, nh, T, hd], dk/dv [B, nkv, T, hd]");
   const int B = (int)dq.size(0), nh = (int)dq.size(1), T = (int)dq.size(2), hd = (int)dq.size(3);
-  TORCH_CHECK(out.size(0) == (int64_t)B * T && out.size(1) == 3 * (int64_t)nh * hd, "out must be [B*T, 3*nh*hd]");
+  if (nkv < 0) nkv = nh;
+  TORCH_CHECK(nkv > 0 && nh % nkv == 0 && dk.size(0) == B && dk.size(1) == nkv && dk.size(2) == T && dk.size(3) == hd,
+              "dk/dv must be [B, nkv, T, hd] with nh % nkv == 0");
+  TORCH_CHECK(dk.strides() == dv.strides() && dk.stride(3) == 1, "dk/dv must share strides");
+  TORCH_CHECK(nkv != nh || dq.strides() == dk.strides(), "dq/dk/dv must share strides");
+  TORCH_CHECK(out.size(0) == (int64_t)B * T && out.size(1) == (nh + 2 * nkv) * hd, "out must be [B*T, (nh+2*nkv)*hd]");
   for (const Tensor* t : {&dq, &dk, &dv}) TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, "16-byte alignment required");
   c10::cuda::CUDAGuard guard(out.device());
-  rb::rope_pack_bwd(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), dq.stride(0), dq.stride(1), dq.stride(2), out.data_ptr(), out.stride(0), B, T, nh,
-                    hd, (int)rotary_dim, cos.data_ptr(), sin.data_ptr(), (int)pos0, cur_stream());
+  rb::rope_pack_bwd(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), dq.stride(0), dq.stride(1), dq.stride(2), dk.stride(0), dk.stride(1), dk.stride(2),
+                    out.data_ptr(), out.stride(0), B, T, nh, (int)nkv, hd, (int)rotary_dim, cos.data_ptr(), sin.data_ptr(), (int)pos0, cur_stream());
 }
 
 void swiglu_fwd(const Tensor& gu, Tensor& h, const OptTensor& hd, const OptTensor& seed, int64_t key, double p, const OptTensor& q8,
@@ -709,15 +718,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("n_e4m3") = -1);
   m.def("attention_smem_bytes", [](int64_t hd) { return rb::attention_smem_bytes((int)hd); });
   m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("out"), py::arg("lse"), py::arg("B"), py::arg("T"), py::arg("nh"), py::arg("hd"),
-        py::arg("scale"), py::arg("interleaved") = false);
+        py::arg("scale"), py::arg("interleaved") = false, py::arg("nkv") = -1);
   m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("delta"), py::arg("dqkv"),
         py::arg("B"), py::arg("T"), py::arg("nh"), py::arg("hd"), py::arg("scale"), py::arg("ds_workspace") = py::none(),
-        py::arg("interleaved") = false);
+        py::arg("interleaved") = false, py::arg("nkv") = -1);
   m.def("attention_ds_workspace_elems", &rb::attention_ds_workspace_elems);
   m.def("lora_dx", &lora_dx, py::arg("dy"), py::arg("w"), py::arg("du"), py::arg("a"), py::arg("out"), py::arg("seed"), py::arg("keys"),
         py::arg("p"), py::arg("base") = py::none());
   m.def("rope_inplace", &rope_inplace);
-  m.def("rope_pack_bwd", &rope_pack_bwd);
+  m.def("rope_pack_bwd", &rope_pack_bwd, py::arg("dq"), py::arg("dk"), py::arg("dv"), py::arg("out"), py::arg("rotary_dim"), py::arg("cos"),
+        py::arg("sin"), py::arg("pos0"), py::arg("nkv") = -1);
   m.def("swiglu_fwd", &swiglu_fwd, py::arg("gu"), py::arg("h"), py::arg("hd") = py::none(), py::arg("seed") = py::none(),
         py::arg("key") = 0, py::arg("p") = 0.0, py::arg("q8") = py::none(), py::arg("q_inv_scale") = py::none(), py::arg("q_amax") = py::none());
   m.def("swiglu_bwd", &swiglu_bwd);

@@ -39,10 +39,11 @@ void rope_inplace(void* buf, long long ld, int M, int T, int n_rot_heads, int hd
 
 bool rope_inplace_vec(void* buf, long long ld, int M, int T, int n_rot_heads, int hd, int rotary_dim, const void* cos,
                       const void* sin, bool backward, int pos0, cudaStream_t s);
-// dqkv[b*T+t, which*nh*hd + h*hd + d] <- inverse-rotated dq / dk and dv, each [B, nh, T, hd] with strides (sB, sH, sT, 1)
-void rope_pack_bwd(const void* dq, const void* dk, const void* dv, long long sB, long long sH, long long sT, void* out,
-                   long long ldo, int B, int T, int nh, int hd, int rotary_dim, const void* cos, const void* sin, int pos0,
-                   cudaStream_t s);
+// dqkv[b*T+t, (q: nh | k: nkv | v: nkv) x hd] <- inverse-rotated dq / dk and dv; dq [B, nh, T, hd] with strides (sB, sH, sT, 1),
+// dk and dv [B, nkv, T, hd] with strides (kB, kH, kT, 1); nh % nkv == 0
+void rope_pack_bwd(const void* dq, const void* dk, const void* dv, long long sB, long long sH, long long sT, long long kB, long long kH,
+                   long long kT, void* out, long long ldo, int B, int T, int nh, int nkv, int hd, int rotary_dim, const void* cos,
+                   const void* sin, int pos0, cudaStream_t s);
 
 // ---- SwiGLU --------------------------------------------------------------------------------
 // gu: [M, 2F] (gate | up) -> h[M, F] = silu(gate) * up

@@ -1,7 +1,7 @@
 // Rotary position embedding kernels with 128-bit accesses.
 //   rope_inplace_vec : in-place rotation of q,k heads inside the packed [tokens, 3h] QKV buffer (forward / backward)
-//   rope_pack_bwd    : attention-backward epilogue: gathers dq, dk, dv ([B, nh, T, hd], arbitrary batch/head/token strides)
-//                      into the packed dQKV buffer and applies the inverse rotation to dq, dk on the way
+//   rope_pack_bwd    : attention-backward epilogue: gathers dq [B, nh, T, hd], dk, dv [B, nkv, T, hd] (arbitrary batch/head/token
+//                      strides) into the packed dQKV buffer [q: nh | k: nkv | v: nkv] and applies the inverse rotation to dq, dk on the way
 //                      (replaces three strided copies + an in-place rotation pass).
 // Half-rotation layout (reference modeling_llama.py:126-141): y1 = x1 c - x2 s, y2 = x2 c + x1 s; backward uses -s.
 #include "common.cuh"
@@ -59,14 +59,15 @@ bool rope_inplace_vec(void* buf, long long ld, int M, int T, int n_rot_heads, in
   return true;
 }
 
+// one thread per 8 columns of a query head; the threads of heads h < nkv also carry KV head h
 __global__ void __launch_bounds__(256) rope_pack_bwd_kernel(const bf16* __restrict__ dq, const bf16* __restrict__ dk, const bf16* __restrict__ dv,
-                                                            long long sB, long long sH, long long sT, bf16* __restrict__ out, long long ldo,
-                                                            long long total, int T, int nh, int hd, int half, const bf16* __restrict__ cosp,
-                                                            const bf16* __restrict__ sinp, int pos0) {
+                                                            long long sB, long long sH, long long sT, long long kB, long long kH, long long kT,
+                                                            bf16* __restrict__ out, long long ldo, long long total, int T, int nh, int nkv, int hd,
+                                                            int half, const bf16* __restrict__ cosp, const bf16* __restrict__ sinp, int pos0) {
   pdl_wait();
   pdl_launch_dependents();
   const int nv = hd / 8, nr = half / 8;
-  const long long hsz = (long long)nh * hd;
+  const long long qsz = (long long)nh * hd, ksz = (long long)nkv * hd;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int j = int(i % nv);
     const long long t = i / nv;
@@ -74,9 +75,11 @@ __global__ void __launch_bounds__(256) rope_pack_bwd_kernel(const bf16* __restri
     const long long row = t / nh;
     const long long b = row / T, tt = row % T;
     const long long src = b * sB + h * sH + tt * sT + j * 8;
+    const long long ksrc = b * kB + h * kH + tt * kT + j * 8;
+    const bool kv = h < nkv;
     bf16* o = out + row * ldo + (long long)h * hd + j * 8;
     // v: plain gather
-    *reinterpret_cast<uint4*>(o + 2 * hsz) = *reinterpret_cast<const uint4*>(dv + src);
+    if (kv) *reinterpret_cast<uint4*>(o + qsz + ksz) = *reinterpret_cast<const uint4*>(dv + ksrc);
     if (j < nr) {
       const int pos = int(tt) + pos0;
       const uint4 c = *reinterpret_cast<const uint4*>(cosp + (long long)pos * 2 * half + j * 8);
@@ -85,25 +88,29 @@ __global__ void __launch_bounds__(256) rope_pack_bwd_kernel(const bf16* __restri
       rotate8(*reinterpret_cast<const uint4*>(dq + src), *reinterpret_cast<const uint4*>(dq + src + half), c, s, -1.f, oa, ob);
       *reinterpret_cast<uint4*>(o) = oa;
       *reinterpret_cast<uint4*>(o + half) = ob;
-      rotate8(*reinterpret_cast<const uint4*>(dk + src), *reinterpret_cast<const uint4*>(dk + src + half), c, s, -1.f, oa, ob);
-      *reinterpret_cast<uint4*>(o + hsz) = oa;
-      *reinterpret_cast<uint4*>(o + hsz + half) = ob;
+      if (kv) {
+        rotate8(*reinterpret_cast<const uint4*>(dk + ksrc), *reinterpret_cast<const uint4*>(dk + ksrc + half), c, s, -1.f, oa, ob);
+        *reinterpret_cast<uint4*>(o + qsz) = oa;
+        *reinterpret_cast<uint4*>(o + qsz + half) = ob;
+      }
     } else if (j >= 2 * nr) {  // dims beyond the rotary part pass through
       *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(dq + src);
-      *reinterpret_cast<uint4*>(o + hsz) = *reinterpret_cast<const uint4*>(dk + src);
+      if (kv) *reinterpret_cast<uint4*>(o + qsz) = *reinterpret_cast<const uint4*>(dk + ksrc);
     }
   }
 }
 
-void rope_pack_bwd(const void* dq, const void* dk, const void* dv, long long sB, long long sH, long long sT, void* out, long long ldo, int B,
-                   int T, int nh, int hd, int rotary_dim, const void* cos, const void* sin, int pos0, cudaStream_t s) {
+void rope_pack_bwd(const void* dq, const void* dk, const void* dv, long long sB, long long sH, long long sT, long long kB, long long kH,
+                   long long kT, void* out, long long ldo, int B, int T, int nh, int nkv, int hd, int rotary_dim, const void* cos,
+                   const void* sin, int pos0, cudaStream_t s) {
   const int half = rotary_dim / 2;
-  if (half % 8 != 0 || hd % 8 != 0 || ldo % 8 != 0 || sB % 8 != 0 || sH % 8 != 0 || sT % 8 != 0)
+  if (half % 8 != 0 || hd % 8 != 0 || ldo % 8 != 0 || sB % 8 != 0 || sH % 8 != 0 || sT % 8 != 0 || kB % 8 != 0 || kH % 8 != 0 || kT % 8 != 0)
     throw std::runtime_error("rope_pack_bwd: head_dim / rotary_dim / strides must allow 128-bit accesses");
+  if (nkv <= 0 || nkv > nh || nh % nkv != 0) throw std::runtime_error("rope_pack_bwd: nh must be a multiple of nkv");
   const long long total = (long long)B * T * nh * (hd / 8);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 16);
-  launch_k(rope_pack_bwd_kernel, grid, 256, 0, s, (const bf16*)dq, (const bf16*)dk, (const bf16*)dv, sB, sH, sT, (bf16*)out, ldo, total, T, nh, hd,
-                                            half, (const bf16*)cos, (const bf16*)sin, pos0);
+  launch_k(rope_pack_bwd_kernel, grid, 256, 0, s, (const bf16*)dq, (const bf16*)dk, (const bf16*)dv, sB, sH, sT, kB, kH, kT, (bf16*)out, ldo,
+                                            total, T, nh, nkv, hd, half, (const bf16*)cos, (const bf16*)sin, pos0);
   RB_CHECK_LAUNCH("rope_pack_bwd");
 }
 

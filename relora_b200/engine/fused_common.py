@@ -53,10 +53,14 @@ class FusedStepperBase:
         self.trainable_names = [n for n, _ in named]
         self.lora_params = [p for n, p in named if "lora_" in n]
 
-    def _stacked_view(self, p, rows_mult: int = 1):
-        """(params, grads) views over ``rows_mult`` adjacent parameters of the flat store, starting at ``p``."""
+    def _stacked_view(self, p, rows_mult: int = 1, rows: Optional[int] = None):
+        """(params, grads) views over ``rows_mult`` adjacent parameters of the flat store, starting at ``p``; or, with ``rows``,
+        over adjacent 2-D parameters of ``p``'s width and ``rows`` rows in all (blocks of unequal row counts, such as the LoRA
+        B factors of q | k | v under grouped-query attention)."""
         o, n = self.store.segment(p)
         ps = self.store.storage.get(id(p), tuple(p.shape))  # padded block shape where one exists
+        if rows is not None:
+            return self.store.params[o:o + rows * ps[1]].view(rows, ps[1]), self.store.grads[o:o + rows * ps[1]].view(rows, ps[1])
         shape = (ps[0] * rows_mult, ps[1]) if p.dim() == 2 else (ps[0] * rows_mult,)
         tot = n * rows_mult
         return self.store.params[o:o + tot].view(shape), self.store.grads[o:o + tot].view(shape)
@@ -97,8 +101,11 @@ class FusedStepperBase:
         raise NotImplementedError
 
     # ------------------------------------------------------------------ LoRA groups
-    def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False, bias=None):
+    def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False, bias=None, Nq=None):
         """u = s·xd_g·A_gᵀ (grouped) ; out = [xn | u]·[W | B]ᵀ (+ bias) (+ residual).
+
+        ``Nq``: width of the first group when it differs from the other G-1 groups' ``Ng`` (the q | k | v projections of
+        grouped-query attention); its output columns and the rest are then two launches into column windows of ``out``.
 
         fp8 path (``site = (layer, index)``): xn is quantised to E4M3 with the site's delayed scale and multiplied with the E4M3
         copy of W on the kind::f8f6f4 tensor-core path; the bf16 LoRA term shares the accumulator, so u is produced pre-divided
@@ -117,25 +124,46 @@ class FusedStepperBase:
               fp8=True, alpha_dev=self.alpha_main[l, s_i:s_i + 1])
             return
         g(xd, A, u, M=M, N=G * r, K1=K, n_per_group=r, a1_group_kofs=K if drop else 0, alpha=self.scale)
+        if Nq is not None and Nq != Ng:
+            assert residual is None and bias is None and G > 1
+            g(xn, W[:Nq], out[:, :Nq], M=M, N=Nq, K1=K, a2=u[:, :r], b2=B[:Nq], K2=r)
+            g(xn, W[Nq:], out[:, Nq:], M=M, N=(G - 1) * Ng, K1=K, a2=u[:, r:], b2=B[Nq:], K2=r, n_per_group=Ng, a2_group_kofs=r)
+            return
         g(xn, W, out, M=M, N=G * Ng, K1=K, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, residual=residual, bias=bias)
 
-    def _lora_group_bwd(self, dy, S_B, S_W, S_A, gA, gB, xd, u, keys, *, G, K, Ng, base_out, out, tag, site=None):
+    def _lora_group_bwd(self, dy, S_B, S_W, S_A, gA, gB, xd, u, keys, *, G, K, Ng, base_out, out, tag, site=None, Nq=None):
         """Backward of one stacked LoRA group.  dy [M, G·Ng] -> out [M, K] (grad of the group's input).
+
+        ``Nq`` (see ``_lora_group_fwd``): dy is [M, Nq + (G-1)·Ng]; du and dB then run as two launches each, the first group
+        alone and the other G-1 groups together.
 
         The two weight-gradient GEMMs only read (dy, du, xd, u), so they are forked onto a side stream and fill the
         SMs that the skinny du / parts GEMMs and kernel tails of the main chain leave idle; ``self._wg_done[tag]``
         is the event the main stream waits on before it overwrites one of their inputs (see ``_backward``)."""
         C, g, M, r, s = self.C, fused.gemm, self.M_, self.r, self.scale
         du = self.du_bufs[tag]
-        # du_g = s · dy_g · B_g          (B stacked [G·Ng, r], read MN-major; K window g·Ng)
-        g(dy, S_B, du, M=M, N=G * r, K1=Ng, b1_mn=True, n_per_group=r, a1_group_kofs=Ng if G > 1 else 0,
-          b1_group_kofs=Ng if G > 1 else 0, b1_local_n=True, alpha=s)
+        split = Nq is not None and Nq != Ng
+        width = Nq + (G - 1) * Ng if split else G * Ng
+        if split:
+            assert G > 1 and not (self.fp8 and site is not None)
+            g(dy[:, :Nq], S_B[:Nq], du[:, :r], M=M, N=r, K1=Nq, b1_mn=True, alpha=s)
+            g(dy[:, Nq:], S_B[Nq:], du[:, r:], M=M, N=(G - 1) * r, K1=Ng, b1_mn=True, n_per_group=r, a1_group_kofs=Ng,
+              b1_group_kofs=Ng, b1_local_n=True, alpha=s)
+        else:
+            # du_g = s · dy_g · B_g          (B stacked [G·Ng, r], read MN-major; K window g·Ng)
+            g(dy, S_B, du, M=M, N=G * r, K1=Ng, b1_mn=True, n_per_group=r, a1_group_kofs=Ng if G > 1 else 0,
+              b1_group_kofs=Ng if G > 1 else 0, b1_local_n=True, alpha=s)
         drop = self.p > 0
         shared_x = (not drop) or xd.shape[1] != G * K
 
         def wgrads():  # fp32, accumulated across micro-batches, split-K over tokens
             g(du, xd, gA, M=G * r, N=K, K1=M, a1_mn=True, b1_mn=True, accumulate=True, split_k=self.wgrad_split_k,
               m_per_group=r if G > 1 else 0, b1_mn_ofs_per_mgroup=0 if shared_x else K)
+            if split:
+                g(dy[:, :Nq], u[:, :r], gB[:Nq], M=Nq, N=r, K1=M, a1_mn=True, b1_mn=True, accumulate=True, split_k=self.wgrad_split_k)
+                g(dy[:, Nq:], u[:, r:], gB[Nq:], M=(G - 1) * Ng, N=r, K1=M, a1_mn=True, b1_mn=True, accumulate=True,
+                  split_k=self.wgrad_split_k, m_per_group=Ng, b1_mn_ofs_per_mgroup=r)
+                return
             # fp8 path: the saved u is u / (s_x·s_w); the product scale is multiplied back here
             g(dy, u, gB, M=G * Ng, N=r, K1=M, a1_mn=True, b1_mn=True, accumulate=True, split_k=self.wgrad_split_k,
               m_per_group=Ng if G > 1 else 0, b1_mn_ofs_per_mgroup=r if G > 1 else 0,
@@ -152,25 +180,25 @@ class FusedStepperBase:
             self._wg_done[tag] = done
         if self.fused_dx:
             sd, ks, pp = (self.seed, list(keys), self.p) if drop else (None, [0] * G, 0.0)
-            if G * Ng >= self.dx_split_k:
+            if width >= self.dx_split_k:
                 # long reductions: the frozen-path product runs on the GEMM, whose TMA-store epilogue overlaps the next
                 # tile's k-loop, then one light pass adds the masked low-rank terms
                 if self.fp8_bwd and site is not None:
                     # E5M2 copy of the output gradient (delayed scale) x E4M3 copy of Wᵀ on the kind::f8f6f4 path
                     l_, s_i = site
-                    dy8 = self.dy8[G * Ng]
+                    dy8 = self.dy8[width]
                     C.fp8_quantize_act(dy, dy8, self._inv_sx2[1, l_, s_i:s_i + 1], self._act_state2[1, l_, s_i, 1:2], True)
                 if self.fp8_bwd and site is not None and self._fp8_bwd_calibrated:
                     g(dy8, self.W8T[s_i][l_], base_out, M=M, N=K, K1=G * Ng, fp8=2, alpha_dev=self._alpha_main2[1, l_, s_i:s_i + 1])
                 else:
-                    g(dy, S_W, base_out, M=M, N=K, K1=G * Ng, b1_mn=True)
+                    g(dy, S_W, base_out, M=M, N=K, K1=width, b1_mn=True)
                 C.lora_dx(None, None, du, S_A, out, sd, ks, pp, base_out)
             else:
                 # one kernel: out = dy·W + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)  (masked LoRA terms folded into the register accumulator)
                 C.lora_dx(dy, S_W, du, S_A, out, sd, ks, pp)
         else:
             # frozen path: base = dy · W     (W stacked [G·Ng, K], read MN-major)
-            g(dy, S_W, base_out, M=M, N=K, K1=G * Ng, b1_mn=True)
+            g(dy, S_W, base_out, M=M, N=K, K1=width, b1_mn=True)
             # low-rank path per group: part_g = du_g · A_g
             parts = self.parts.view(-1)[: M * G * K].view(M, G * K)
             g(du, S_A, parts, M=M, N=G * K, K1=r, b1_mn=True, n_per_group=K, a1_group_kofs=r if G > 1 else 0,

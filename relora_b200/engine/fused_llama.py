@@ -4,9 +4,10 @@ The reference executes one ``ReLoRaLinear`` as ~8 eager kernels (``relora.py:319
 layer as ~100 (``modeling_llama.py:243-308``), re-reading every activation several times, and is
 launch/CPU-bound at the 250M scale.  This executor instead
 
-* keeps the frozen weights of a layer *stacked* (``Wqkv [3h,h]``, ``Wgu [2f,h]``) and the LoRA factors
-  stacked alongside (``A_qkv [3r,h]``, ``B_qkv [3h,r]`` …) — the ``nn.Module`` parameters are views into these
-  buffers, so checkpoints keep the reference layout;
+* keeps the frozen weights of a layer *stacked* (``Wqkv [h + 2·kv, h]`` with kv = nkv·head_dim, i.e. ``[3h, h]`` without
+  grouped-query attention; ``Wgu [2f,h]``) and the LoRA factors stacked alongside (``A_qkv [3r,h]``, ``B_qkv [h + 2·kv, r]`` …) —
+  the ``nn.Module`` parameters are views into these buffers, so checkpoints keep the reference layout.  Under grouped-query
+  attention the q group and the equal-width k | v groups of the stacked projections run as two launches into column windows;
 * runs every projection as ONE wgmma GEMM launch with the low-rank up-projection folded into the K loop
   (``y = [x | u]·[W | B]ᵀ``, residual add in the epilogue), the three / two down-projections of a stacked group
   as one grouped launch, and all backward GEMMs (``dx``, ``du``, stacked ``dA`` / ``dB`` with split-K) on the same
@@ -28,7 +29,7 @@ from typing import Dict, List, Tuple
 import torch
 import torch.nn.functional as F_
 
-from ..models.llama import LlamaForCausalLM
+from ..models.llama import LlamaForCausalLM, num_kv_heads
 from ..ops import fused, native
 from ..parallel.dist import DistInfo
 from ..parallel.grad_sync import broadcast_params
@@ -48,8 +49,14 @@ def supports(model, args=None) -> Tuple[bool, str]:
         return False, "lora_only / trainable scaling / quantized frozen weights use the module path"
     cfg = inner.config
     h, f, nh = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads
+    nkv = num_kv_heads(cfg)
     r = model.r
     hd = h // nh
+    if nkv != nh:
+        if nkv * hd % 128:
+            return False, f"grouped-query attention needs num_key_value_heads x head_dim ({nkv} x {hd}) to be a multiple of 128"
+        if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+            return False, "--frozen_dtype fp8 with grouped-query attention uses the module path (the fp8 weight copies are [3h, h])"
     if h % 128 or r % 128:
         # the intermediate size may be anything (llama_1b: 5461): its buffers are zero-padded to a multiple of 128
         return False, f"hidden ({h}) and rank ({r}) must be multiples of 128 for stacked groups"
@@ -81,6 +88,8 @@ class FusedLlamaStepper(FusedStepperBase):
         ok, why = supports(model)
         if not ok:
             raise RuntimeError(why)
+        if fp8 and num_kv_heads(model.wrapped_model.config) != model.wrapped_model.config.num_attention_heads:
+            raise RuntimeError("--frozen_dtype fp8 with grouped-query attention uses the module path (the fp8 weight copies are [3h, h])")
         self.model, self.info = model, info
         self.inner: LlamaForCausalLM = model.wrapped_model
         self.C = fused._C()
@@ -91,6 +100,9 @@ class FusedLlamaStepper(FusedStepperBase):
         cfg = self.inner.config
         self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
         self.hd = self.h // self.nh
+        self.nkv = num_kv_heads(cfg)
+        self.kv = self.nkv * self.hd  # width of the k and v projections (h without grouped-query attention)
+        self.qkv_w = self.h + 2 * self.kv  # packed [q | k | v] row
         self.fp = (self.f + 127) // 128 * 128  # padded intermediate size (zero rows / columns keep every GEMM extent a multiple of the 128-wide tile)
         self.r = model.r
         self.L = cfg.num_hidden_layers
@@ -103,7 +115,8 @@ class FusedLlamaStepper(FusedStepperBase):
         # ---------------------------------------------------------------- stacked frozen weights
         dev = self.device
         h, f, fp, r, L = self.h, self.f, self.fp, self.r, self.L
-        self.Wqkv = torch.empty(L, 3 * h, h, dtype=BF, device=dev)
+        kv = self.kv
+        self.Wqkv = torch.empty(L, h + 2 * kv, h, dtype=BF, device=dev)
         self.Wo = torch.empty(L, h, h, dtype=BF, device=dev)
         self.Wgu = torch.zeros(L, 2 * fp, h, dtype=BF, device=dev)
         self.Wd = torch.zeros(L, h, fp, dtype=BF, device=dev)
@@ -111,8 +124,8 @@ class FusedLlamaStepper(FusedStepperBase):
         with torch.no_grad():
             for l, layer in enumerate(layers):
                 at, mlp = layer.self_attn, layer.mlp
-                for j, m in enumerate((at.q_proj, at.k_proj, at.v_proj)):
-                    self._rehome(m.weight, self.Wqkv[l, j * h:(j + 1) * h])
+                for m, r0, r1 in ((at.q_proj, 0, h), (at.k_proj, h, h + kv), (at.v_proj, h + kv, h + 2 * kv)):
+                    self._rehome(m.weight, self.Wqkv[l, r0:r1])
                 self._rehome(at.o_proj.weight, self.Wo[l])
                 self._rehome(mlp.gate_proj.weight, self.Wgu[l, :f])
                 self._rehome(mlp.up_proj.weight, self.Wgu[l, fp:fp + f])
@@ -161,7 +174,7 @@ class FusedLlamaStepper(FusedStepperBase):
             l = len(self.layers)
             S.Wqkv, S.Wo, S.Wgu, S.Wd = self.Wqkv[l], self.Wo[l], self.Wgu[l], self.Wd[l]
             S.A_qkv, S.gA_qkv = pv(at.q_proj.lora_A.weight, 3)
-            S.B_qkv, S.gB_qkv = pv(at.q_proj.lora_B.weight, 3)
+            S.B_qkv, S.gB_qkv = pv(at.q_proj.lora_B.weight, 3) if kv == h else pv(at.q_proj.lora_B.weight, rows=h + 2 * kv)
             S.A_o, S.gA_o = pv(at.o_proj.lora_A.weight)
             S.B_o, S.gB_o = pv(at.o_proj.lora_B.weight)
             S.A_gu, S.gA_gu = pv(mlp.gate_proj.lora_A.weight, 2)
@@ -177,6 +190,7 @@ class FusedLlamaStepper(FusedStepperBase):
             S.mods = (at.q_proj, at.k_proj, at.v_proj, at.o_proj, mlp.gate_proj, mlp.up_proj, mlp.down_proj)
             # sanity: the stacked views must alias the module parameters
             assert S.A_qkv[r:2 * r].data_ptr() == at.k_proj.lora_A.weight.data_ptr()
+            assert S.B_qkv[h + kv:].data_ptr() == at.v_proj.lora_B.weight.data_ptr() and S.B_qkv.shape == (h + 2 * kv, r)
             assert S.B_gu[fp:].data_ptr() == mlp.up_proj.lora_B.weight.data_ptr()
             assert S.A_d.data_ptr() == mlp.down_proj.lora_A.weight.data_ptr() and S.A_d.shape == (r, fp)
             # (B, A, W) blocks of the merge GEMM  W += s·B·A  (padded blocks where the module views are strided)
@@ -276,7 +290,7 @@ class FusedLlamaStepper(FusedStepperBase):
         self.u_o = e(L, M, r)
         self.u_gu = e(L, M, 2 * r)
         self.u_d = e(L, M, r)
-        self.qkv = e(L, M, 3 * h)
+        self.qkv = e(L, M, self.qkv_w)
         self.gu = e(L, M, 2 * f)
         # transients
         self.xn = e(M, h)
@@ -285,7 +299,7 @@ class FusedLlamaStepper(FusedStepperBase):
         self.dxf = e(M, h)
         self.dx_a, self.dx_b, self.dxn, self.dxn2 = e(M, h), e(M, h), e(M, h), e(M, h)
         self.dattn = e(M, h)
-        self.dqkv = e(M, 3 * h)
+        self.dqkv = e(M, self.qkv_w)
         self.dgu = e(M, 2 * f)
         self.dhmid, self.dhmid2 = e(M, f), e(M, f)
         self.du_bufs = {"d": e(M, r), "gu": e(M, 2 * r), "o": e(M, r), "qkv": e(M, 3 * r)}
@@ -313,17 +327,26 @@ class FusedLlamaStepper(FusedStepperBase):
             # wgmma flash attention straight out of the packed projection buffer (csrc/attention.cu); the output and the
             # log-sum-exp of the layer are what the backward kernels need
             out = self.attn_o[sl]
-            self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd))
+            if self.nkv == nh:
+                self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd))
+            else:
+                self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd), nkv=self.nkv)
             return out
-        v5 = qkv.view(B, T, 3, nh, hd)
-        q, k, v = (v5[:, :, i].transpose(1, 2) for i in range(3))
+        if self.nkv == nh:
+            v5 = qkv.view(B, T, 3, nh, hd)
+            q, k, v = (v5[:, :, i].transpose(1, 2) for i in range(3))
+            gqa = {}
+        else:  # [q: nh | k: nkv | v: nkv] heads of the packed row
+            v3 = qkv.view(B, T, nh + 2 * self.nkv, hd)
+            q, k, v = (v3[:, :, a:b].transpose(1, 2) for a, b in ((0, nh), (nh, nh + self.nkv), (nh + self.nkv, nh + 2 * self.nkv)))
+            gqa = {"enable_gqa": True}
         if train:
             q, k, v = (t.detach().requires_grad_() for t in (q, k, v))
             with torch.enable_grad():
-                o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True)
+                o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **gqa)
             self._attn_saved.append((o, q, k, v))
         else:
-            o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True)
+            o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **gqa)
         return o.detach().transpose(1, 2).reshape(self.M_, self.h)
 
     def _q8(self, l, s_i, K):
@@ -354,8 +377,9 @@ class FusedLlamaStepper(FusedStepperBase):
                 xn = xn if xn.is_contiguous() else self.xn
                 C.rmsnorm_fwd(x, S.w1, xn, self.rstd1[sl], self.eps, None, None, [], 0.0)
                 xd = xn
-            self._lora_group_fwd(xn, xd, S.A_qkv, S.B_qkv, S.Wqkv, self.u_qkv[sl], qkv, G=3, K=h, Ng=h, site=(l, 0), prequant=p > 0)
-            C.rope_inplace(qkv, self.T_, 2 * self.nh, self.hd, self.hd, self.cos, self.sin, False, 0)
+            self._lora_group_fwd(xn, xd, S.A_qkv, S.B_qkv, S.Wqkv, self.u_qkv[sl], qkv, G=3, K=h, Ng=self.kv, site=(l, 0),
+                                 prequant=p > 0, Nq=h)
+            C.rope_inplace(qkv, self.T_, self.nh + self.nkv, self.hd, self.hd, self.cos, self.sin, False, 0)
             attn = self._attention(qkv, train, sl)
             if p > 0:
                 xd_o = self.xd_o[sl]
@@ -411,9 +435,13 @@ class FusedLlamaStepper(FusedStepperBase):
                                  G=1, K=h, Ng=h, base_out=self.dxn, out=self.dattn, tag="o", site=(l, 1))
             if self.native_attn:
                 self._join("qkv")  # the previous layer's qkv weight gradients read dqkv / du_qkv
-                C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
-                                1.0 / math.sqrt(hd))
-                C.rope_inplace(self.dqkv, T, 2 * nh, hd, hd, self.cos, self.sin, True, 0)  # back through the rotation of q, k
+                if self.nkv == nh:
+                    C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
+                                    1.0 / math.sqrt(hd))
+                else:
+                    C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
+                                    1.0 / math.sqrt(hd), nkv=self.nkv)
+                C.rope_inplace(self.dqkv, T, nh + self.nkv, hd, hd, self.cos, self.sin, True, 0)  # back through the rotation of q, k
                 dq = None
             else:
                 o, q, k, v = self._attn_saved[l]
@@ -421,14 +449,19 @@ class FusedLlamaStepper(FusedStepperBase):
                 self._join("qkv")  # the previous layer's qkv weight gradients read dqkv / du_qkv
             if dq is None:
                 pass
-            elif dq.stride() == dk.stride() == dv.stride() and dq.stride(3) == 1:
+            elif self.nkv == nh and dq.stride() == dk.stride() == dv.stride() and dq.stride(3) == 1:
                 C.rope_pack_bwd(dq, dk, dv, self.dqkv, hd, self.cos, self.sin, 0)  # gather + inverse rotation in one pass
+            elif self.nkv != nh and dk.stride() == dv.stride() and dq.stride(3) == 1 and dk.stride(3) == 1:
+                C.rope_pack_bwd(dq, dk, dv, self.dqkv, hd, self.cos, self.sin, 0, nkv=self.nkv)
             else:
-                d5 = self.dqkv.view(B, T, 3, nh, hd)
-                d5[:, :, 0].copy_(dq.transpose(1, 2)); d5[:, :, 1].copy_(dk.transpose(1, 2)); d5[:, :, 2].copy_(dv.transpose(1, 2))
-                C.rope_inplace(self.dqkv, T, 2 * nh, hd, hd, self.cos, self.sin, True, 0)
+                nkv = self.nkv
+                d3 = self.dqkv.view(B, T, nh + 2 * nkv, hd)
+                d3[:, :, :nh].copy_(dq.transpose(1, 2))
+                d3[:, :, nh:nh + nkv].copy_(dk.transpose(1, 2))
+                d3[:, :, nh + nkv:].copy_(dv.transpose(1, 2))
+                C.rope_inplace(self.dqkv, T, nh + nkv, hd, hd, self.cos, self.sin, True, 0)
             self._lora_group_bwd(self.dqkv, S.B_qkv, S.Wqkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd_qkv[l], self.u_qkv[l],
-                                 S.keys_qkv, G=3, K=h, Ng=h, base_out=self.dxn, out=self.dxn2, tag="qkv", site=(l, 0))
+                                 S.keys_qkv, G=3, K=h, Ng=self.kv, base_out=self.dxn, out=self.dxn2, tag="qkv", site=(l, 0), Nq=h)
             self._join("d")  # this layer's down_proj weight gradients read the buffer written next
             C.rmsnorm_bwd(self.dxn2, self.x_in[l], S.w1, self.rstd1[l], dx, dx_other, S.gw1, ws, tk)
             dx, dx_other = dx_other, dx

@@ -71,6 +71,22 @@ class _DeviceTimer:
         return time.perf_counter() - self._t0
 
 
+def pretrained_model(path: str, revision: Optional[str] = None):
+    """The model of a local checkpoint directory, by the ``model_type`` of its ``config.json``: ``llama`` (Llama-family
+    checkpoints, grouped-query attention included) or ``gpt_neox`` (Pythia)."""
+    cfg_file = os.path.join(path, "config.json")
+    if os.path.isdir(path) and os.path.exists(cfg_file):
+        import json
+
+        with open(cfg_file) as f:
+            model_type = json.load(f).get("model_type")
+        if model_type == "llama":
+            return LlamaForCausalLM.from_pretrained(path)
+        if model_type != "gpt_neox":
+            raise NotImplementedError(f"model_type {model_type!r} in {cfg_file}: only llama and gpt_neox checkpoints are supported")
+    return GPTNeoXForCausalLM.from_pretrained(path, revision=revision)
+
+
 def _max_over_ranks(x: float, device) -> float:
     if dist.is_initialized() and dist.get_world_size() > 1:
         t = torch.tensor([x], dtype=torch.float64, device=device if device.type == "cuda" else "cpu")
@@ -121,7 +137,7 @@ def _build_data(args, info, state_update_step: int):
     """Return ``(train_loader, eval_loader, test_loader, prep_args, vocab_size_or_None)``."""
     if args.synthetic_data is not None:
         n = int(args.synthetic_data)
-        cfg = load_config(args.model_config)
+        cfg = load_config(args.model_config or args.model_name_or_path)
         train = SyntheticTokens(n, args.max_length, cfg.vocab_size, seed=args.seed + 1)
         val = SyntheticTokens(max(args.batch_size * info.world_size * 2, 64), args.max_length, cfg.vocab_size, seed=args.seed + 2)
         check_dataset_size(len(train), args.max_length, args.total_batch_size, args.num_training_steps, args.parity_quirks)
@@ -248,7 +264,7 @@ def run(args) -> dict:
         model = LlamaForCausalLM(model_config)
     else:
         logger.info(f"Using pretrained model {args.model_name_or_path} revision {args.model_revision}")
-        model = GPTNeoXForCausalLM.from_pretrained(args.model_name_or_path, revision=args.model_revision)
+        model = pretrained_model(args.model_name_or_path, args.model_revision)
         model_config = model.config
 
     if args.warmed_up_model is not None:

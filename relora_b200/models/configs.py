@@ -11,7 +11,7 @@ import json
 import os
 from typing import Any, Dict
 
-__all__ = ["load_config", "save_config", "SimpleConfig", "config_to_dict"]
+__all__ = ["load_config", "save_config", "SimpleConfig", "config_to_dict", "rope_settings"]
 
 _LLAMA_DEFAULTS = dict(
     model_type="llama",
@@ -29,6 +29,7 @@ _LLAMA_DEFAULTS = dict(
     bos_token_id=1,
     eos_token_id=2,
     tie_word_embeddings=False,
+    rope_theta=10000.0,
 )
 
 _NEOX_DEFAULTS = dict(
@@ -68,6 +69,8 @@ class SimpleConfig:
             setattr(self, k, v)
         for k, v in kw.items():
             setattr(self, k, v)
+        if mt == "llama" and getattr(self, "num_key_value_heads", None) is None:
+            self.num_key_value_heads = self.num_attention_heads  # multi-head attention unless the config says otherwise
 
     def to_dict(self) -> Dict[str, Any]:
         return copy.deepcopy(self.__dict__)
@@ -111,6 +114,23 @@ def load_config(path: str, prefer_hf: bool = True):
         except Exception:
             pass
     return SimpleConfig(**raw)
+
+
+def rope_settings(config):
+    """(rotary fraction, base, scaling dict) from either config dialect: the classic GPT-NeoX fields ``rotary_pct`` /
+    ``rotary_emb_base`` / ``rope_scaling`` (modeling_pythia.py:95-106 of the reference, checkpoints' ``config.json``; Llama has ``rope_theta``) or the
+    ``rope_parameters`` dict that transformers >= 5 folds them into (``partial_rotary_factor``, ``rope_theta``, ``rope_type``, ``factor``)."""
+    rp = getattr(config, "rope_parameters", None) or {}
+    pct = getattr(config, "rotary_pct", None)
+    if pct is None:
+        pct = rp.get("partial_rotary_factor", getattr(config, "partial_rotary_factor", 0.25))
+    base = getattr(config, "rotary_emb_base", None)
+    if base is None:
+        base = rp.get("rope_theta", getattr(config, "rope_theta", 10000))
+    scaling = getattr(config, "rope_scaling", None)
+    if (scaling is None or not scaling.get("type", scaling.get("rope_type"))) and rp.get("rope_type") not in (None, "default"):
+        scaling = {"type": rp["rope_type"], "factor": rp.get("factor", 1.0)}
+    return float(pct), base, scaling
 
 
 def config_to_dict(config) -> Dict[str, Any]:

@@ -9,6 +9,11 @@ This is a plain ``nn.Module`` tree (no ``PreTrainedModel`` machinery); ``save_pr
 ``from_pretrained`` read and write the reference checkpoint layout (``config.json`` +
 ``pytorch_model.bin``).  State-dict keys match the reference exactly, including the persistent
 ``rotary_emb.inv_freq`` buffers, so checkpoints are interchangeable in both directions.
+``from_pretrained`` also reads Hugging Face Llama-family checkpoint directories (``model.safetensors``, or a
+sharded ``*.index.json`` of either format), which carry no ``inv_freq`` buffers.
+
+Grouped-query attention (``num_key_value_heads < num_attention_heads``) and ``rope_theta`` are supported; rotary
+scaling, tied embeddings and biased projections are refused (:func:`check_llama_config`).
 
 Two execution paths share these parameters:
 
@@ -29,7 +34,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .configs import load_config, save_config
+from .configs import load_config, rope_settings, save_config
 
 __all__ = [
     "LlamaRMSNorm",
@@ -44,6 +49,9 @@ __all__ = [
     "SequenceClassifierOutput",
     "rotate_half",
     "apply_rotary_pos_emb",
+    "repeat_kv",
+    "check_llama_config",
+    "num_kv_heads",
 ]
 
 
@@ -138,6 +146,38 @@ def apply_rotary_pos_emb(q, k, cos, sin, position_ids):
     return (q * cos) + (rotate_half(q) * sin), (k * cos) + (rotate_half(k) * sin)
 
 
+def repeat_kv(x: torch.Tensor, n_rep: int) -> torch.Tensor:
+    """[B, nkv, T, hd] -> [B, nkv·n_rep, T, hd]: KV head j serves query heads j·n_rep .. (j+1)·n_rep - 1."""
+    if n_rep == 1:
+        return x
+    B, nkv, T, hd = x.shape
+    return x[:, :, None].expand(B, nkv, n_rep, T, hd).reshape(B, nkv * n_rep, T, hd)
+
+
+def num_kv_heads(config) -> int:
+    return getattr(config, "num_key_value_heads", None) or config.num_attention_heads
+
+
+def check_llama_config(config) -> None:
+    """Refuse the Llama-family options this model does not implement; the error names the config field."""
+    h, nh, nkv = config.hidden_size, config.num_attention_heads, num_kv_heads(config)
+    scaling = rope_settings(config)[2]
+    if scaling is not None and scaling.get("type", scaling.get("rope_type")) not in (None, "default"):
+        raise ValueError(f"rope_scaling={scaling} is not supported (only unscaled rotary embeddings)")
+    if getattr(config, "tie_word_embeddings", False):
+        raise ValueError("tie_word_embeddings=True is not supported: lm_head and embed_tokens are separate weights")
+    for field in ("attention_bias", "mlp_bias"):
+        if getattr(config, field, False):
+            raise ValueError(f"{field}=True is not supported: the projections have no bias")
+    if h % nh:
+        raise ValueError(f"hidden_size must be divisible by num_heads (got `hidden_size`: {h} and `num_heads`: {nh}).")
+    head_dim = getattr(config, "head_dim", None)
+    if head_dim is not None and head_dim != h // nh:
+        raise ValueError(f"head_dim={head_dim} is not supported: it must equal hidden_size / num_attention_heads = {h // nh}")
+    if nkv <= 0 or nh % nkv:
+        raise ValueError(f"num_key_value_heads={nkv} must divide num_attention_heads={nh}")
+
+
 class LlamaMLP(nn.Module):
     def __init__(self, hidden_size: int, intermediate_size: int, hidden_act: str = "silu"):
         super().__init__()
@@ -157,23 +197,23 @@ class LlamaAttention(nn.Module):
         self.hidden_size = config.hidden_size
         self.num_heads = config.num_attention_heads
         self.head_dim = self.hidden_size // self.num_heads
-        if self.head_dim * self.num_heads != self.hidden_size:
-            raise ValueError(
-                f"hidden_size must be divisible by num_heads (got `hidden_size`: {self.hidden_size}"
-                f" and `num_heads`: {self.num_heads})."
-            )
+        check_llama_config(config)
+        self.num_key_value_heads = num_kv_heads(config)
+        self.num_key_value_groups = self.num_heads // self.num_key_value_heads
+        kv_size = self.num_key_value_heads * self.head_dim
         self.max_position_embeddings = config.max_position_embeddings
         self.q_proj = nn.Linear(self.hidden_size, self.hidden_size, bias=False)
-        self.k_proj = nn.Linear(self.hidden_size, self.hidden_size, bias=False)
-        self.v_proj = nn.Linear(self.hidden_size, self.hidden_size, bias=False)
+        self.k_proj = nn.Linear(self.hidden_size, kv_size, bias=False)
+        self.v_proj = nn.Linear(self.hidden_size, kv_size, bias=False)
         self.o_proj = nn.Linear(self.hidden_size, self.hidden_size, bias=False)
-        self.rotary_emb = LlamaRotaryEmbedding(self.head_dim, max_position_embeddings=self.max_position_embeddings)
+        self.rotary_emb = LlamaRotaryEmbedding(self.head_dim, max_position_embeddings=self.max_position_embeddings,
+                                               base=float(rope_settings(config)[1]))
 
     def forward(self, hidden_states, position_ids=None, past_key_value=None, use_cache=False):
         B, T, _ = hidden_states.shape
         q = self.q_proj(hidden_states).view(B, T, self.num_heads, self.head_dim).transpose(1, 2)
-        k = self.k_proj(hidden_states).view(B, T, self.num_heads, self.head_dim).transpose(1, 2)
-        v = self.v_proj(hidden_states).view(B, T, self.num_heads, self.head_dim).transpose(1, 2)
+        k = self.k_proj(hidden_states).view(B, T, self.num_key_value_heads, self.head_dim).transpose(1, 2)
+        v = self.v_proj(hidden_states).view(B, T, self.num_key_value_heads, self.head_dim).transpose(1, 2)
         kv_len = T + (past_key_value[0].shape[-2] if past_key_value is not None else 0)
         cos, sin = self.rotary_emb(v, seq_len=kv_len)
         q, k = apply_rotary_pos_emb(q, k, cos, sin, position_ids)
@@ -181,6 +221,8 @@ class LlamaAttention(nn.Module):
             k = torch.cat([past_key_value[0], k], dim=2)
             v = torch.cat([past_key_value[1], v], dim=2)
         present = (k, v) if use_cache else None
+        # grouped-query attention: every query head of a group attends with its group's KV head
+        k, v = repeat_kv(k, self.num_key_value_groups), repeat_kv(v, self.num_key_value_groups)
         # the padding mask is ignored and causality always applied (reference :221-224)
         causal = past_key_value is None or T > 1
         if past_key_value is not None and T > 1:
@@ -226,6 +268,31 @@ class LlamaDecoderLayer(nn.Module):
 
 
 # --------------------------------------------------------------------------- base classes
+def load_state_dict_files(path: str) -> dict:
+    """The state dict of a local checkpoint directory, from the first of ``pytorch_model.bin``, ``model.safetensors`` and
+    a sharded checkpoint's ``*.index.json`` (``weight_map`` of key -> shard file, ``.bin`` or ``.safetensors``) that exists."""
+    def read(file):
+        if file.endswith(".safetensors"):
+            from safetensors.torch import load_file
+
+            return load_file(file)
+        return torch.load(file, map_location="cpu", weights_only=True)
+
+    for name in ("pytorch_model.bin", "model.safetensors"):
+        if os.path.exists(os.path.join(path, name)):
+            return read(os.path.join(path, name))
+    for name in ("model.safetensors.index.json", "pytorch_model.bin.index.json"):
+        index = os.path.join(path, name)
+        if os.path.exists(index):
+            with open(index) as f:
+                shards = sorted(set(json.load(f)["weight_map"].values()))
+            state = {}
+            for shard in shards:
+                state.update(read(os.path.join(path, shard)))
+            return state
+    raise FileNotFoundError(f"no pytorch_model.bin, model.safetensors or sharded index in {path}")
+
+
 class _PretrainedMixin:
     """``save_pretrained`` / ``from_pretrained`` in the reference layout."""
 
@@ -260,16 +327,14 @@ class _PretrainedMixin:
 
     @classmethod
     def from_pretrained(cls, path: str, **kwargs):
+        """Load a local checkpoint directory: ``pytorch_model.bin`` or ``model.safetensors``, or a sharded checkpoint
+        (``pytorch_model.bin.index.json`` / ``model.safetensors.index.json``).  Keys are strict, except that the
+        ``rotary_emb.inv_freq`` buffers (absent from Hugging Face checkpoints) keep the values built from the config."""
         config = load_config(path)
         model = cls(config, **kwargs)
-        bin_path = os.path.join(path, "pytorch_model.bin")
-        if os.path.exists(bin_path):
-            state = torch.load(bin_path, map_location="cpu", weights_only=True)
-        else:
-            from safetensors.torch import load_file
+        from ..ckpt import load_model_weights
 
-            state = load_file(os.path.join(path, "model.safetensors"))
-        model.load_state_dict(state, strict=True)
+        load_model_weights(model, path, strict=True)
         return model
 
     def num_parameters(self, only_trainable: bool = False) -> int:

@@ -25,6 +25,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from .configs import rope_settings
 from .llama import CausalLMOutput, _PretrainedMixin, rotate_half
 
 __all__ = [
@@ -101,25 +102,8 @@ def apply_partial_rotary(q, k, cos, sin, position_ids):
     return (q * cos) + (rotate_half(q) * sin), (k * cos) + (rotate_half(k) * sin)
 
 
-def _rope_settings(config):
-    """(rotary fraction, base, scaling dict) from either config dialect: the classic GPT-NeoX fields ``rotary_pct`` /
-    ``rotary_emb_base`` / ``rope_scaling`` (modeling_pythia.py:95-106 of the reference, checkpoints' ``config.json``) or the
-    ``rope_parameters`` dict that transformers >= 5 folds them into (``partial_rotary_factor``, ``rope_theta``, ``rope_type``, ``factor``)."""
-    rp = getattr(config, "rope_parameters", None) or {}
-    pct = getattr(config, "rotary_pct", None)
-    if pct is None:
-        pct = rp.get("partial_rotary_factor", getattr(config, "partial_rotary_factor", 0.25))
-    base = getattr(config, "rotary_emb_base", None)
-    if base is None:
-        base = rp.get("rope_theta", getattr(config, "rope_theta", 10000))
-    scaling = getattr(config, "rope_scaling", None)
-    if (scaling is None or not scaling.get("type", scaling.get("rope_type"))) and rp.get("rope_type") not in (None, "default"):
-        scaling = {"type": rp["rope_type"], "factor": rp.get("factor", 1.0)}
-    return float(pct), base, scaling
-
-
 def _make_rope(config, rotary_ndims):
-    _, base, scaling = _rope_settings(config)
+    _, base, scaling = rope_settings(config)
     if scaling is None or scaling.get("type", scaling.get("rope_type")) in (None, "default"):
         return GPTNeoXRotaryEmbedding(rotary_ndims, config.max_position_embeddings, base=base)
     kind = scaling.get("type", scaling.get("rope_type"))
@@ -139,7 +123,7 @@ class GPTNeoXAttention(nn.Module):
         if self.hidden_size % self.num_attention_heads != 0:
             raise ValueError("The hidden size is not divisble by the number of attention heads! Make sure to update them")
         self.head_size = self.hidden_size // self.num_attention_heads
-        self.rotary_ndims = int(self.head_size * _rope_settings(config)[0])
+        self.rotary_ndims = int(self.head_size * rope_settings(config)[0])
         self.rotary_emb = _make_rope(config, self.rotary_ndims)
         bias = getattr(config, "attention_bias", True)
         self.query_key_value = nn.Linear(config.hidden_size, 3 * config.hidden_size, bias=bias)
