@@ -109,8 +109,13 @@ class FusedStepperBase:
 
         fp8 path (``site = (layer, index)``): xn is quantised to E4M3 with the site's delayed scale and multiplied with the E4M3
         copy of W on the kind::f8f6f4 tensor-core path; the bf16 LoRA term shares the accumulator, so u is produced pre-divided
-        by the product scale s_x·s_w, which the epilogue multiplies back."""
+        by the product scale s_x·s_w, which the epilogue multiplies back.
+
+        Full-rank training (``A is None``): out = xn·Wᵀ (+ bias) (+ residual), one launch over the whole stacked group."""
         g, r, M = fused.gemm, self.r, self.M_
+        if A is None:
+            g(xn, W, out, M=M, N=W.shape[0], K1=K, residual=residual, bias=bias)
+            return
         drop = self.p > 0 and xd.shape[1] == G * K
         if self.fp8 and site is not None:
             l, s_i = site
@@ -131,7 +136,8 @@ class FusedStepperBase:
             return
         g(xn, W, out, M=M, N=G * Ng, K1=K, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, residual=residual, bias=bias)
 
-    def _lora_group_bwd(self, dy, S_B, S_W, S_A, gA, gB, xd, u, keys, *, G, K, Ng, base_out, out, tag, site=None, Nq=None):
+    def _lora_group_bwd(self, dy, S_B, S_W, S_A, gA, gB, xd, u, keys, *, G, K, Ng, base_out, out, tag, site=None, Nq=None,
+                        gW=None):
         """Backward of one stacked LoRA group.  dy [M, G·Ng] -> out [M, K] (grad of the group's input).
 
         ``Nq`` (see ``_lora_group_fwd``): dy is [M, Nq + (G-1)·Ng]; du and dB then run as two launches each, the first group
@@ -139,8 +145,20 @@ class FusedStepperBase:
 
         The two weight-gradient GEMMs only read (dy, du, xd, u), so they are forked onto a side stream and fill the
         SMs that the skinny du / parts GEMMs and kernel tails of the main chain leave idle; ``self._wg_done[tag]``
-        is the event the main stream waits on before it overwrites one of their inputs (see ``_backward``)."""
+        is the event the main stream waits on before it overwrites one of their inputs (see ``_backward``).
+
+        Full-rank training (``S_A is None``): out = dy·W and gW += dyᵀ·xd (fp32, on the side stream like dA / dB)."""
         C, g, M, r, s = self.C, fused.gemm, self.M_, self.r, self.scale
+        if S_A is None:
+            N = S_W.shape[0]
+            wgrad = lambda: g(dy, xd, gW, M=N, N=K, K1=M, a1_mn=True, b1_mn=True, accumulate=True,  # noqa: E731
+                              split_k=self.wgrad_split_k)
+            if self.side is not None:
+                self._fork_wgrads(tag, wgrad)
+            g(dy, S_W, out, M=M, N=K, K1=N, b1_mn=True)
+            if self.side is None:
+                wgrad()
+            return
         du = self.du_bufs[tag]
         split = Nq is not None and Nq != Ng
         width = Nq + (G - 1) * Ng if split else G * Ng
@@ -170,14 +188,7 @@ class FusedStepperBase:
               alpha_dev=self.alpha_main[site[0], site[1]:site[1] + 1] if (self.fp8 and site is not None) else None)
 
         if self.side is not None:
-            fork = torch.cuda.Event()
-            fork.record()
-            self.side.wait_event(fork)
-            with torch.cuda.stream(self.side):
-                wgrads()
-                done = torch.cuda.Event()
-                done.record()
-            self._wg_done[tag] = done
+            self._fork_wgrads(tag, wgrads)
         if self.fused_dx:
             sd, ks, pp = (self.seed, list(keys), self.p) if drop else (None, [0] * G, 0.0)
             if width >= self.dx_split_k:
@@ -209,6 +220,17 @@ class FusedStepperBase:
                 torch.add(base_out, parts.view(M, G, K).sum(1) if G > 1 else parts, out=out)
         if self.side is None:
             wgrads()
+
+    def _fork_wgrads(self, tag, wgrads):
+        """Runs ``wgrads`` on the side stream after the work issued so far; ``self._wg_done[tag]`` marks its end."""
+        fork = torch.cuda.Event()
+        fork.record()
+        self.side.wait_event(fork)
+        with torch.cuda.stream(self.side):
+            wgrads()
+            done = torch.cuda.Event()
+            done.record()
+        self._wg_done[tag] = done
 
     def _join(self, tag):
         """Main stream waits for the side-stream weight gradients tagged ``tag`` (no-op if none are pending)."""

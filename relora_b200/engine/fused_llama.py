@@ -17,6 +17,10 @@ launch/CPU-bound at the 250M scale.  This executor instead
 * captures forward+backward of a micro-batch in a CUDA graph (dropout seeds live on the device and advance
   inside the graph), so a micro-step costs one graph launch on the host.
 
+Full-rank training (a bare ``LlamaForCausalLM``, ``--engine fused``) runs the same layer loop without the low-rank branch: the
+projection weights are trainable, live in the flat store as stacked views, and their fp32 gradients ``gW += dyᵀ·x`` run on the
+side stream where ``dA`` / ``dB`` run under ReLoRA.
+
 Math per layer (training, dropout p, scale s): see ``ops/reference.py`` — numerics tests compare this executor
 with the module-by-module PyTorch path on identical weights and masks.
 """
@@ -32,6 +36,7 @@ import torch.nn.functional as F_
 from ..models.llama import LlamaForCausalLM, num_kv_heads
 from ..ops import fused, native
 from ..parallel.dist import DistInfo
+from ..parallel.flat import _ALIGN as _STORE_ALIGN
 from ..parallel.grad_sync import broadcast_params
 from ..relora import ReLoRaLinear, ReLoRaModel
 from .fused_common import FusedStepperBase
@@ -71,27 +76,73 @@ def supports(model, args=None) -> Tuple[bool, str]:
     return True, "ok"
 
 
+def supports_full_rank(model, args=None) -> Tuple[bool, str]:
+    """Whether the executor can train ``model`` (an unwrapped Llama) full-rank, and if not, why.  The device and dtype are
+    checked last, so every other reason is visible on a CPU model."""
+    if not isinstance(model, LlamaForCausalLM):
+        return False, "only Llama is fused for full-rank training"
+    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return False, f"--frozen_dtype {args.frozen_dtype} has no frozen weights to act on in full-rank training"
+    cfg = model.config
+    h, nh = cfg.hidden_size, cfg.num_attention_heads
+    hd = h // nh
+    kv = num_kv_heads(cfg) * hd
+    # every GEMM operand is read through a TMA tensor map, whose row pitch must be a multiple of 16 bytes (gemm_wgmma.cu:
+    # make_map_2d): x / dx [tokens, hidden], W and dW [*, hidden], and the packed q | k | v row of h + 2·kv
+    if h % 8 or (h + 2 * kv) % 8:
+        return False, f"hidden ({h}) and hidden + 2 x num_key_value_heads x head_dim ({h + 2 * kv}) must be multiples of 8 for the GEMM's 16-byte row pitch"
+    # the stacked Wqkv view needs q / k / v adjacent in the flat store, whose segments start on 128-element boundaries
+    if (h * h) % _STORE_ALIGN or (kv * h) % _STORE_ALIGN:
+        return False, f"hidden x hidden ({h * h}) and kv width x hidden ({kv * h}) must be multiples of {_STORE_ALIGN} for the stacked q | k | v weights"
+    if h > 8192:
+        return False, f"hidden ({h}) is above the RMSNorm kernels' 8192"
+    if hd % 8:
+        return False, f"head_dim ({hd}) must be a multiple of 8 for the attention and RoPE kernels"
+    attention = getattr(args, "attention", "auto")
+    if attention == "native" and fused.attention_backend(hd, attention) != "native":
+        return False, f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM}, got {hd}"
+    for m in model.modules():
+        if isinstance(m, torch.nn.Linear) and m.bias is not None:
+            return False, "biased projections use the module path"
+    p = next(model.parameters())
+    if not p.is_cuda or p.dtype != BF:
+        return False, "needs CUDA + bfloat16"
+    return True, "ok"
+
+
 class _Layer:
-    """Stacked views of one decoder layer's parameters and gradients."""
+    """Stacked views of one decoder layer's parameters and gradients (None where a mode has no such tensor: the LoRA factors
+    in full-rank training, the projection-weight gradients under ReLoRA)."""
 
     __slots__ = ("Wqkv", "Wo", "Wgu", "Wd", "A_qkv", "B_qkv", "A_o", "B_o", "A_gu", "B_gu", "A_d", "B_d", "w1", "w2",
                  "gA_qkv", "gB_qkv", "gA_o", "gB_o", "gA_gu", "gB_gu", "gA_d", "gB_d", "gw1", "gw2", "keys_qkv", "key_o",
-                 "keys_gu", "key_d", "mods", "merge")
+                 "keys_gu", "key_d", "mods", "merge", "gWqkv", "gWo", "gWgu", "gWd")
+
+    def __init__(self):
+        for k in self.__slots__:
+            setattr(self, k, None)
 
 
 class FusedLlamaStepper(FusedStepperBase):
-    def __init__(self, model: ReLoRaModel, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
+    """``model`` is a ``ReLoRaModel`` around a Llama (ReLoRA: frozen stacked weights, trainable LoRA factors) or a bare
+    ``LlamaForCausalLM`` (full-rank training: the projection weights are trainable and live in the flat store; every projection
+    is the ReLoRA one without its low-rank branch)."""
+
+    def __init__(self, model, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, symm_factory=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
                  overlap_wgrad: bool = True, attention: str = "auto", fp8: bool = False, fp8_backward: bool = False,
                  deterministic: bool = False):
-        ok, why = supports(model)
+        self.full = not isinstance(model, ReLoRaModel)
+        ok, why = supports_full_rank(model) if self.full else supports(model)
         if not ok:
             raise RuntimeError(why)
+        if self.full and fp8:
+            raise RuntimeError("--frozen_dtype fp8 has no frozen weights to act on in full-rank training")
         if fp8 and num_kv_heads(model.wrapped_model.config) != model.wrapped_model.config.num_attention_heads:
             raise RuntimeError("--frozen_dtype fp8 with grouped-query attention uses the module path (the fp8 weight copies are [3h, h])")
         self.model, self.info = model, info
-        self.inner: LlamaForCausalLM = model.wrapped_model
+        self.inner: LlamaForCausalLM = model if self.full else model.wrapped_model
         self.C = fused._C()
         self.ga = grad_accumulation
         self.clip = clip_grad_norm
@@ -104,32 +155,34 @@ class FusedLlamaStepper(FusedStepperBase):
         self.kv = self.nkv * self.hd  # width of the k and v projections (h without grouped-query attention)
         self.qkv_w = self.h + 2 * self.kv  # packed [q | k | v] row
         self.fp = (self.f + 127) // 128 * 128  # padded intermediate size (zero rows / columns keep every GEMM extent a multiple of the 128-wide tile)
-        self.r = model.r
+        self.r = 0 if self.full else model.r
         self.L = cfg.num_hidden_layers
         self.eps = cfg.rms_norm_eps
-        self.p = float(model.lora_dropout)
-        self.scale = float(model.lora_alpha) / model.r
+        self.p = 0.0 if self.full else float(model.lora_dropout)
+        self.scale = 1.0 if self.full else float(model.lora_alpha) / model.r
         self.device = info.device
         broadcast_params(model)
 
-        # ---------------------------------------------------------------- stacked frozen weights
+        # ---------------------------------------------------------------- stacked frozen weights (ReLoRA)
         dev = self.device
         h, f, fp, r, L = self.h, self.f, self.fp, self.r, self.L
         kv = self.kv
-        self.Wqkv = torch.empty(L, h + 2 * kv, h, dtype=BF, device=dev)
-        self.Wo = torch.empty(L, h, h, dtype=BF, device=dev)
-        self.Wgu = torch.zeros(L, 2 * fp, h, dtype=BF, device=dev)
-        self.Wd = torch.zeros(L, h, fp, dtype=BF, device=dev)
         layers = self.inner.model.layers
-        with torch.no_grad():
-            for l, layer in enumerate(layers):
-                at, mlp = layer.self_attn, layer.mlp
-                for m, r0, r1 in ((at.q_proj, 0, h), (at.k_proj, h, h + kv), (at.v_proj, h + kv, h + 2 * kv)):
-                    self._rehome(m.weight, self.Wqkv[l, r0:r1])
-                self._rehome(at.o_proj.weight, self.Wo[l])
-                self._rehome(mlp.gate_proj.weight, self.Wgu[l, :f])
-                self._rehome(mlp.up_proj.weight, self.Wgu[l, fp:fp + f])
-                self._rehome(mlp.down_proj.weight, self.Wd[l][:, :f])
+        self.Wqkv = self.Wo = self.Wgu = self.Wd = None  # full rank: the trainable weights are stacked views into the flat store
+        if not self.full:
+            self.Wqkv = torch.empty(L, h + 2 * kv, h, dtype=BF, device=dev)
+            self.Wo = torch.empty(L, h, h, dtype=BF, device=dev)
+            self.Wgu = torch.zeros(L, 2 * fp, h, dtype=BF, device=dev)
+            self.Wd = torch.zeros(L, h, fp, dtype=BF, device=dev)
+            with torch.no_grad():
+                for l, layer in enumerate(layers):
+                    at, mlp = layer.self_attn, layer.mlp
+                    for m, r0, r1 in ((at.q_proj, 0, h), (at.k_proj, h, h + kv), (at.v_proj, h + kv, h + 2 * kv)):
+                        self._rehome(m.weight, self.Wqkv[l, r0:r1])
+                    self._rehome(at.o_proj.weight, self.Wo[l])
+                    self._rehome(mlp.gate_proj.weight, self.Wgu[l, :f])
+                    self._rehome(mlp.up_proj.weight, self.Wgu[l, fp:fp + f])
+                    self._rehome(mlp.down_proj.weight, self.Wd[l][:, :f])
 
         # ---------------------------------------------------------------- flat trainable store (stack-friendly order)
         named: List[Tuple[str, torch.nn.Parameter]] = []
@@ -140,14 +193,18 @@ class FusedLlamaStepper(FusedStepperBase):
 
         for layer in layers:
             at, mlp = layer.self_attn, layer.mlp
-            for m in (at.q_proj, at.k_proj, at.v_proj):
-                add(m.lora_A.weight)
-            for m in (at.q_proj, at.k_proj, at.v_proj):
-                add(m.lora_B.weight)
-            add(at.o_proj.lora_A.weight); add(at.o_proj.lora_B.weight)
-            add(mlp.gate_proj.lora_A.weight); add(mlp.up_proj.lora_A.weight)
-            add(mlp.gate_proj.lora_B.weight); add(mlp.up_proj.lora_B.weight)
-            add(mlp.down_proj.lora_A.weight); add(mlp.down_proj.lora_B.weight)
+            if self.full:
+                for m in (at.q_proj, at.k_proj, at.v_proj, at.o_proj, mlp.gate_proj, mlp.up_proj, mlp.down_proj):
+                    add(m.weight)
+            else:
+                for m in (at.q_proj, at.k_proj, at.v_proj):
+                    add(m.lora_A.weight)
+                for m in (at.q_proj, at.k_proj, at.v_proj):
+                    add(m.lora_B.weight)
+                add(at.o_proj.lora_A.weight); add(at.o_proj.lora_B.weight)
+                add(mlp.gate_proj.lora_A.weight); add(mlp.up_proj.lora_A.weight)
+                add(mlp.gate_proj.lora_B.weight); add(mlp.up_proj.lora_B.weight)
+                add(mlp.down_proj.lora_A.weight); add(mlp.down_proj.lora_B.weight)
             add(layer.input_layernorm.weight); add(layer.post_attention_layernorm.weight)
         add(self.inner.model.embed_tokens.weight)
         add(self.inner.model.norm.weight)
@@ -161,6 +218,11 @@ class FusedLlamaStepper(FusedStepperBase):
         if fp != f:
             for layer in layers:
                 mlp = layer.mlp
+                if self.full:  # zero rows of gate / up and zero columns of down: zero gradients, so AdamW leaves them zero
+                    padded[id(mlp.gate_proj.weight)] = (fp, h)
+                    padded[id(mlp.up_proj.weight)] = (fp, h)
+                    padded[id(mlp.down_proj.weight)] = (h, fp)
+                    continue
                 padded[id(mlp.gate_proj.lora_B.weight)] = (fp, r)
                 padded[id(mlp.up_proj.lora_B.weight)] = (fp, r)
                 padded[id(mlp.down_proj.lora_A.weight)] = (r, fp)
@@ -172,6 +234,20 @@ class FusedLlamaStepper(FusedStepperBase):
             at, mlp = layer.self_attn, layer.mlp
             S = _Layer()
             l = len(self.layers)
+            S.w1, S.gw1 = pv(layer.input_layernorm.weight)
+            S.w2, S.gw2 = pv(layer.post_attention_layernorm.weight)
+            if self.full:
+                S.Wqkv, S.gWqkv = pv(at.q_proj.weight, rows=h + 2 * kv)
+                S.Wo, S.gWo = pv(at.o_proj.weight)
+                S.Wgu, S.gWgu = pv(mlp.gate_proj.weight, 2)
+                S.Wd, S.gWd = pv(mlp.down_proj.weight)
+                # sanity: the stacked views must alias the module parameters
+                assert S.Wqkv[h:h + kv].data_ptr() == at.k_proj.weight.data_ptr()
+                assert S.Wqkv[h + kv:].data_ptr() == at.v_proj.weight.data_ptr() and S.Wqkv.shape == (h + 2 * kv, h)
+                assert S.Wgu[fp:].data_ptr() == mlp.up_proj.weight.data_ptr() and S.Wgu.shape == (2 * fp, h)
+                assert S.Wd.data_ptr() == mlp.down_proj.weight.data_ptr() and S.Wd.shape == (h, fp)
+                self.layers.append(S)
+                continue
             S.Wqkv, S.Wo, S.Wgu, S.Wd = self.Wqkv[l], self.Wo[l], self.Wgu[l], self.Wd[l]
             S.A_qkv, S.gA_qkv = pv(at.q_proj.lora_A.weight, 3)
             S.B_qkv, S.gB_qkv = pv(at.q_proj.lora_B.weight, 3) if kv == h else pv(at.q_proj.lora_B.weight, rows=h + 2 * kv)
@@ -181,8 +257,6 @@ class FusedLlamaStepper(FusedStepperBase):
             S.B_gu, S.gB_gu = pv(mlp.gate_proj.lora_B.weight, 2)
             S.A_d, S.gA_d = pv(mlp.down_proj.lora_A.weight)
             S.B_d, S.gB_d = pv(mlp.down_proj.lora_B.weight)
-            S.w1, S.gw1 = pv(layer.input_layernorm.weight)
-            S.w2, S.gw2 = pv(layer.post_attention_layernorm.weight)
             S.keys_qkv = [m.module_index + 1 for m in (at.q_proj, at.k_proj, at.v_proj)]
             S.key_o = at.o_proj.module_index + 1
             S.keys_gu = [mlp.gate_proj.module_index + 1, mlp.up_proj.module_index + 1]
@@ -211,7 +285,7 @@ class FusedLlamaStepper(FusedStepperBase):
         self._init_optimizer(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, zero=zero, native=native)
         self._attn_saved: List = []
         # ---- fp8 frozen-weight path: E4M3 copies of the stacked weights + per-site activation scales (csrc/fp8.cu)
-        self.fp8 = bool(fp8) or os.environ.get("RELORA_B200_FP8", "0") == "1"
+        self.fp8 = not self.full and (bool(fp8) or os.environ.get("RELORA_B200_FP8", "0") == "1")
         if self.fp8:
             u8 = lambda *sh: torch.zeros(*sh, dtype=torch.uint8, device=dev)  # noqa: E731
             self.W8 = [u8(L, 3 * h, h), u8(L, h, h), u8(L, 2 * fp, h), u8(L, h, fp)]  # sites: qkv, o, gate/up, down
@@ -286,10 +360,6 @@ class FusedLlamaStepper(FusedStepperBase):
         self.xd_o = e(L, M, h)
         self.xd_gu = e(L, M, G2 * h)
         self.xd_d = e(L, M, f)
-        self.u_qkv = e(L, M, 3 * r)
-        self.u_o = e(L, M, r)
-        self.u_gu = e(L, M, 2 * r)
-        self.u_d = e(L, M, r)
         self.qkv = e(L, M, self.qkv_w)
         self.gu = e(L, M, 2 * f)
         # transients
@@ -297,12 +367,23 @@ class FusedLlamaStepper(FusedStepperBase):
         self.hmid = e(M, f)
         self.xf = e(M, h)
         self.dxf = e(M, h)
-        self.dx_a, self.dx_b, self.dxn, self.dxn2 = e(M, h), e(M, h), e(M, h), e(M, h)
+        self.dx_a, self.dx_b, self.dxn2 = e(M, h), e(M, h), e(M, h)
         self.dattn = e(M, h)
         self.dqkv = e(M, self.qkv_w)
         self.dgu = e(M, 2 * f)
-        self.dhmid, self.dhmid2 = e(M, f), e(M, f)
-        self.du_bufs = {"d": e(M, r), "gu": e(M, 2 * r), "o": e(M, r), "qkv": e(M, 3 * r)}
+        self.dhmid2 = e(M, f)
+        if self.full:
+            # no low-rank branch: the input gradient is one GEMM straight into its output, so there are no u / du buffers and
+            # no separate base product (dxn, dhmid, parts)
+            self.u_qkv = self.u_o = self.u_gu = self.u_d = [None] * L
+            self.dxn = self.dhmid = None
+        else:
+            self.u_qkv = e(L, M, 3 * r)
+            self.u_o = e(L, M, r)
+            self.u_gu = e(L, M, 2 * r)
+            self.u_d = e(L, M, r)
+            self.dxn, self.dhmid = e(M, h), e(M, f)
+            self.du_bufs = {"d": e(M, r), "gu": e(M, 2 * r), "o": e(M, r), "qkv": e(M, 3 * r)}
         if self.fp8:
             self.x8_h = torch.empty(M, h, dtype=torch.uint8, device=dev)
             self.x8_f = torch.empty(M, f, dtype=torch.uint8, device=dev)
@@ -312,7 +393,7 @@ class FusedLlamaStepper(FusedStepperBase):
             self.attn_o = e(L, M, h)
             self.lse = torch.empty(L, B, self.nh, T, dtype=torch.float32, device=dev)
             self.delta = torch.empty(B, self.nh, T, dtype=torch.float32, device=dev)
-        self.parts = e(M, max(3 * h, f))
+        self.parts = None if self.full else e(M, max(3 * h, f))
         ldv = (self.V + 7) // 8 * 8
         self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
         self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
@@ -422,17 +503,17 @@ class FusedLlamaStepper(FusedStepperBase):
             S = self.layers[l]
             # ---- MLP: x_next = hmid·Wdᵀ + u_d·B_dᵀ + x1
             self._lora_group_bwd(dx, S.B_d, S.Wd, S.A_d, S.gA_d, S.gB_d, self.xd_d[l], self.u_d[l], [S.key_d],
-                                 G=1, K=f, Ng=h, base_out=self.dhmid, out=self.dhmid2, tag="d", site=(l, 3))
+                                 G=1, K=f, Ng=h, base_out=self.dhmid, out=self.dhmid2, tag="d", site=(l, 3), gW=S.gWd)
             self._join("gu")  # the previous layer's gate/up weight gradients read dgu / du_gu
             C.swiglu_bwd(self.dhmid2, self.gu[l], self.dgu)
             self._lora_group_bwd(self.dgu, S.B_gu, S.Wgu, S.A_gu, S.gA_gu, S.gB_gu, self.xd_gu[l], self.u_gu[l], S.keys_gu,
-                                 G=2, K=h, Ng=f, base_out=self.dxn, out=self.dxn2, tag="gu", site=(l, 2))
+                                 G=2, K=h, Ng=f, base_out=self.dxn, out=self.dxn2, tag="gu", site=(l, 2), gW=S.gWgu)
             self._join("o")  # ... and its o_proj weight gradients read the buffer this norm backward writes
             C.rmsnorm_bwd(self.dxn2, self.x1[l], S.w2, self.rstd2[l], dx, dx_other, S.gw2, ws, tk)
             dx, dx_other = dx_other, dx  # dx = grad wrt x1
             # ---- attention: x1 = attn·Woᵀ + u_o·B_oᵀ + x
             self._lora_group_bwd(dx, S.B_o, S.Wo, S.A_o, S.gA_o, S.gB_o, self.xd_o[l], self.u_o[l], [S.key_o],
-                                 G=1, K=h, Ng=h, base_out=self.dxn, out=self.dattn, tag="o", site=(l, 1))
+                                 G=1, K=h, Ng=h, base_out=self.dxn, out=self.dattn, tag="o", site=(l, 1), gW=S.gWo)
             if self.native_attn:
                 self._join("qkv")  # the previous layer's qkv weight gradients read dqkv / du_qkv
                 if self.nkv == nh:
@@ -461,7 +542,8 @@ class FusedLlamaStepper(FusedStepperBase):
                 d3[:, :, nh + nkv:].copy_(dv.transpose(1, 2))
                 C.rope_inplace(self.dqkv, T, nh + nkv, hd, hd, self.cos, self.sin, True, 0)
             self._lora_group_bwd(self.dqkv, S.B_qkv, S.Wqkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd_qkv[l], self.u_qkv[l],
-                                 S.keys_qkv, G=3, K=h, Ng=self.kv, base_out=self.dxn, out=self.dxn2, tag="qkv", site=(l, 0), Nq=h)
+                                 S.keys_qkv, G=3, K=h, Ng=self.kv, base_out=self.dxn, out=self.dxn2, tag="qkv", site=(l, 0), Nq=h,
+                                 gW=S.gWqkv)
             self._join("d")  # this layer's down_proj weight gradients read the buffer written next
             C.rmsnorm_bwd(self.dxn2, self.x_in[l], S.w1, self.rstd1[l], dx, dx_other, S.gw1, ws, tk)
             dx, dx_other = dx_other, dx
@@ -515,6 +597,8 @@ class FusedLlamaStepper(FusedStepperBase):
     @torch.no_grad()
     def merge_and_reinit(self):
         """W += s·B@A on the stacked buffers (wgmma GEMM accumulating into W in fp32), then hash re-init."""
+        if self.full:
+            raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
         self._merge_modules([blk for S in self.layers for blk in zip(S.mods, S.merge)])
         if self.fp8:
             self._quantize_weights()

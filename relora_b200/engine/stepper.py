@@ -199,10 +199,19 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
                                      fp8_backward=getattr(args, "frozen_dtype", None) == "fp8_full",
                                      deterministic=bool(getattr(args, "deterministic", False)), **kw)
         if engine == "fused":
-            # Pythia (GPT-NeoX) has its own executor; `auto` keeps it on the module path
+            # Pythia (GPT-NeoX) and full-rank Llama run fused only on request; `auto` keeps both on the module path
+            from ..models.llama import LlamaForCausalLM
             from ..models.pythia import GPTNeoXForCausalLM
+            from .fused_llama import supports_full_rank
             from .fused_pythia import FusedPythiaStepper, supports as pythia_supports
 
+            if isinstance(model, LlamaForCausalLM):
+                ok, why = supports_full_rank(model, args)
+                if ok:
+                    return FusedLlamaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
+                                             attention=getattr(args, "attention", "auto"),
+                                             deterministic=bool(getattr(args, "deterministic", False)), **kw)
+                raise RuntimeError(f"--engine fused requested but not applicable: {why}")
             ok, why_p = pythia_supports(model, args)
             if ok:
                 return FusedPythiaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
