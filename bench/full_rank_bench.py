@@ -1,11 +1,17 @@
-"""Full-rank training: the fused Llama executor against the module path, and the weight-gradient GEMM against cuBLAS.
+"""Full-rank training: the fused executors against the module path, and the weight-gradient GEMM against cuBLAS.
 
     python bench/full_rank_bench.py [--models llama_250m,llama_1b] [--steps 8] [--rounds 3] [--out FILE]
+    python bench/full_rank_bench.py --models pythia_160m,pythia_410m,pythia_1b [--ga 4]
+
+Llama models come from ``configs/<name>.json`` (T 512).  Pythia models are GPT-NeoX at the shapes and batches of
+``bench/pythia_bench.py`` (V 50304, parallel residual, rotary 0.25, GELU, T 2049, the recipe's sequence length); their rows also
+carry an estimate of the fused executor's memory from shapes (bf16 parameters, fp32 gradients and AdamW moments, and the
+activations the executor saves per token), printed next to the measured peak.
 
 End to end: both executors train the same model from identical weights on the same seeded token batches, in one process.  After
-a warm-up of both, they alternate ``--rounds`` times, each round timing ``--steps`` updates (one micro-batch per update) between
-device synchronises; the median tokens/s of each is reported, with the loss both reached after the same steps.  The fused
-executor's peak memory (``torch.cuda.max_memory_allocated``) is taken before the module path is built.
+a warm-up of both, they alternate ``--rounds`` times, each round timing ``--steps`` updates (``--ga`` micro-batches per update,
+default 1) between device synchronises; the median tokens/s of each is reported, with the loss both reached after the same steps.
+The fused executor's peak memory (``torch.cuda.max_memory_allocated``) is taken before the module path is built.
 
 Per kernel: ``gW += dyᵀ·x`` (fp32, both operands MN-major) at the full-rank projection shapes of both models over 12 288 tokens,
 split-K on (the default) and off (``--deterministic``), against ``torch.addmm(gW, dy.t(), x, out_dtype=torch.float32)``.  CUDA
@@ -78,25 +84,59 @@ def wgrad_rows(cfg, name, M, flush):
     return rows
 
 
-def end_to_end(name, steps, rounds, warmup, T=512):
+def pythia_config(name):
+    from pythia_bench import SHAPES  # bench/ is on sys.path when this file runs as a script
+
+    from relora_b200.models import SimpleConfig
+
+    h, L, nh, f, B = SHAPES[name[len("pythia_"):]]
+    cfg = SimpleConfig(model_type="gpt_neox", vocab_size=50304, hidden_size=h, num_hidden_layers=L, num_attention_heads=nh,
+                       intermediate_size=f, rotary_pct=0.25, max_position_embeddings=2048, layer_norm_eps=1e-5,
+                       use_parallel_residual=True, hidden_act="gelu", rotary_emb_base=10000, tie_word_embeddings=False)
+    return cfg, B
+
+
+def pythia_memory_estimate(cfg, B, T, native_attn):
+    """Bytes the fused full-rank executor holds, from shapes: 14 bytes per parameter (bf16 value, fp32 gradient, two fp32 AdamW
+    moments), and per token and layer the bf16 tensors it saves for the backward (input, the two norm outputs, the post-rotary
+    qkv, the attention output (twice with the wgmma kernels), the pre-GELU and GELU outputs; plus the sequential residual's x1)
+    and the fp32 norm statistics.  Transients (one layer's gradients, the LM-head chunk) are not counted."""
+    h, f, L, V = cfg.hidden_size, cfg.intermediate_size, cfg.num_hidden_layers, cfg.vocab_size
+    per_layer = 4 * h * h + 2 * h * f + 9 * h + f  # query_key_value + dense, the two MLP projections; biases and norms
+    P = L * per_layer + 2 * V * h + 2 * h
+    saved = 2 * ((1 + 2 + 3 + 1 + int(native_attn) + int(not cfg.use_parallel_residual)) * h + 2 * f) + 4 * 2 * (
+        1 + int(not cfg.use_parallel_residual))
+    per_token = L * saved + 2 * h  # and the last layer's output
+    return {"params": P, "state_GB": 14 * P / 1e9, "saved_activations_per_token_MB": per_token / 1e6,
+            "saved_activations_GB": per_token * B * T / 1e9, "total_GB": (14 * P + per_token * B * T) / 1e9}
+
+
+def end_to_end(name, steps, rounds, warmup, T=512, ga=1):
     from relora_b200.engine.fused_llama import FusedLlamaStepper
+    from relora_b200.engine.fused_pythia import FusedPythiaStepper
     from relora_b200.engine.stepper import ModuleStepper
-    from relora_b200.models import LlamaForCausalLM, load_config
+    from relora_b200.models import GPTNeoXForCausalLM, LlamaForCausalLM, load_config
     from relora_b200.parallel.dist import DistInfo
 
     info = DistInfo(0, 0, 1, torch.device("cuda", torch.cuda.current_device()), "nccl")
-    cfg = load_config(os.path.join(ROOT, "configs", f"{name}.json"))
-    B = BATCH[name]
+    pythia = name.startswith("pythia_")
+    if pythia:
+        cfg, B = pythia_config(name)
+        T = 2049
+    else:
+        cfg = load_config(os.path.join(ROOT, "configs", f"{name}.json"))
+        B = BATCH[name]
+    Fused = FusedPythiaStepper if pythia else FusedLlamaStepper
     torch.manual_seed(0)
-    host = LlamaForCausalLM(cfg).to(BF)
+    host = (GPTNeoXForCausalLM if pythia else LlamaForCausalLM)(cfg).to(BF)
     g = torch.Generator().manual_seed(1)
     n_total = warmup + steps * rounds
-    batches = [torch.randint(0, cfg.vocab_size, (B, T), generator=g) for _ in range(n_total)]
-    kw = dict(lr=3e-4, weight_decay=0.0, clip_grad_norm=1.0, grad_accumulation=1)
+    batches = [torch.randint(0, cfg.vocab_size, (B, T), generator=g) for _ in range(n_total * ga)]
+    kw = dict(lr=3e-4, weight_decay=0.0, clip_grad_norm=1.0, grad_accumulation=ga)
 
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
-    st = {"fused": FusedLlamaStepper(copy.deepcopy(host).cuda(), info, cuda_graphs=True, **kw)}
+    st = {"fused": Fused(copy.deepcopy(host).cuda(), info, cuda_graphs=True, **kw)}
     pos = {"fused": 0, "module": 0}
     losses = {"fused": [], "module": []}
 
@@ -105,10 +145,11 @@ def end_to_end(name, steps, rounds, warmup, T=512):
         torch.cuda.synchronize()
         t0 = time.perf_counter()
         for _ in range(n):
-            ids = batches[pos[eng]].cuda(non_blocking=True)
-            losses[eng].append(s.micro_step(ids))
+            for _ in range(ga):
+                ids = batches[pos[eng]].cuda(non_blocking=True)
+                losses[eng].append(s.micro_step(ids))
+                pos[eng] += 1
             s.update()
-            pos[eng] += 1
         torch.cuda.synchronize()
         return time.perf_counter() - t0
 
@@ -120,13 +161,16 @@ def end_to_end(name, steps, rounds, warmup, T=512):
     tps = {"fused": [], "module": []}
     for _ in range(rounds):
         for eng in ("fused", "module"):
-            tps[eng].append(steps * B * T / run(eng, steps))
+            tps[eng].append(steps * ga * B * T / run(eng, steps))
     med = {k: sorted(v)[len(v) // 2] for k, v in tps.items()}
-    rec = {"model": name, "batch": B, "seq": T, "steps_per_round": steps, "rounds": rounds,
+    rec = {"model": name, "batch": B, "seq": T, "grad_accumulation": ga, "steps_per_round": steps, "rounds": rounds,
            "fused_tokens_per_s": med["fused"], "module_tokens_per_s": med["module"], "fused_over_module": med["fused"] / med["module"],
            "fused_tokens_per_s_all": tps["fused"], "module_tokens_per_s_all": tps["module"],
            "final_loss_fused": float(losses["fused"][-1]), "final_loss_module": float(losses["module"][-1]), "after_updates": n_total,
            "fused_max_memory_allocated_GB": fused_peak / 1e9}
+    if pythia:
+        rec["fused_memory_estimate"] = pythia_memory_estimate(cfg, B, T, st["fused"].native_attn)  # per micro-batch
+        rec["attention_native"] = st["fused"].native_attn
     print(json.dumps(rec), flush=True)
     del st
     torch.cuda.empty_cache()
@@ -139,6 +183,7 @@ def main():
     ap.add_argument("--steps", type=int, default=8)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--ga", type=int, default=1, help="micro-batches per update (gradient accumulation)")
     ap.add_argument("--skip-e2e", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -150,12 +195,12 @@ def main():
     res = {"card": card(), "wgrad": [], "e2e": []}
     print(json.dumps(res["card"]), flush=True)
     flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device="cuda")
-    for name in names:
+    for name in (n for n in names if not n.startswith("pythia_")):  # the dW GEMM rows cover the Llama configs
         res["wgrad"] += wgrad_rows(load_config(os.path.join(ROOT, "configs", f"{name}.json")), name, 12288, flush)
     del flush
     if not a.skip_e2e:
         for name in names:
-            res["e2e"].append(end_to_end(name, a.steps, a.rounds, a.warmup))
+            res["e2e"].append(end_to_end(name, a.steps, a.rounds, a.warmup, ga=a.ga))
     res["card_after"] = card()
     if a.out:
         with open(a.out, "w") as f:

@@ -16,6 +16,12 @@ The frozen weights stay where the modules keep them; the trainable parameters (L
 views of the flat store, so checkpoints keep the HF GPT-NeoX keys.  Numerics tests compare this executor with the module path on
 identical weights and dropout masks.
 
+Full-rank training (a bare ``GPTNeoXForCausalLM``, ``--engine fused``) runs the same layer loop without the low-rank branch: the
+four projection weights of each layer are trainable views of the flat store, every projection is one GEMM with the bias (and
+residual) epilogue, the input gradient is ``dy·W``, and the fp32 weight gradient ``gW += dyᵀ·x`` runs on the side stream where
+``dA`` / ``dB`` run under ReLoRA.  ``x`` is what the executor already saves with p = 0: the norm outputs, the attention output and
+the GELU output.
+
 Parallel residual:   x_next = x + dense(attn(LN1 x)) + b_o + mlp(LN2 x) + b_4
 Sequential residual: x1 = x + dense(attn(LN1 x)) + b_o ;  x_next = x1 + mlp(LN2 x1) + b_4
 """
@@ -77,24 +83,69 @@ def supports(model, args=None) -> Tuple[bool, str]:
     return True, "ok"
 
 
+def supports_full_rank(model, args=None) -> Tuple[bool, str]:
+    """Whether the executor can train ``model`` (an unwrapped GPT-NeoX) full-rank, and if not, why.  The device and dtype are
+    checked last, so every other reason is visible on a CPU model."""
+    if not isinstance(model, GPTNeoXForCausalLM):
+        return False, "only GPT-NeoX (Pythia) is fused for full-rank training here"
+    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return False, f"--frozen_dtype {args.frozen_dtype} has no frozen weights to act on in full-rank training"
+    cfg = model.config
+    if float(getattr(cfg, "hidden_dropout", 0.0)) != 0.0 or float(getattr(cfg, "attention_dropout", 0.0)) != 0.0:
+        return False, "hidden / attention dropout must be 0"
+    layer0 = model.gpt_neox.layers[0]
+    if not isinstance(layer0.mlp.act, nn.GELU):
+        return False, "only the GELU activation is fused"
+    h, f, nh = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads
+    if h % 128 or f % 128:
+        return False, f"hidden ({h}) and intermediate ({f}) must be multiples of 128"
+    if h > MAX_HIDDEN:
+        return False, f"hidden ({h}) must be <= {MAX_HIDDEN} (LayerNorm kernel limit)"
+    hd = h // nh
+    if hd % 8:
+        return False, f"head_dim ({hd}) must be a multiple of 8 for the attention and rotary kernels"
+    if layer0.attention.rotary_ndims % 2:
+        return False, "the number of rotary dims must be even"
+    at, mlp = layer0.attention, layer0.mlp
+    if any(m.bias is None for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)):
+        return False, "projections without bias use the module path"
+    attention = getattr(args, "attention", "auto")
+    if attention == "native" and fused.attention_backend(hd, attention) != "native":
+        return False, f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM}, got {hd}"
+    p = next(model.parameters())
+    if not p.is_cuda or p.dtype != BF:
+        return False, "needs CUDA + bfloat16"
+    return True, "ok"
+
+
 class _Layer:
-    """Views of one GPT-NeoX layer's parameters and gradients."""
+    """Views of one GPT-NeoX layer's parameters and gradients (None where a mode has no such tensor: the LoRA factors in full-rank
+    training, the projection-weight gradients under ReLoRA)."""
 
     __slots__ = ("W_qkv", "W_o", "W_h", "W_4", "A_qkv", "B_qkv", "b_qkv", "A_o", "B_o", "b_o", "A_h", "B_h", "b_h", "A_4", "B_4", "b_4",
                  "w1", "c1", "w2", "c2", "gA_qkv", "gB_qkv", "gb_qkv", "gA_o", "gB_o", "gb_o", "gA_h", "gB_h", "gb_h", "gA_4", "gB_4",
-                 "gb_4", "gw1", "gc1", "gw2", "gc2", "key_qkv", "key_o", "key_h", "key_4", "mods")
+                 "gb_4", "gw1", "gc1", "gw2", "gc2", "key_qkv", "key_o", "key_h", "key_4", "mods", "gW_qkv", "gW_o", "gW_h", "gW_4")
+
+    def __init__(self):
+        for k in self.__slots__:
+            setattr(self, k, None)
 
 
 class FusedPythiaStepper(FusedStepperBase):
-    def __init__(self, model: ReLoRaModel, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
+    """``model`` is a ``ReLoRaModel`` around a GPT-NeoX (ReLoRA: frozen weights, trainable LoRA factors) or a bare
+    ``GPTNeoXForCausalLM`` (full-rank training: the projection weights are trainable and live in the flat store; every projection
+    is the ReLoRA one without its low-rank branch)."""
+
+    def __init__(self, model, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, symm_factory=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
-                 overlap_wgrad: bool = True, attention: str = "auto"):
-        ok, why = supports(model)
+                 overlap_wgrad: bool = True, attention: str = "auto", deterministic: bool = False):
+        self.full = not isinstance(model, ReLoRaModel)
+        ok, why = supports_full_rank(model) if self.full else supports(model)
         if not ok:
             raise RuntimeError(why)
         self.model, self.info = model, info
-        self.inner: GPTNeoXForCausalLM = model.wrapped_model
+        self.inner: GPTNeoXForCausalLM = model if self.full else model.wrapped_model
         self.C = fused._C()
         self.ga = grad_accumulation
         self.clip = clip_grad_norm
@@ -103,10 +154,10 @@ class FusedPythiaStepper(FusedStepperBase):
         cfg = self.inner.config
         self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
         self.hd = self.h // self.nh
-        self.r = model.r
+        self.r = 0 if self.full else model.r
         self.L = cfg.num_hidden_layers
-        self.p = float(model.lora_dropout)
-        self.scale = float(model.lora_alpha) / model.r
+        self.p = 0.0 if self.full else float(model.lora_dropout)
+        self.scale = 1.0 if self.full else float(model.lora_alpha) / model.r
         self.device = info.device
         self.fp8 = self.fp8_bwd = False
         broadcast_params(model)
@@ -130,7 +181,10 @@ class FusedPythiaStepper(FusedStepperBase):
         for layer in layers:
             at, mlp = layer.attention, layer.mlp
             for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h):
-                add(m.lora_A.weight); add(m.lora_B.weight); add(m.bias)
+                if self.full:
+                    add(m.weight); add(m.bias)
+                else:
+                    add(m.lora_A.weight); add(m.lora_B.weight); add(m.bias)
             for ln in (layer.input_layernorm, layer.post_attention_layernorm):
                 add(ln.weight); add(ln.bias)
         add(neox.embed_in.weight)
@@ -149,6 +203,17 @@ class FusedPythiaStepper(FusedStepperBase):
             at, mlp = layer.attention, layer.mlp
             S = _Layer()
             for tag, m in (("qkv", at.query_key_value), ("o", at.dense), ("h", mlp.dense_h_to_4h), ("4", mlp.dense_4h_to_h)):
+                if self.full:
+                    # trainable weight, [out, in] in the flat store; query_key_value's rows are in the head-interleaved order
+                    # of dqkv, so its gradient needs no permutation
+                    W, gW = pv(m.weight)
+                    b, gb = pv(m.bias)
+                    for k, v in (("W_", W), ("gW_", gW), ("b_", b), ("gb_", gb)):
+                        setattr(S, k + tag, v)
+                    # sanity: the store views must alias the module parameters
+                    assert W.data_ptr() == m.weight.data_ptr() and W.shape == m.weight.shape
+                    assert b.data_ptr() == m.bias.data_ptr()
+                    continue
                 setattr(S, "W_" + tag, m.weight.data)  # frozen weight, [out, in] contiguous as the module keeps it
                 A, gA = pv(m.lora_A.weight)
                 B, gB = pv(m.lora_B.weight)
@@ -179,7 +244,11 @@ class FusedPythiaStepper(FusedStepperBase):
         self.side = torch.cuda.Stream(device=self.device) if overlap_wgrad else None
         self.fused_dx = True
         self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0")) or 4096
-        self.wgrad_split_k = 0
+        # --deterministic (full-rank training only): the weight-gradient GEMMs run without split-K, so one CTA owns an output tile
+        # for the whole token reduction.  The 1-D gradients (LayerNorm γ / β and the projection biases) stay column sums whose
+        # block partials meet in fp32 atomics.
+        det = deterministic or os.environ.get("RELORA_B200_DETERMINISTIC", "0") == "1"
+        self.wgrad_split_k = 1 if (self.full and det) else 0
         self.deterministic_embedding = os.environ.get("RELORA_B200_ATOMIC_EMBEDDING", "0") != "1"
 
     # ------------------------------------------------------------------ buffers
@@ -199,7 +268,10 @@ class FusedPythiaStepper(FusedStepperBase):
         self.xd_o = e(L, M, h)                       # attention output (dropout copy when p > 0): LoRA input of dense
         self.z = e(L, M, f)                          # pre-GELU
         self.xd_4 = e(L, M, f)                       # GELU output (dropout copy when p > 0): LoRA input of dense_4h_to_h
-        self.u_qkv, self.u_o, self.u_h, self.u_4 = e(L, M, r), e(L, M, r), e(L, M, r), e(L, M, r)
+        if self.full:  # no low-rank branch: no u / du buffers, and the input gradient needs no separate base product
+            self.u_qkv = self.u_o = self.u_h = self.u_4 = [None] * L
+        else:
+            self.u_qkv, self.u_o, self.u_h, self.u_4 = e(L, M, r), e(L, M, r), e(L, M, r), e(L, M, r)
         if not self.parallel:
             self.x1 = e(L, M, h)
             self.mean2, self.rstd2 = f32(L, M), f32(L, M)
@@ -212,10 +284,14 @@ class FusedPythiaStepper(FusedStepperBase):
         self.a = e(M, f)
         self.mean_f, self.rstd_f = f32(M), f32(M)
         self.xf, self.dxf = e(M, h), e(M, h)
-        self.dx_a, self.dx_b, self.dxn1, self.dxn2, self.dattn, self.tmp_h = e(M, h), e(M, h), e(M, h), e(M, h), e(M, h), e(M, h)
+        self.dx_a, self.dx_b, self.dxn1, self.dxn2, self.dattn = e(M, h), e(M, h), e(M, h), e(M, h), e(M, h)
         self.dqkv = e(M, 3 * h)
-        self.da, self.dz, self.tmp_f = e(M, f), e(M, f), e(M, f)
-        self.du_bufs = {"4": e(M, r), "h": e(M, r), "o": e(M, r), "qkv": e(M, r)}
+        self.da, self.dz = e(M, f), e(M, f)
+        if self.full:
+            self.tmp_h = self.tmp_f = None
+        else:
+            self.tmp_h, self.tmp_f = e(M, h), e(M, f)
+            self.du_bufs = {"4": e(M, r), "h": e(M, r), "o": e(M, r), "qkv": e(M, r)}
         ldv = (self.V + 7) // 8 * 8
         self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
         self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
@@ -330,11 +406,11 @@ class FusedPythiaStepper(FusedStepperBase):
             S = self.layers[l]
             # ---- MLP: x_next = a·W_4ᵀ + u_4·B_4ᵀ + b_4 + x1   (output gradient dx)
             self._lora_group_bwd(dx, S.B_4, S.W_4, S.A_4, S.gA_4, S.gB_4, self.xd_4[l], self.u_4[l], [S.key_4],
-                                 G=1, K=f, Ng=h, base_out=self.tmp_f, out=self.da, tag="4")
+                                 G=1, K=f, Ng=h, base_out=self.tmp_f, out=self.da, tag="4", gW=S.gW_4)
             self._join("h")  # the previous layer's dense_h_to_4h weight gradients read dz / du
             C.gelu_bwd(self.da, self.z[l], self.dz, self.tanh, dbias=S.gb_h)
             self._lora_group_bwd(self.dz, S.B_h, S.W_h, S.A_h, S.gA_h, S.gB_h, self.xd2[l], self.u_h[l], [S.key_h],
-                                 G=1, K=h, Ng=f, base_out=self.tmp_h, out=self.dxn2, tag="h")
+                                 G=1, K=h, Ng=f, base_out=self.tmp_h, out=self.dxn2, tag="h", gW=S.gW_h)
             if self.parallel:
                 d_attn_out = dx  # dense's output gradient is the block's
             else:
@@ -345,7 +421,7 @@ class FusedPythiaStepper(FusedStepperBase):
                 d_attn_out = dx
             # ---- attention: x1 = attn·W_oᵀ + u_o·B_oᵀ + b_o + x
             self._lora_group_bwd(d_attn_out, S.B_o, S.W_o, S.A_o, S.gA_o, S.gB_o, self.xd_o[l], self.u_o[l], [S.key_o],
-                                 G=1, K=h, Ng=h, base_out=self.tmp_h, out=self.dattn, tag="o")
+                                 G=1, K=h, Ng=h, base_out=self.tmp_h, out=self.dattn, tag="o", gW=S.gW_o)
             if self.native_attn:
                 self._join("qkv")  # the previous layer's query_key_value weight gradients read dqkv / du
                 C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
@@ -361,7 +437,7 @@ class FusedPythiaStepper(FusedStepperBase):
                 C.neox_rope(self.dqkv, T, nh, hd, self.rot, self.cos, self.sin, 0, True)  # back through the rotation of q, k
             C.colsum(self.dqkv, S.gb_qkv)
             self._lora_group_bwd(self.dqkv, S.B_qkv, S.W_qkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd1[l], self.u_qkv[l], [S.key_qkv],
-                                 G=1, K=h, Ng=3 * h, base_out=self.tmp_h, out=self.dxn1, tag="qkv")
+                                 G=1, K=h, Ng=3 * h, base_out=self.tmp_h, out=self.dxn1, tag="qkv", gW=S.gW_qkv)
             self._join("o")  # this layer's dense / dense_4h_to_h weight gradients read the buffer written next
             if self.parallel:
                 # dx = dx_next + LN1ᵀ(dxn1) + LN2ᵀ(dxn2); Σ dx_next is the bias gradient of both dense and dense_4h_to_h
@@ -394,4 +470,6 @@ class FusedPythiaStepper(FusedStepperBase):
     @torch.no_grad()
     def merge_and_reinit(self):
         """W += s·B@A per module (wgmma GEMM accumulating into W in fp32), then the hash re-init of the module path."""
+        if self.full:
+            raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
         self._merge_modules([(m, (m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data)) for S in self.layers for m in S.mods])

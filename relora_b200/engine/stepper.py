@@ -203,7 +203,7 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
             from ..models.llama import LlamaForCausalLM
             from ..models.pythia import GPTNeoXForCausalLM
             from .fused_llama import supports_full_rank
-            from .fused_pythia import FusedPythiaStepper, supports as pythia_supports
+            from .fused_pythia import FusedPythiaStepper, supports as pythia_supports, supports_full_rank as pythia_supports_full_rank
 
             if isinstance(model, LlamaForCausalLM):
                 ok, why = supports_full_rank(model, args)
@@ -211,6 +211,13 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
                     return FusedLlamaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
                                              attention=getattr(args, "attention", "auto"),
                                              deterministic=bool(getattr(args, "deterministic", False)), **kw)
+                raise RuntimeError(f"--engine fused requested but not applicable: {why}")
+            if isinstance(model, GPTNeoXForCausalLM):
+                ok, why = pythia_supports_full_rank(model, args)
+                if ok:
+                    return FusedPythiaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
+                                              attention=getattr(args, "attention", "auto"),
+                                              deterministic=bool(getattr(args, "deterministic", False)), **kw)
                 raise RuntimeError(f"--engine fused requested but not applicable: {why}")
             ok, why_p = pythia_supports(model, args)
             if ok:
