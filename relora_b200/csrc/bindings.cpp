@@ -259,6 +259,13 @@ void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Te
   rb::lora_dx(d, cur_stream());
 }
 
+// The attention kernels read out rows with 16-byte loads and store 4-byte pairs into out / dqkv, so those tensors obey the
+// rule the TMA maps enforce for qkv / dout: a 16-byte-aligned base and a row pitch that is a multiple of 8 elements.
+void chk_attn_rows(const Tensor& t, const char* name) {
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0 && t.stride(0) % 8 == 0, "attention: ", name,
+              " needs a 16-byte-aligned base and a row pitch that is a multiple of 8 elements");
+}
+
 // causal flash attention over the packed (post-RoPE) qkv buffer [B*T, (nh + 2*nkv)*hd]; nkv < 0 means nkv = nh
 void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64_t T, int64_t nh, int64_t hd, double scale, bool interleaved,
                    int64_t nkv) {
@@ -267,6 +274,7 @@ void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64
   TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == (nh + 2 * nkv) * hd, "qkv must be [B*T, (nh+2*nkv)*hd]");
   TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd, "out must be [B*T, nh*hd]");
   TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
+  chk_attn_rows(out, "out");
   rb::AttnDesc d;
   d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0); d.lse = lse.data_ptr<float>();
   d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.nkv = (int)nkv; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
@@ -283,6 +291,8 @@ void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, con
   TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd && dout.size(0) == B * T && dout.size(1) == nh * hd, "out / dout must be [B*T, nh*hd]");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
   TORCH_CHECK(delta.is_cuda() && delta.scalar_type() == at::kFloat && delta.is_contiguous() && delta.numel() == B * nh * T, "delta must be fp32 [B, nh, T]");
+  chk_attn_rows(out, "out");
+  chk_attn_rows(dqkv, "dqkv");
   rb::AttnBwdDesc d;
   d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0);
   d.dout = dout.data_ptr(); d.ld_dout = dout.stride(0); d.lse = lse.data_ptr<float>(); d.delta = delta.data_ptr<float>();

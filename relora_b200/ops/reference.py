@@ -368,6 +368,171 @@ def assert_gemm_close(out: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor,
     return worst
 
 
+# ----------------------------------------------------------------------------- wgmma attention (csrc/attention.h)
+# Coefficients of assert_attention_close.  ATTN_C_P / ATTN_C_D are analytic: bf16 round-to-nearest has a unit roundoff of 2⁻⁸
+# (8 significant bits), and P (forward, dV) and dS (dQ, dK) are packed to bf16 once as wgmma register operands; twice that
+# rounding leaves room for the fp32 accumulation, ex2.approx and the fp32 row sums, which are all below 2⁻²⁰ relative.
+# ATTN_C_S / ATTN_C_L are set from the worst element observed on an H100 80GB HBM3 (700 W) over tests/test_attention_modes_gpu.py,
+# with headroom: the lse error reached 1.0e-7·(1 + |lse|) where the score term is zero (q = 0), and 5.0e-7 per unit of the score
+# term elsewhere (the rising-maximum regime at head_dim 128, the c_l share included).  ATTN_C_S is the constant the GEMM uses for
+# the same fp32 wgmma accumulation (GEMM_C_ACC_BF16).
+ATTN_C_P = 2.0 ** -7
+ATTN_C_D = 2.0 ** -7
+ATTN_C_S = 2.0 ** -16
+ATTN_C_L = 2.0 ** -20
+# The kernels flush fp32 subnormals (ex2.approx.ftz, FTZ arithmetic): every term of a sum may lose up to this much absolutely.
+ATTN_FTZ = 2.0 ** -126
+_ATTN_C = {"out": ATTN_C_P, "lse": ATTN_C_L, "dq": ATTN_C_D, "dk": ATTN_C_D, "dv": ATTN_C_D}
+_LOG2E = 1.0 / math.log(2.0)
+
+
+def attention_unpack(x: torch.Tensor, B: int, T: int, nh: int, hd: int, *, nkv: int = -1, interleaved: bool = False):
+    """Views ``(q, k, v)`` — ``[B, nh, T, hd]``, ``[B, nkv, T, hd]``, ``[B, nkv, T, hd]`` — of a packed ``qkv`` / ``dqkv``
+    buffer ``[B*T, (nh + 2·nkv)·hd]``: ``[q: nh | k: nkv | v: nkv]`` heads per row, or ``[nh, (q|k|v), hd]`` when
+    ``interleaved`` (GPT-NeoX ``query_key_value``).  A ``[B*T, nh·hd]`` buffer (``out`` / ``dout``) unpacks with
+    :func:`attention_heads`."""
+    nkv = nh if nkv < 0 else nkv
+    if interleaved and nkv != nh:
+        raise ValueError("attention: the interleaved layout has no grouped-query form")
+    if interleaved:
+        x5 = x.reshape(B, T, nh, 3, hd)
+        return tuple(x5[:, :, :, i].transpose(1, 2) for i in range(3))
+    x4 = x.reshape(B, T, nh + 2 * nkv, hd)
+    return tuple(x4[:, :, a:b].transpose(1, 2) for a, b in ((0, nh), (nh, nh + nkv), (nh + nkv, nh + 2 * nkv)))
+
+
+def attention_heads(x: torch.Tensor, B: int, T: int, nh: int, hd: int) -> torch.Tensor:
+    """``[B, nh, T, hd]`` view of a ``[B*T, nh·hd]`` buffer (``out`` / ``dout``)."""
+    return x.reshape(B, T, nh, hd).transpose(1, 2)
+
+
+def _spread(w: torch.Tensor, v: torch.Tensor, o: torch.Tensor) -> torch.Tensor:
+    """Σ_k w_ik |v_kj − o_ij| over ``w [B, H, T, T]``, ``v, o [B, H, T, hd]``, a few query rows at a time."""
+    Bh, T, hd = w.shape[0] * w.shape[1], w.shape[2], v.shape[-1]
+    res = torch.empty_like(o)
+    step = max(1, (1 << 24) // (Bh * T * hd))
+    for i0 in range(0, T, step):
+        i1 = min(T, i0 + step)
+        res[:, :, i0:i1] = (w[:, :, i0:i1, :, None] * (v[:, :, None] - o[:, :, i0:i1, None]).abs()).sum(3)
+    return res
+
+
+def attention_ref(qkv: torch.Tensor, B: int, T: int, nh: int, hd: int, scale: float, interleaved: bool = False, nkv: int = -1,
+                  out: Optional[torch.Tensor] = None, dout: Optional[torch.Tensor] = None) -> dict:
+    """fp64 reference of the extension's ``attention_fwd(qkv, out, lse, B, T, nh, hd, scale, interleaved, nkv)`` and, with
+    ``out`` (the bf16 output of the forward, as passed to the backward) and ``dout``, of ``attention_bwd``.  Computed on the
+    device of ``qkv``.  Returns ``{name: (ref, bound, score, floor)}`` for ``out``, ``lse`` and, for the backward, ``dq``, ``dk``,
+    ``dv``, laid out as :func:`attention_unpack` / :func:`attention_heads` lay out the kernel's buffers (``lse``: ``[B, nh, T]``).
+
+    Query head h of batch b reads KV head κ(h) = h // (nh / nkv) (h itself when interleaved).  For query i and key k ≤ i, all
+    from the bf16 inputs as stored:
+
+        s_ik = scale·Σ_d q_id k_kd     σ_ik = |scale|·Σ_d |q_id||k_kd|     P = causal softmax of s     O = P·V
+        lse_i = log2 Σ_k exp(s_ik)     (the log2 domain the kernels store)
+        dP_ik = Σ_j dO_ij v_kj     Δ_i = Σ_j dO_ij O'_ij     dS_ik = P_ik (dP_ik − Δ_i)
+        dQ = scale·dS·K     dK_κ = scale·Σ_{h: κ(h) = κ} dSᵀ·Q     dV_κ = Σ_{h: κ(h) = κ} Pᵀ·dO
+
+    O' is ``out`` as passed: the bf16 rounding of the forward output inside Δ is part of the definition, as it is in the
+    kernels, and is not a tolerance term.
+
+    ``bound`` is the magnitude the operand roundings scale with (:func:`assert_attention_close` multiplies it by c_p, c_l or
+    c_d):
+
+        out: Σ_k P_ik |v_kj|          P packed to bf16 as the register A operand of O += P·V; ex2.approx; the fp32 row sum
+        lse: 1 + |lse_i|              fp32 row maximum and row sum, ex2.approx and log2 of the sum
+        dq:  |scale|·Σ_k D_ik |k_kd|  dS packed to bf16 for dQ += dS·K; fp32 dP and Δ (Δ from the bf16 ``out``)
+        dk:  |scale|·Σ D_ik |q_id|    dS packed to bf16 for dK += dSᵀ·Q
+        dv:  Σ P_ik |dO_ij|           P packed to bf16 for dV += Pᵀ·dO
+        with D_ik = P_ik·(Σ_j |dO_ij||v_kj| + Σ_j |dO_ij||O'_ij|) ≥ |dS_ik|, sums over the group's query heads for dk / dv.
+
+    ``score`` is the magnitude the fp32 score error scales with (multiplied by c_s): the scores are accumulated in fp32 and
+    rounded again in s·scale·log2(e), an error of up to c_s·σ_ik in s_ik.  It moves O_ij by Σ_k P_ik δs_ik (v_kj − O_ij) and
+    lse_i by log2(e)·Σ_k P_ik δs_ik, so
+
+        out: Σ_k P_ik σ_ik |v_kj − O_ij|     lse: log2(e)·Σ_k P_ik σ_ik
+
+    The backward recomputes P from s and the stored lse, so P_ik carries a relative error of up to c_s·ρ_ik with
+    ρ_ik = σ_ik + Σ_k' P_ik' σ_ik' (its own score and the lse); the part c_l·(1 + |lse|) of the lse error adds at most
+    ln2·c_l·(1 + |lse|) relative, below 2⁻¹⁰ for |lse| < 1000, which c_d covers.  Hence dq: |scale|·Σ_k D_ik ρ_ik |k_kd|,
+    dk: |scale|·Σ D_ik ρ_ik |q_id|, dv: Σ P_ik ρ_ik |dO_ij|.
+
+    ``floor`` is the absolute error of flushing fp32 subnormals to zero (ATTN_FTZ = 2⁻¹²⁶ per flushed factor or product): a
+    probability, a dS element or a product that underflows loses at most 2⁻¹²⁶ times the other factors of its term, and the
+    output itself at most 2⁻¹²⁶.  With A_ik = Σ_j |dO_ij||v_kj| + Σ_j |dO_ij||O'_ij| (≥ |dP_ik − Δ_i|) over the causal k ≤ i:
+
+        out: 2⁻¹²⁶·(1 + Σ_k (1 + |v_kj|))                  lse: 0
+        dq:  2⁻¹²⁶·(1 + |scale|·Σ_k (1 + A_ik)(1 + |k_kd|))   dk: 2⁻¹²⁶·(1 + |scale|·Σ (1 + A_ik)(1 + |q_id|))
+        dv:  2⁻¹²⁶·(1 + Σ (1 + |dO_ij|))
+
+    It is negligible unless the result itself is below the fp32 normal range (|s| in the hundreds)."""
+    nkv = nh if nkv < 0 else nkv
+    group = nh // nkv
+    q, k, v = attention_unpack(qkv.to(_F64), B, T, nh, hd, nkv=nkv, interleaved=interleaved)
+    kvh = torch.arange(nh, device=qkv.device) // group
+    kr, vr = k[:, kvh], v[:, kvh]
+    causal = torch.ones(T, T, dtype=torch.bool, device=qkv.device).tril()
+    s = (scale * (q @ kr.transpose(-1, -2))).masked_fill(~causal, -math.inf)
+    sig = (abs(scale) * (q.abs() @ kr.abs().transpose(-1, -2))).masked_fill(~causal, 0.0)
+    lse_e = torch.logsumexp(s, -1)
+    P = torch.exp(s - lse_e[..., None])
+    o = P @ vr
+    Psig = P * sig
+    cf = causal.to(_F64)
+    lse2 = lse_e * _LOG2E
+    res = {"out": (o, P @ vr.abs(), _spread(Psig, vr, o), ATTN_FTZ * (1.0 + cf @ (1.0 + vr.abs()))),
+           "lse": (lse2, 1.0 + lse2.abs(), _LOG2E * Psig.sum(-1), torch.zeros_like(lse2))}
+    if out is None and dout is None:
+        return res
+    if out is None or dout is None:
+        raise ValueError("attention_ref: the backward needs both out and dout")
+    Op, dO = attention_heads(out.to(_F64), B, T, nh, hd), attention_heads(dout.to(_F64), B, T, nh, hd)
+    dS = P * (dO @ vr.transpose(-1, -2) - (dO * Op).sum(-1, keepdim=True))
+    A = dO.abs() @ vr.abs().transpose(-1, -2) + (dO.abs() * Op.abs()).sum(-1, keepdim=True)
+    D = P * A
+    M = cf * (1.0 + A)
+    rho = sig + Psig.sum(-1, keepdim=True)
+    Drho, Prho = D * rho, P * rho
+    per_kv = lambda x: x.reshape(B, nkv, group, T, hd).sum(2)  # noqa: E731  (query head h = κ·group + g)
+    sc = abs(scale)
+    tT = lambda x: x.transpose(-1, -2)  # noqa: E731
+    res["dq"] = (scale * (dS @ kr), sc * (D @ kr.abs()), sc * (Drho @ kr.abs()), ATTN_FTZ * (1.0 + sc * (M @ (1.0 + kr.abs()))))
+    res["dk"] = (per_kv(scale * (tT(dS) @ q)), per_kv(sc * (tT(D) @ q.abs())), per_kv(sc * (tT(Drho) @ q.abs())),
+                 ATTN_FTZ * (1.0 + per_kv(sc * (tT(M) @ (1.0 + q.abs())))))
+    res["dv"] = (per_kv(tT(P) @ dO), per_kv(tT(P) @ dO.abs()), per_kv(tT(Prho) @ dO.abs()),
+                 ATTN_FTZ * (1.0 + per_kv(tT(cf) @ (1.0 + dO.abs()))))
+    return res
+
+
+def assert_attention_close(name: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, score: torch.Tensor,
+                           floor: torch.Tensor) -> float:
+    """Element-wise check of one attention result (``name`` in out, lse, dq, dk, dv) against :func:`attention_ref`:
+
+        |got − ref| ≤ c_out·|ref| + c·bound + c_s·score + floor
+
+    ``c_out`` is the output rounding (2⁻⁸ for bf16, 0 for the fp32 lse, whose rounding c_l covers), ``c`` is
+    :data:`ATTN_C_P` (out), :data:`ATTN_C_L` (lse) or :data:`ATTN_C_D` (dq, dk, dv), ``c_s`` :data:`ATTN_C_S`.  A NaN fails.
+    Returns the worst ratio of error to tolerance (<= 1 when it passes); the failure message names the element
+    (b, head, row, col)."""
+    g = got.to(_F64)
+    c_out = 2.0 ** -8 if got.dtype == torch.bfloat16 else 0.0
+    err = (g - ref).abs()
+    tol = c_out * ref.abs() + _ATTN_C[name] * bound + ATTN_C_S * score + floor
+    ratio = torch.where(tol > 0, err / tol.clamp(min=1e-300), torch.where(err == 0, 0.0, math.inf))
+    ratio = torch.nan_to_num(ratio, nan=math.inf, posinf=math.inf)
+    flat = int(torch.argmax(ratio))
+    idx = list(torch.unravel_index(torch.tensor(flat), ratio.shape))
+    idx = tuple(int(i) for i in idx)
+    worst = float(ratio[idx])
+    if not worst <= 1.0:
+        n_bad = int((ratio > 1.0).sum())
+        where = ", ".join(f"{n} {i}" for n, i in zip(("b", "head", "row", "col"), idx))
+        raise AssertionError(
+            f"attention {name} out of tolerance at {n_bad} of {ratio.numel()} elements; worst ratio {worst:.3g} at ({where}): "
+            f"got={float(g[idx]):.6g} ref={float(ref[idx]):.6g} tol={float(tol[idx]):.6g} (bound={float(bound[idx]):.6g}, "
+            f"score={float(score[idx]):.6g}, floor={float(floor[idx]):.3g})")
+    return worst
+
+
 # ----------------------------------------------------------------------------- merge
 def merge_delta(weight: torch.Tensor, lora_a: torch.Tensor, lora_b: torch.Tensor, scale: float) -> torch.Tensor:
     """W + s·B@A accumulated in fp32, rounded to ``weight.dtype`` (reference relora.py:275-276)."""

@@ -1,5 +1,6 @@
-"""The wgmma attention kernels at head sizes 72..256 (two to four 64-column panels per head): kernel numerics, the module path,
-the fused executor and the Pythia module path against torch SDPA (run on an H100: -m gpu)."""
+"""The wgmma attention kernels at head sizes 72..256 (two to four 64-column panels per head): the head-size refusals, the module
+path, the fused executor and the Pythia module path against torch SDPA (run on an H100: -m gpu).  The kernels' numerics at these
+head sizes are checked element by element in test_attention_modes_gpu.py."""
 import copy
 import math
 
@@ -37,38 +38,6 @@ def _rand(*shape, scale=1.0):
 def _relerr(a, b):
     a, b = a.float(), b.float()
     return float((a - b).norm() / b.norm().clamp(min=1e-12))
-
-
-@pytest.mark.parametrize("B,T,nh,hd", [(1, 320, 2, 80), (2, 200, 2, 96), (1, 1000, 2, 128), (1, 130, 1, 136), (1, 257, 2, 192),
-                                       (2, 64, 2, 256), (1, 2049, 1, 256)])
-def test_attention_wide_heads_fwd_bwd(C, B, T, nh, hd):
-    """Forward, lse and dq/dk/dv vs an fp32 reference; outputs start as NaN so an unwritten column panel or row tail shows."""
-    torch.manual_seed(T + hd)
-    h = nh * hd
-    qkv = _rand(B * T, 3 * h)
-    out = torch.full((B * T, h), float("nan"), device="cuda", dtype=BF)
-    lse = torch.full((B, nh, T), float("nan"), device="cuda", dtype=torch.float32)
-    scale = 1.0 / math.sqrt(hd)
-    C.attention_fwd(qkv, out, lse, B, T, nh, hd, scale)
-    assert not out.isnan().any() and not lse.isnan().any()
-    q, k, v = (qkv.view(B, T, 3, nh, hd)[:, :, i].transpose(1, 2).float().detach().requires_grad_() for i in range(3))
-    s = (q @ k.transpose(-1, -2)) * scale
-    mask = torch.ones(T, T, dtype=torch.bool, device="cuda").tril()
-    s = s.masked_fill(~mask, float("-inf"))
-    want = torch.softmax(s, dim=-1) @ v
-    assert _relerr(out.view(B, T, nh, hd).transpose(1, 2), want) < 8e-3
-    want_lse = torch.logsumexp(s, dim=-1) / math.log(2.0)
-    assert (lse - want_lse).abs().max() < 2e-2
-    dout = _rand(B * T, h, scale=0.5)
-    want.backward(dout.view(B, T, nh, hd).transpose(1, 2).float())
-    delta = torch.empty(B, nh, T, device="cuda", dtype=torch.float32)
-    dqkv = torch.full((B * T, 3 * h), float("nan"), device="cuda", dtype=BF)
-    C.attention_bwd(qkv, out, dout, lse, delta, dqkv, B, T, nh, hd, scale)
-    assert not dqkv.isnan().any()
-    d5 = dqkv.view(B, T, 3, nh, hd)
-    for i, (name, ref_t) in enumerate((("dq", q), ("dk", k), ("dv", v))):
-        e = _relerr(d5[:, :, i].transpose(1, 2), ref_t.grad)
-        assert e < 2e-2, (name, e)
 
 
 @pytest.mark.parametrize("hd", [84, 264])

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from gemm_forms import FORMS, lora_group_call, lora_group_shapes
+from guarded_buffers import Guarded
 from relora_b200.ops import reference as ref
 
 pytestmark = pytest.mark.gpu
@@ -40,33 +41,9 @@ def F():
     return fused
 
 
-class _Buf:
-    """``view`` at row 1, column 16 of a larger buffer (pitch a multiple of 16 elements, so every row start stays 16-byte
-    aligned); the rest of the buffer holds ``fill``."""
-
-    def __init__(self, src: torch.Tensor, fill, interior=None):
-        self.src_shape = tuple(src.shape)
-        if src.dim() == 1:
-            self.buf = torch.full((src.numel() + 48,), fill, dtype=src.dtype, device="cuda")
-            self.view = self.buf[16:16 + src.numel()]
-        else:
-            rows, cols = src.shape
-            pitch = (cols + 16 + 40 + 15) // 16 * 16
-            self.buf = torch.full((rows + 3, pitch), fill, dtype=src.dtype, device="cuda")
-            self.view = self.buf[1:1 + rows, 16:16 + cols]
-        self.view.copy_(src if interior is None else interior)
-        self.snap = self.buf.clone()
-
-    def guards_intact(self) -> bool:
-        b = self.buf.clone()
-        b[self._region()] = self.snap[self._region()]
-        bits = {1: torch.uint8, 2: torch.int16, 4: torch.int32}[b.element_size()]
-        return torch.equal(b.view(bits), self.snap.view(bits))
-
-    def _region(self):
-        if len(self.src_shape) == 1:
-            return slice(16, 16 + self.src_shape[0])
-        return (slice(1, 1 + self.src_shape[0]), slice(16, 16 + self.src_shape[1]))
+def _Buf(src, fill, interior=None):
+    # pitch a multiple of 16 elements: every row start stays 16-byte aligned for the one-byte fp8 operands too
+    return Guarded(src, fill, interior, pitch_multiple=16)
 
 
 def _operand(t):

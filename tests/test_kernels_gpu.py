@@ -550,41 +550,6 @@ def test_llama_module_path_on_gpu_matches_cpu_reference():
             assert _relerr(g_fused[n], p.grad.float()) < 0.12, n
 
 
-# ----------------------------------------------------------------------------------------- attention
-@pytest.mark.parametrize("B,T,nh,hd", [(2, 512, 4, 48), (1, 320, 2, 64), (3, 128, 2, 32), (1, 1000, 3, 64), (2, 64, 1, 16)])
-def test_attention_fwd_bwd(C, B, T, nh, hd):
-    """wgmma causal flash attention over the packed qkv buffer vs an fp32 PyTorch reference (forward, lse and dq/dk/dv)."""
-    torch.manual_seed(T + hd)
-    h = nh * hd
-    qkv = _rand(B * T, 3 * h)
-    out = torch.zeros(B * T, h, device="cuda", dtype=BF)
-    lse = torch.zeros(B, nh, T, device="cuda", dtype=torch.float32)
-    scale = 1.0 / math.sqrt(hd)
-    C.attention_fwd(qkv, out, lse, B, T, nh, hd, scale)
-    q, k, v = (qkv.view(B, T, 3, nh, hd)[:, :, i].transpose(1, 2).float().detach().requires_grad_() for i in range(3))
-    s = (q @ k.transpose(-1, -2)) * scale
-    mask = torch.ones(T, T, dtype=torch.bool, device="cuda").tril()
-    s = s.masked_fill(~mask, float("-inf"))
-    p = torch.softmax(s, dim=-1)
-    want = p @ v  # [B, nh, T, hd]
-    got = out.view(B, T, nh, hd).transpose(1, 2)
-    assert _relerr(got, want) < 8e-3
-    want_lse = torch.logsumexp(s, dim=-1) / math.log(2.0)
-    assert (lse - want_lse).abs().max() < 2e-2
-    dout = _rand(B * T, h, scale=0.5)
-    want.backward(dout.view(B, T, nh, hd).transpose(1, 2).float())
-    delta = torch.empty(B, nh, T, device="cuda", dtype=torch.float32)
-    # both backward forms: dQ recomputing S / dP, and dQ = dS·K from the dSᵀ tiles the dK/dV kernel stores (the default)
-    for use_ws in (False, True):
-        dqkv = torch.zeros(B * T, 3 * h, device="cuda", dtype=BF)
-        ws = torch.full((C.attention_ds_workspace_elems(B, T, nh),), float("nan"), device="cuda", dtype=BF) if use_ws else None
-        C.attention_bwd(qkv, out, dout, lse, delta, dqkv, B, T, nh, hd, scale, ws)
-        d5 = dqkv.view(B, T, 3, nh, hd)
-        for i, (name, ref_t) in enumerate((("dq", q), ("dk", k), ("dv", v))):
-            e = _relerr(d5[:, :, i].transpose(1, 2), ref_t.grad)
-            assert e < 2e-2, (name, use_ws, e)
-
-
 # ----------------------------------------------------------------------------------------- fp8 frozen-weight path
 @pytest.mark.parametrize("M,N,K,pair", [(256, 256, 256, 0), (1000, 768, 640, 0), (512, 1024, 2048, 1), (12288, 2304, 768, 0)])
 def test_gemm_fp8_frozen_path_with_bf16_lora_branch(C, F, M, N, K, pair):
