@@ -78,7 +78,7 @@ def main():
             except Exception as e:  # keep benchmarking the other variants
                 rec[f"ours_bn{bn}_error"] = str(e)[:200]
         try:
-            t = timeit(lambda: F.gemm(x, W, out, block_n=256, pair=1), flush)
+            t = timeit(lambda: F.gemm(x, W, out, block_n=128, pair=1), flush)
             rec["ours_pair_us"] = t * 1e6
             rec["ours_pair_tflops"] = flops / t / 1e12
             rec["ours_pair_frac_of_measured_peak"] = flops / t / 1e12 / peak
@@ -91,7 +91,7 @@ def main():
             t = timeit(lambda: F.gemm(x, W, out, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, block_n=bn, pair=0), flush)
             rec["ours_fused_lora_us"] = t * 1e6
             rec["ours_fused_lora_tflops"] = fl2 / t / 1e12
-            t = timeit(lambda: F.gemm(x, W, out, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, block_n=256, pair=1), flush)
+            t = timeit(lambda: F.gemm(x, W, out, a2=u, b2=B, K2=r, n_per_group=Ng, a2_group_kofs=r, block_n=128, pair=1), flush)
             rec["ours_fused_lora_pair_us"] = t * 1e6
             rec["ours_fused_lora_pair_tflops"] = fl2 / t / 1e12
             # what the reference does for the same math: F.linear + 2 small GEMMs + mul + add (no dropout here)
@@ -108,7 +108,7 @@ def main():
             t = timeit(lambda: F.gemm(dy, W, dx, M=Mx, N=K, K1=N, b1_mn=True, pair=0), flush)
             rec["ours_dx_mnB_us"] = t * 1e6
             rec["ours_dx_mnB_tflops"] = flops / t / 1e12
-            t = timeit(lambda: F.gemm(dy, W, dx, M=Mx, N=K, K1=N, b1_mn=True, block_n=256, pair=1), flush)
+            t = timeit(lambda: F.gemm(dy, W, dx, M=Mx, N=K, K1=N, b1_mn=True, block_n=128, pair=1), flush)
             rec["ours_dx_mnB_pair_us"] = t * 1e6
             rec["ours_dx_mnB_pair_tflops"] = flops / t / 1e12
             t = timeit(lambda: torch.matmul(dy, W, out=dx), flush)

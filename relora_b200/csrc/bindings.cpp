@@ -63,7 +63,7 @@ rb::Fp8Out fp8_out(const OptTensor& q8, const OptTensor& inv_scale, const OptTen
 void gemm(const Tensor& a1, const Tensor& b1, Tensor& out, int64_t M, int64_t N, int64_t K1, const OptTensor& a2, const OptTensor& b2,
           int64_t K2, bool a1_mn, bool b1_mn, int64_t n_per_group, int64_t a1_group_kofs, int64_t a2_group_kofs,
           const OptTensor& residual, double alpha, bool accumulate, int64_t block_n, int64_t split_k, int64_t b1_group_kofs,
-          bool b1_local_n, int64_t m_per_group, int64_t b1_mn_ofs_per_mgroup, const OptTensor& bias, int64_t /*cta_pair: no CTA-pair MMA on sm_90*/, int64_t fp8,
+          bool b1_local_n, int64_t m_per_group, int64_t b1_mn_ofs_per_mgroup, const OptTensor& bias, int64_t pair, int64_t fp8,
           const OptTensor& alpha_dev) {
   c10::cuda::CUDAGuard guard(out.device());
   rb::GemmDesc d;
@@ -92,7 +92,7 @@ void gemm(const Tensor& a1, const Tensor& b1, Tensor& out, int64_t M, int64_t N,
   TORCH_CHECK(out.scalar_type() == at::kBFloat16 || out.scalar_type() == at::kFloat, "out must be bf16 or fp32");
   TORCH_CHECK(out.size(0) >= M && out.size(1) >= N, "out too small");
   d.out = out.data_ptr(); d.ldc = out.stride(0); d.out_f32 = out.scalar_type() == at::kFloat;
-  d.accumulate = accumulate; d.alpha = (float)alpha; d.block_n = (int)block_n; d.split_k = (int)split_k;
+  d.accumulate = accumulate; d.alpha = (float)alpha; d.block_n = (int)block_n; d.split_k = (int)split_k; d.pair = (int)pair;
   d.b1_group_kofs = (int)b1_group_kofs; d.b1_local_n = b1_local_n; d.m_per_group = (int)m_per_group;
   d.b1_mn_ofs_per_mgroup = (int)b1_mn_ofs_per_mgroup;
   if (residual.has_value()) {
@@ -224,7 +224,7 @@ void fp8_prep(Tensor& state, const Tensor& w_scale, Tensor& inv_sx, Tensor& alph
 
 // out[M,N] = dy[M,Kb]·W[Kb,N] + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)     (fused input gradient of a stacked LoRA group)
 void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Tensor& a, Tensor& out, const OptTensor& seed,
-             std::vector<int64_t> keys, double p, const OptTensor& base) {
+             std::vector<int64_t> keys, double p, const OptTensor& base, int64_t pair) {
   chk_bf16(du, "du"); chk_bf16(a, "a"); chk_bf16(out, "out");
   chk_2d_rowmajor(du, "du"); chk_2d_rowmajor(a, "a"); chk_2d_rowmajor(out, "out");
   const int G = (int)keys.size();
@@ -255,6 +255,7 @@ void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Te
   d.inv_keep = (float)(1.0 / (1.0 - p));
   d.seed_ptr = u32ptr(seed);
   for (int i = 0; i < G; ++i) d.seed_key[i] = (uint32_t)keys[i];
+  d.pair = (int)pair;
   c10::cuda::CUDAGuard guard(out.device());
   rb::lora_dx(d, cur_stream());
 }
@@ -707,13 +708,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "relora_b200 sm_90a kernels";
   m.def("gemm", &gemm, "wgmma GEMM with fused LoRA K-extension");
   m.def("gemm_clear_descriptor_cache", &rb::gemm_clear_descriptor_cache);
-  // host-side schedule of one gemm call (no launch): (block_n, tma_store, dynamic shared memory bytes)
-  m.def("gemm_plan", [](int64_t block_n, bool out_f32, int64_t out_addr, int64_t ldc, int64_t n, int64_t split_k) {
+  // host-side schedule of one gemm call (no launch): (block_n, tma_store, dynamic shared memory bytes, CTA pairs)
+  m.def("gemm_plan", [](int64_t block_n, bool out_f32, int64_t out_addr, int64_t ldc, int64_t n, int64_t split_k, int64_t m,
+                        int64_t m_per_group, int64_t pair, int64_t k) {
     rb::GemmDesc d;
     d.block_n = (int)block_n; d.out_f32 = out_f32; d.out = reinterpret_cast<void*>(out_addr); d.ldc = ldc; d.N = (int)n;
+    d.M = (int)m; d.m_per_group = (int)m_per_group; d.pair = (int)pair; d.K1 = (int)k;
     const int bn = rb::gemm_block_n(d);
-    return py::make_tuple(bn, rb::gemm_uses_tma_store(d, bn, (int)split_k), rb::gemm_smem_bytes(bn));
-  }, py::arg("block_n"), py::arg("out_f32"), py::arg("out_addr"), py::arg("ldc"), py::arg("n"), py::arg("split_k"));
+    return py::make_tuple(bn, rb::gemm_uses_tma_store(d, bn, (int)split_k), rb::gemm_smem_bytes(bn), rb::gemm_pairs(d, bn));
+  }, py::arg("block_n"), py::arg("out_f32"), py::arg("out_addr"), py::arg("ldc"), py::arg("n"), py::arg("split_k"),
+     py::arg("m") = 0, py::arg("m_per_group") = 0, py::arg("pair") = -1, py::arg("k") = 0);
+  // (CTA pairs, TMA-store epilogue) of one lora_dx call with G = 1 and rank r
+  m.def("lora_dx_plan", [](int64_t m, int64_t n, int64_t pair, int64_t kb, int64_t r) {
+    rb::LoraDxDesc d;
+    d.M = (int)m; d.N = (int)n; d.pair = (int)pair; d.Kb = (int)kb; d.r = (int)r;
+    return py::make_tuple(rb::lora_dx_pairs(d), rb::lora_dx_uses_tma_store(d));
+  }, py::arg("m"), py::arg("n"), py::arg("pair") = -1, py::arg("kb") = 0, py::arg("r") = 128);
   m.def("rmsnorm_fwd", &rmsnorm_fwd, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("rstd"), py::arg("eps"), py::arg("xd"), py::arg("seed"),
         py::arg("keys"), py::arg("p"), py::arg("q8") = py::none(), py::arg("q_inv_scale") = py::none(), py::arg("q_amax") = py::none());
   m.def("rmsnorm_bwd", &rmsnorm_bwd);
@@ -734,7 +744,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("interleaved") = false, py::arg("nkv") = -1);
   m.def("attention_ds_workspace_elems", &rb::attention_ds_workspace_elems);
   m.def("lora_dx", &lora_dx, py::arg("dy"), py::arg("w"), py::arg("du"), py::arg("a"), py::arg("out"), py::arg("seed"), py::arg("keys"),
-        py::arg("p"), py::arg("base") = py::none());
+        py::arg("p"), py::arg("base") = py::none(), py::arg("pair") = -1);
   m.def("rope_inplace", &rope_inplace);
   m.def("rope_pack_bwd", &rope_pack_bwd, py::arg("dq"), py::arg("dk"), py::arg("dv"), py::arg("out"), py::arg("rotary_dim"), py::arg("cos"),
         py::arg("sin"), py::arg("pos0"), py::arg("nkv") = -1);

@@ -47,19 +47,49 @@ inline bool pdl_enabled() {
   }
   return v != 0;
 }
+// `cluster` > 1: the grid (a multiple of it) is launched as clusters of `cluster` CTAs along x
 template <typename... KArgs, typename... Args>
-inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+inline void launch_k_cluster(int cluster, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cluster > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n++].val.clusterDim = {(unsigned)cluster, 1, 1};
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = n;
   check(cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...), "cudaLaunchKernelEx");
+}
+template <typename... KArgs, typename... Args>
+inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+  launch_k_cluster(1, kern, grid, block, smem, s, std::forward<Args>(args)...);
+}
+// how many clusters of `cluster` CTAs of `kern` (one CTA per SM) fit on the device at once; an H100's GPCs need not hold an
+// even number of SMs, so this can be less than num_sms() / cluster
+template <typename... KArgs>
+inline int max_active_clusters(void (*kern)(KArgs...), int cluster, int threads, size_t smem) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(cluster, 1, 1);
+  cfg.blockDim = dim3(threads, 1, 1);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim = {(unsigned)cluster, 1, 1};
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  check(cudaOccupancyMaxActiveClusters(&n, kern, &cfg), "cudaOccupancyMaxActiveClusters");
+  if (n <= 0) throw std::runtime_error("no cluster of this kernel fits on the device");
+  return n;
 }
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

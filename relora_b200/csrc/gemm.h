@@ -46,6 +46,7 @@ struct GemmDesc {
   bool fp8 = false;  // A1 / B1 hold E4M3 bytes (K-major, leading dimensions in bytes); A2 / B2 (the LoRA branch) stay bf16
   int block_n = 0;  // 0 = auto, else 128 or 256
   int split_k = 1;  // 1 = off, 0 = auto, >1 = fixed (fp32 accumulate outputs only: partial sums via atomics)
+  int pair = -1;    // CTA pairs sharing the B tile (gemm_pairs): -1 = auto, 0 = off, 1 = wherever the call form allows
   // dropout-combine epilogue (backward of the LoRA branch): if n_lora_acc > 0 the A2/B2 products of
   // the first n_lora_acc K2-windows (each of width lora_r) are kept in separate accumulators and combined as
   //     out = acc0 + sum_g keep_g(row, col) * acc_{1+g} * inv_keep
@@ -63,6 +64,9 @@ void gemm_bf16(const GemmDesc& d, cudaStream_t stream);
 int gemm_block_n(const GemmDesc& d);
 bool gemm_uses_tma_store(const GemmDesc& d, int block_n, int split_k);
 int gemm_smem_bytes(int block_n);
+// whether the call runs as CTA pairs: 128-wide tiles, at least two M tiles, M groups of whole pairs; auto: long reductions
+// into wide outputs
+bool gemm_pairs(const GemmDesc& d, int block_n);
 
 // Input gradient of a stacked LoRA group with the dropout mask applied in the epilogue:
 //   out[M,N] = dy[M,Kb]·W[Kb,N] + inv_keep · Σ_g keep(seed_g; row, col) ⊙ (du_g[M,r]·A_g[r,N]),  g < groups <= 3
@@ -82,8 +86,12 @@ struct LoraDxDesc {
   float inv_keep = 1.0f;
   const uint32_t* seed_ptr = nullptr;
   uint32_t seed_key[3] = {0, 0, 0};
+  int pair = -1;  // CTA pairs sharing the A / W tile: -1 = auto (gemm_pairs' rule), 0 = off, 1 = on when M has two tiles or more
 };
 void lora_dx(const LoraDxDesc& d, cudaStream_t stream);
+bool lora_dx_pairs(const LoraDxDesc& d);
+// the output leaves through shared memory and TMA stores unless a row is not a whole number of 16-byte chunks
+bool lora_dx_uses_tma_store(const LoraDxDesc& d);
 
 // Drop cached TMA descriptors (call when buffers are freed / reallocated).
 void gemm_clear_descriptor_cache();

@@ -11,6 +11,7 @@
 // Roles (384 threads, 1 CTA / SM, persistent over output tiles):
 //   warpgroup 0   TMA producer (warp 0, one elected lane issues)        smem ring: full[s] / empty[s]
 //   warpgroups 1-2 consumers: each issues the wgmma of its 64 rows of the 128-row tile and writes them out
+// Long reductions into wide outputs run as clusters of two CTAs that share each B tile (CtaPair, gemm_pairs).
 #include <cuda.h>
 
 #include <cstdlib>
@@ -51,6 +52,7 @@ struct KernelArgs {
   int tiles_per_group;  // N-tiles per output-column group (the last one of a group may be ragged)
   int split_k;  // >1: each output tile is computed by split_k CTAs over disjoint K ranges, combined with fp32 atomics
   int tma_store;  // bf16 output through shared memory and TMA stores (map_out); else stored from registers
+  int paired;     // clusters of 2 CTAs own M-tiles (2i, 2i + 1) of one N tile and multicast the B tile (CtaPair)
 };
 
 template <int BLOCK_N>
@@ -76,6 +78,55 @@ __device__ __forceinline__ void load_operand(const CUtensorMap* map, uint64_t* b
   } else {
 #pragma unroll
     for (int j = 0; j < BLOCK_MN / 64; ++j) tma_load_2d(map, bar, dst + j * 8192, mn0 + j * 64, k0, hint);  // box {64 (MN), 64 (K)}
+  }
+}
+
+// CTA pairs: a cluster of 2 CTAs computes M tiles 2u and 2u + 1 of one N tile over the same k range.  Each CTA loads its own
+// A tile and half of the B tile, which the TMA unit multicasts into the same stage of both CTAs, so each B tile crosses from
+// L2 once per pair instead of once per CTA.  A stage's full barrier still expects the whole stage; its empty barrier also
+// counts one arrival from each consumer warp of the peer, whose multicast writes into this CTA's stage.  When the last pair
+// has a second tile past M, that CTA still loads its half of B, computes on zero-filled A and stores nothing.  Unpaired, each
+// CTA is a work unit of its own and nothing below changes the single-CTA schedule.
+struct CtaPair {
+  int on;
+  uint32_t rank;  // in the cluster; 0 unpaired
+  __device__ __forceinline__ explicit CtaPair(int paired) : on(paired), rank(paired ? cluster_ctarank() : 0) {}
+  __device__ __forceinline__ int m_units(int num_m_tiles) const { return on ? (num_m_tiles + 1) / 2 : num_m_tiles; }
+  __device__ __forceinline__ int first_unit() const { return blockIdx.x >> on; }
+  __device__ __forceinline__ int unit_stride() const { return gridDim.x >> on; }
+  __device__ __forceinline__ int m_tile(int m_unit) const { return (m_unit << on) + rank; }
+  __device__ __forceinline__ uint32_t empty_arrivals() const { return on ? 256 + 8 : 256; }
+  // consumer release of a stage: every consumer thread arrives here; paired, lane 0 of each warp also arrives at the peer
+  __device__ __forceinline__ void release(uint64_t* bar) const {
+    mbar_arrive(bar);
+    if (on && lane_id() == 0) mbar_arrive_cluster(bar, rank ^ 1);
+  }
+  // after barrier init: the peer may multicast into this CTA or arrive on its barriers only once they are initialised
+  __device__ __forceinline__ void start() const {
+    if (on) cluster_sync();
+    else __syncthreads();
+  }
+  // before exit: no CTA leaves while its peer may still arrive on its barriers
+  __device__ __forceinline__ void finish() const {
+    if (on) cluster_sync();
+  }
+};
+
+// Loads of the B tile, which both CTAs of a pair share: unpaired the whole tile, paired this CTA's half (64-row or 64-wide MN
+// chunk; K-major maps of a pair have a box of BLOCK_MN / 2 rows), multicast to both CTAs.
+template <int BLOCK_MN, bool MN_MAJOR>
+__device__ __forceinline__ void load_shared_operand(const CtaPair& pair, const CUtensorMap* map, uint64_t* bar, uint8_t* dst, int mn0,
+                                                    int k0, uint64_t hint) {
+  if (!pair.on) {
+    load_operand<BLOCK_MN, MN_MAJOR>(map, bar, dst, mn0, k0, hint);
+    return;
+  }
+  const int ofs = pair.rank * (BLOCK_MN / 2);  // rows of 128 bytes either way
+  if constexpr (!MN_MAJOR) {
+    tma_load_2d_multicast(map, bar, dst + ofs * 128, k0, mn0 + ofs, 0x3, hint);
+  } else {
+#pragma unroll
+    for (int j = 0; j < BLOCK_MN / 128; ++j) tma_load_2d_multicast(map, bar, dst + ofs * 128 + j * 8192, mn0 + ofs + j * 64, k0, 0x3, hint);
   }
 }
 
@@ -116,6 +167,7 @@ struct MmaRing {
   const uint32_t smem0;
   uint64_t* const full_bar;
   uint64_t* const empty_bar;
+  const CtaPair pair;
   int stage = 0;
   uint32_t phase = 0;
   int held = -1;
@@ -129,7 +181,7 @@ struct MmaRing {
       mma(smem0 + stage * kStageBytes);
       wgmma_commit();
       wgmma_wait<1>();
-      if (held >= 0) mbar_arrive(&empty_bar[held]);
+      if (held >= 0) pair.release(&empty_bar[held]);
       held = stage;
       if (++stage == kStages) {
         stage = 0;
@@ -140,7 +192,7 @@ struct MmaRing {
   // wait for every issued batch, then release the last stage; the caller fences the accumulator before reading it
   __device__ __forceinline__ void drain() {
     wgmma_wait<0>();
-    if (held >= 0) mbar_arrive(&empty_bar[held]);
+    if (held >= 0) pair.release(&empty_bar[held]);
     held = -1;
   }
 };
@@ -159,6 +211,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
 
   const uint32_t warp = warp_id();
   const int wg = threadIdx.x / 128;
+  const CtaPair pair(p.paired);
   if (threadIdx.x == 0) {
     pdl_launch_dependents();
     tma_prefetch_desc(&map_a1);
@@ -170,15 +223,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     if (p.tma_store) tma_prefetch_desc(&map_out);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 256);  // every consumer thread releases the slot
+      mbar_init(&empty_bar[s], pair.empty_arrivals());  // every consumer thread releases the slot (+ the peer's warps)
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  pair.start();
   pdl_wait();  // everything above is CTA-local: it overlaps the tail of the previous kernel in the stream (PDL)
 
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-  const int num_work = num_tiles * p.split_k;
+  // work unit: (M unit, N tile, split); an M unit is one M tile, or a pair's two
+  const int num_work = pair.m_units(p.num_m_tiles) * p.num_n_tiles * p.split_k;
   const int kstep1 = p.fp8 ? 2 * BLOCK_K : BLOCK_K;  // elements per k-block of segment 1 (always 128 bytes per row)
   const int kb1 = (p.K1 + kstep1 - 1) / kstep1;
   const int kb2 = (p.K2 + BLOCK_K - 1) / BLOCK_K;
@@ -188,12 +241,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
   if (wg == 0) {
     // ===================================================================== TMA producer (whole warp walks the loop)
     setmaxnreg_dec<40>();
-    if (warp != 0) return;
     int stage = 0;
     uint32_t phase = 0;
-    for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+    for (int work = pair.first_unit(); warp == 0 && work < num_work; work += pair.unit_stride()) {
       const int tile = work / p.split_k, split = work % p.split_k;
-      const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+      const int mu = tile / p.num_n_tiles;
+      const int m0 = pair.m_tile(mu) * BLOCK_M;
       const int tn = tile % p.num_n_tiles;
       const int g = tn / p.tiles_per_group;
       const int nl = (tn % p.tiles_per_group) * BLOCK_N;  // column offset inside the group
@@ -201,7 +254,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
       const int a1_k = g * p.a1_group_kofs;
       const int a2_k = g * p.a2_group_kofs;
       const int b1_k = g * p.b1_group_kofs;
-      const int b1_n = (p.b1_local_n ? nl : n0) + (m0 / p.m_per_group) * p.b1_mn_ofs_per_mgroup;
+      // the M group of the unit's first tile: a pair never straddles M groups (m_per_group is a multiple of 2 tiles)
+      const int b1_n = (p.b1_local_n ? nl : n0) + (pair.m_tile(mu) - pair.rank) * BLOCK_M / p.m_per_group * p.b1_mn_ofs_per_mgroup;
       const int kb_begin = split * kb_per_split, kb_end = min(num_kb, kb_begin + kb_per_split);
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -211,11 +265,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
           mbar_arrive_expect_tx(&full_bar[stage], L::kStageBytes);
           if (kb < kb1) {
             load_operand<BLOCK_M, A_MN>(&map_a1, &full_bar[stage], sa, m0, a1_k + kb * kstep1, kEvictNormal);
-            load_operand<BLOCK_N, B_MN>(&map_b1, &full_bar[stage], sb, b1_n, b1_k + kb * kstep1, kEvictLast);
+            load_shared_operand<BLOCK_N, B_MN>(pair, &map_b1, &full_bar[stage], sb, b1_n, b1_k + kb * kstep1, kEvictLast);
           } else {
             const int k = (kb - kb1) * BLOCK_K;
             load_operand<BLOCK_M, false>(&map_a2, &full_bar[stage], sa, m0, a2_k + k, kEvictNormal);
-            load_operand<BLOCK_N, false>(&map_b2, &full_bar[stage], sb, n0, k, kEvictLast);
+            load_shared_operand<BLOCK_N, false>(pair, &map_b2, &full_bar[stage], sb, n0, k, kEvictLast);
           }
         }
         __syncwarp();
@@ -225,6 +279,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
         }
       }
     }
+    pair.finish();
     return;
   }
 
@@ -235,14 +290,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
   const float alpha_eff = p.alpha * (p.alpha_dev != nullptr ? *p.alpha_dev : 1.0f);
   const bool out_vec = (p.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 7) == 0);
   const bool res_vec = p.residual != nullptr && (p.ldr % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0);
-  MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar};
+  MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar, pair};
   const uint32_t a_ofs = cw * 8192;  // this warpgroup's 64 rows of the A tile (either major)
   const bool store_lead = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's TMA stores
   const uint32_t stage_u32 = smem0 + L::kTileBytes;  // store staging, 1024-byte aligned (128B swizzle)
+  const bool plain = p.bias == nullptr && p.residual == nullptr && !p.accumulate;
   float acc[BLOCK_N / 2];
-  for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+  for (int work = pair.first_unit(); work < num_work; work += pair.unit_stride()) {
     const int tile = work / p.split_k, split = work % p.split_k;
-    const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+    const int m0 = pair.m_tile(tile / p.num_n_tiles) * BLOCK_M;
     const int tn = tile % p.num_n_tiles;
     const int nl = (tn % p.tiles_per_group) * BLOCK_N;
     const int n0 = (tn / p.tiles_per_group) * p.n_per_group + nl;
@@ -264,23 +320,31 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     ring.run(kb_end - kb_mid, [&](uint32_t s) { mma_bf16_kblock<BLOCK_N, false, false>(acc, s + a_ofs, s + L::kABytes); });
     ring.drain();
     fence_regs(acc);
+    if (m0 >= p.M) continue;  // a pair's second tile past M
     if (BLOCK_N == 128 && p.tma_store) {
-      // ---- bf16 epilogue through shared memory: each 64-column sub-tile of the warpgroup's 64 rows is written to a
-      // staging buffer in the TMA box layout and stored by one thread; the store drains while the next tile's k-loop runs.
-      // Same fp32 operations in the same order as the register path below, one rounding.  A group's ragged last tile
-      // stores only the sub-tiles inside the group (group widths are multiples of 64); the TMA unit clips rows and columns
-      // past the tensor.
+      // ---- bf16 epilogue through shared memory: both 64-column sub-tiles of the warpgroup's 64 rows are written to staging
+      // buffers in the TMA box layout, then one proxy fence and one barrier, and one thread stores them; the stores drain
+      // while the next tile's k-loop runs.  Same fp32 operations in the same order as the register path below, one
+      // rounding.  A group's ragged last tile stores only the sub-tiles inside the group (group widths are multiples of 64);
+      // the TMA unit clips rows and columns past the tensor, so without bias, residual or accumulation (`plain`) no element
+      // needs a bounds check: that path is a multiply, a pack and a shared store per column pair, where the general one
+      // spends tens of instructions on uniform tests and bounds (about 3 us per tile at N 5120, K 768).
+      if (store_lead) bulk_wait_read<0>();  // the previous tile's stores, issued a whole k-loop ago, have read the staging
+      named_bar_sync(1 + cw, 128);
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 64; ++j) {
         if (n0 + j * 64 >= n_lim) break;
-        // buffer j % 2: wait until the store that last read it has done so (the previous tile's last store, issued a whole
-        // k-loop ago, or sub-tile j - 2)
-        if (store_lead) {
-          if (j == 0) bulk_wait_read<0>();
-          else bulk_wait_read<1>();
+        const uint32_t buf = stage_u32 + (cw * 2 + j) * 8192;
+        if (plain) {
+#pragma unroll
+          for (int q = 0; q < 32; q += 2) {
+            const int i = j * 32 + q;
+            const int r = frag_row(i);
+            st_shared_u32(buf + r * 128 + (((q >> 2) ^ (r & 7)) << 4) + (threadIdx.x & 3) * 4,
+                          pack_bf16x2(acc[i] * alpha_eff, acc[i + 1] * alpha_eff));
+          }
+          continue;
         }
-        named_bar_sync(1 + cw, 128);
-        const uint32_t buf = stage_u32 + (cw * 2 + (j & 1)) * 8192;
 #pragma unroll
         for (int q = 0; q < 32; q += 2) {
           const int i = j * 32 + q;
@@ -314,12 +378,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
           // 16-byte chunk (q / 4) of row r, XOR-swizzled by r % 8: conflict-free, and the layout the TMA unit reads
           st_shared_u32(buf + r * 128 + (((q >> 2) ^ (r & 7)) << 4) + (threadIdx.x & 3) * 4, pack_bf16x2(v0, v1));
         }
-        fence_proxy_async_smem();
-        named_bar_sync(1 + cw, 128);
-        if (store_lead) {
-          tma_store_2d(&map_out, buf, n0 + j * 64, m0 + cw * 64);
-          bulk_commit();
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1 + cw, 128);
+      if (store_lead) {
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 64; ++j) {
+          if (n0 + j * 64 >= n_lim) break;
+          tma_store_2d(&map_out, stage_u32 + (cw * 2 + j) * 8192, n0 + j * 64, m0 + cw * 64);
         }
+        bulk_commit();
       }
       continue;
     }
@@ -382,6 +450,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     }
   }
   if (store_lead && p.tma_store) bulk_wait_all();  // the staging buffers must outlive the stores that read them
+  pair.finish();
 }
 
 // =============================================================================================
@@ -407,21 +476,25 @@ struct LoraDxArgs {
   float inv_keep;
   const uint32_t* seed_ptr;
   uint32_t keys[3];
+  int paired;     // CTA pairs share the MN-major A / W tile (CtaPair)
+  int tma_store;  // output through shared memory and TMA stores (map_out); else stored from registers
 };
 
 __global__ void __launch_bounds__(kNumThreads, 1)
 lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_w,
-               const __grid_constant__ CUtensorMap map_du, const __grid_constant__ CUtensorMap map_a, const LoraDxArgs p) {
+               const __grid_constant__ CUtensorMap map_du, const __grid_constant__ CUtensorMap map_a,
+               const __grid_constant__ CUtensorMap map_out, const LoraDxArgs p) {
   constexpr int BLOCK_N = 128;
   using L = SmemLayout<BLOCK_N>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kTileBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kTileBytes + L::kStoreBytes);
   uint64_t* empty_bar = full_bar + kStages;
 
   const uint32_t warp = warp_id();
   const int wg = threadIdx.x / 128;
+  const CtaPair pair(p.paired);
   if (threadIdx.x == 0) {
     pdl_launch_dependents();
     tma_prefetch_desc(&map_du);
@@ -430,28 +503,28 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
       tma_prefetch_desc(&map_dy);
       tma_prefetch_desc(&map_w);
     }
+    if (p.tma_store) tma_prefetch_desc(&map_out);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 256);
+      mbar_init(&empty_bar[s], pair.empty_arrivals());
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  pair.start();
   pdl_wait();
 
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+  const int num_work = pair.m_units(p.num_m_tiles) * p.num_n_tiles;
   const int kb_lora = p.r / BLOCK_K;  // r is a multiple of 64
   const int kb_base = (p.Kb + BLOCK_K - 1) / BLOCK_K;
 
   if (wg == 0) {
     // ===================================================================== TMA producer
     setmaxnreg_dec<40>();
-    if (warp != 0) return;
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-      const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
+    for (int work = pair.first_unit(); warp == 0 && work < num_work; work += pair.unit_stride()) {
+      const int m0 = pair.m_tile(work / p.num_n_tiles) * BLOCK_M;
+      const int n0 = (work % p.num_n_tiles) * BLOCK_N;
       for (int kb = 0; kb < p.G * kb_lora + kb_base; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         if (elect_one()) {
@@ -459,11 +532,11 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
           mbar_arrive_expect_tx(&full_bar[stage], L::kStageBytes);
           if (kb < p.G * kb_lora) {  // du [M, G·r] K-major ; A [G·r, N] MN-major
             load_operand<BLOCK_M, false>(&map_du, &full_bar[stage], sa, m0, kb * BLOCK_K, kEvictNormal);
-            load_operand<BLOCK_N, true>(&map_a, &full_bar[stage], sa + L::kABytes, n0, kb * BLOCK_K, kEvictLast);
+            load_shared_operand<BLOCK_N, true>(pair, &map_a, &full_bar[stage], sa + L::kABytes, n0, kb * BLOCK_K, kEvictLast);
           } else {                   // dy [M, Kb] K-major ; W [Kb, N] MN-major
             const int k = (kb - p.G * kb_lora) * BLOCK_K;
             load_operand<BLOCK_M, false>(&map_dy, &full_bar[stage], sa, m0, k, kEvictNormal);
-            load_operand<BLOCK_N, true>(&map_w, &full_bar[stage], sa + L::kABytes, n0, k, kEvictLast);
+            load_shared_operand<BLOCK_N, true>(pair, &map_w, &full_bar[stage], sa + L::kABytes, n0, k, kEvictLast);
           }
         }
         __syncwarp();
@@ -473,6 +546,7 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
         }
       }
     }
+    pair.finish();
     return;
   }
 
@@ -480,10 +554,9 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
   const int cw = wg - 1;
   const uint32_t smem0 = smem_u32(smem);
   const uint32_t seed0 = p.seed_ptr ? *p.seed_ptr : 0u;
-  uint32_t seeds[3];
-#pragma unroll
-  for (int g = 0; g < 3; ++g) seeds[g] = mix_seed(seed0, p.keys[g]);
-  MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar};
+  MmaRing<kStages, L::kStageBytes> ring{smem0, full_bar, empty_bar, pair};
+  const bool store_lead = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's TMA stores
+  const uint32_t stage_u32 = smem0 + L::kTileBytes;  // store staging, 1024-byte aligned (128B swizzle)
   // n k-blocks into acc with one batch in flight, drained before the caller reads acc
   auto mma_blocks = [&](float (&acc)[BLOCK_N / 2], int n) {
     fence_regs(acc);
@@ -492,19 +565,20 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
     fence_regs(acc);
   };
   float acc[BLOCK_N / 2], cmb[BLOCK_N / 2];
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int m0 = (tile / p.num_n_tiles) * BLOCK_M + cw * 64;
-    const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
+  for (int work = pair.first_unit(); work < num_work; work += pair.unit_stride()) {
+    const int m0 = pair.m_tile(work / p.num_n_tiles) * BLOCK_M + cw * 64;
+    const int n0 = (work % p.num_n_tiles) * BLOCK_N;
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) cmb[i] = 0.f;
     for (int g = 0; g < p.G; ++g) {
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
       mma_blocks(acc, kb_lora);
+      const uint32_t seed = mix_seed(seed0, g == 0 ? p.keys[0] : g == 1 ? p.keys[1] : p.keys[2]);
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; i += 2) {  // one hash per column pair (common.cuh:keep_drop)
         const uint32_t row = m0 + frag_row(i), col = n0 + frag_col(i);
-        const uint32_t hsh = lowbias32((row * 0x9E3779B1u) ^ seeds[g] ^ ((col >> 1) * 0x85EBCA77u));
+        const uint32_t hsh = lowbias32((row * 0x9E3779B1u) ^ seed ^ ((col >> 1) * 0x85EBCA77u));
         if ((hsh & 0xFFFFu) >= p.thr16) cmb[i] += acc[i];
         if ((hsh >> 16) >= p.thr16) cmb[i + 1] += acc[i + 1];
       }
@@ -512,10 +586,46 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = cmb[i] * p.inv_keep;
     if (kb_base > 0) mma_blocks(acc, kb_base);  // the frozen-path product accumulates on top of the combined LoRA term
+    if (m0 >= p.M) continue;  // rows past M: a ragged last tile's second warpgroup, or a pair's second tile past M
+    if (p.tma_store) {
+      // ---- through shared memory, as gemm_kernel's bf16 epilogue: each 64-column sub-tile of the warpgroup's 64 rows is
+      // written to a staging buffer in the TMA box layout and stored by one thread, draining while the next tile's k-loop
+      // runs.  The TMA unit clips rows past M and columns past N.
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 64; ++j) {
+        if (n0 + j * 64 >= p.N) break;
+        if (store_lead) {
+          if (j == 0) bulk_wait_read<0>();
+          else bulk_wait_read<1>();
+        }
+        named_bar_sync(1 + cw, 128);
+        const uint32_t buf = stage_u32 + (cw * 2 + j) * 8192;
+#pragma unroll
+        for (int q = 0; q < 32; q += 2) {
+          const int i = j * 32 + q;
+          const int r = frag_row(i);
+          const int row = m0 + r, col = n0 + frag_col(i);
+          float v0 = acc[i], v1 = acc[i + 1];
+          if (kb_base == 0 && row < p.M && col < p.N) {
+            const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.base + (long long)row * p.ld_base + col));
+            v0 += b.x;
+            v1 += b.y;
+          }
+          st_shared_u32(buf + r * 128 + (((q >> 2) ^ (r & 7)) << 4) + (threadIdx.x & 3) * 4, pack_bf16x2(v0, v1));
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(1 + cw, 128);
+        if (store_lead) {
+          tma_store_2d(&map_out, buf, n0 + j * 64, m0);
+          bulk_commit();
+        }
+      }
+      continue;
+    }
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; i += 2) {
       const int row = m0 + frag_row(i), col = n0 + frag_col(i);
-      if (row >= p.M || col >= p.N) continue;  // N is a multiple of 8: column pairs are whole
+      if (row >= p.M || col >= p.N) continue;  // N is a multiple of 2: column pairs are whole
       float v0 = acc[i], v1 = acc[i + 1];
       if (kb_base == 0) {
         const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.base + (long long)row * p.ld_base + col));
@@ -525,6 +635,8 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
       *reinterpret_cast<uint32_t*>(p.out + (long long)row * p.ldc + col) = pack_bf16x2(v0, v1);
     }
   }
+  if (store_lead && p.tma_store) bulk_wait_all();  // the staging buffers must outlive the stores that read them
+  pair.finish();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -688,19 +800,22 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   const long long b1_mn_total = (d.b1_local_n ? (long long)p.n_per_group : (long long)d.N) + (long long)(mgroups - 1) * d.b1_mn_ofs_per_mgroup;
   const long long b1_k_total = (long long)d.K1 + (long long)(groups - 1) * d.b1_group_kofs;
   if (d.m_per_group > 0 && (d.m_per_group % BLOCK_M) != 0) throw std::runtime_error("gemm: m_per_group must be a multiple of the M tile");
-  CUtensorMap mb1 = operand_map(d.b1, b1_mn_total, b1_k_total, BLOCK_N, d.fp8);
+  const bool paired = gemm_pairs(d, BLOCK_N);
+  p.paired = paired ? 1 : 0;
+  const int b_box = paired ? BLOCK_N / 2 : BLOCK_N;  // each CTA of a pair loads half of the B tile
+  CUtensorMap mb1 = operand_map(d.b1, b1_mn_total, b1_k_total, b_box, d.fp8);
   CUtensorMap ma2 = ma1, mb2 = mb1;
   if (d.K2 > 0) {
     if (d.a2.mn_major || d.b2.mn_major) throw std::runtime_error("gemm: the LoRA (A2/B2) operands must be K-major");
     const long long a2_k_total = (long long)d.K2 + (long long)(groups - 1) * d.a2_group_kofs;
     ma2 = operand_map(d.a2, d.M, a2_k_total, BLOCK_M);
-    mb2 = operand_map(d.b2, d.N, d.K2, BLOCK_N);
+    mb2 = operand_map(d.b2, d.N, d.K2, b_box);
   }
   auto kern = gemm_kernel<BLOCK_N, A_MN, B_MN>;
-  static bool configured = false;
-  if (!configured) {
+  static int max_pairs = 0;  // clusters of 2 resident at once
+  if (max_pairs == 0) {
     check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal), "cudaFuncSetAttribute(gemm)");
-    configured = true;
+    max_pairs = max_active_clusters(kern, 2, kNumThreads, L::kTotal);
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int num_kb = ceil_div(d.K1, d.fp8 ? 2 * BLOCK_K : BLOCK_K) + ceil_div(d.K2, BLOCK_K);
@@ -716,10 +831,11 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   p.split_k = split;
   p.tma_store = gemm_uses_tma_store(d, BLOCK_N, split) ? 1 : 0;
   const CUtensorMap mout = p.tma_store ? make_map_2d(d.out, d.N, d.M, d.ldc, 64, 64) : ma1;
-  const int work = tiles * split;
-  const int grid = work < num_sms() ? work : num_sms();
+  const int cta_per_unit = paired ? 2 : 1;
+  const int work = ceil_div(p.num_m_tiles, cta_per_unit) * p.num_n_tiles * split;
+  const int grid = std::min(work, paired ? max_pairs : num_sms()) * cta_per_unit;
   if (grid <= 0) return;
-  launch_k(kern, grid, kNumThreads, L::kTotal, stream, ma1, mb1, ma2, mb2, mout, p);
+  launch_k_cluster(cta_per_unit, kern, grid, kNumThreads, L::kTotal, stream, ma1, mb1, ma2, mb2, mout, p);
   RB_CHECK_LAUNCH("gemm_kernel");
 }
 
@@ -743,12 +859,37 @@ int gemm_block_n(const GemmDesc& d) { return d.block_n == 256 ? 256 : 128; }
 
 int gemm_smem_bytes(int block_n) { return block_n == 256 ? SmemLayout<256>::kTotal : SmemLayout<128>::kTotal; }
 
+// CTA pairs (CtaPair): the 128-wide tile only, M of at least two tiles, and M groups (weight gradients) that hold whole
+// pairs, since a pair shares one B tile.  Auto (pair = -1) pairs long reductions into wide outputs: N >= 2048 and at least
+// 32 k-blocks.  Measured on an H100 80GB HBM3 at 700 W (bench/gemm_bench.py, bench/gemm_ksweep.py, M 12288): pairs cut the
+// per-k-block slope at N 5120 from 14.7 to 11.9 us (cuBLAS 10.1) and ran 2 - 6 % faster on every llama_1b projection
+// (K 2048 - 11008) and 14 % faster at 8192^3; at K 768 (N 2304, 5120) they tied, and at N 768 they ran 7 - 14 % slower
+// (o / down of llama_250m and its N 768, K 5120 input gradient), where B is small enough to stay in L2.
+bool gemm_pairs(const GemmDesc& d, int block_n) {
+  if (d.pair == 0 || block_n != 128 || ceil_div(d.M, BLOCK_M) < 2) return false;
+  if (d.m_per_group > 0 && d.m_per_group % (2 * BLOCK_M) != 0) return false;
+  const int num_kb = ceil_div(d.K1, d.fp8 ? 2 * BLOCK_K : BLOCK_K) + ceil_div(d.K2, BLOCK_K);
+  return d.pair == 1 || (d.N >= 2048 && num_kb >= 32);
+}
+
 void gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
   if (d.n_lora_acc != 0) throw std::runtime_error("gemm: dropout-combine epilogue not built into this kernel variant");
   if (d.M <= 0 || d.N <= 0) return;
   if (gemm_block_n(d) == 256) dispatch_major<256>(d, stream);
   else dispatch_major<128>(d, stream);
 }
+
+// Pairs share the A / W tile (MN-major, 64-wide chunks); every call form of this kernel can pair.  Auto: the GEMM's rule
+// (bench/lora_dx_bench.py, same card: pairs 15 % faster on llama_1b down (N 5504) and 3 % on o (N 2048), 7 - 13 % slower
+// at N 768).
+bool lora_dx_pairs(const LoraDxDesc& d) {
+  if (d.pair == 0 || ceil_div(d.M, BLOCK_M) < 2) return false;
+  const int num_kb = d.groups * d.r / BLOCK_K + ceil_div(d.Kb, BLOCK_K);
+  return d.pair == 1 || (d.N >= 2048 && num_kb >= 32);
+}
+// the base, pitch and alignment rules below hold for every call; only a ragged last 16-byte chunk of a row keeps the
+// register epilogue (a TMA store would write past column N)
+bool lora_dx_uses_tma_store(const LoraDxDesc& d) { return d.N % 8 == 0; }
 
 void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
   if (d.M <= 0 || d.N <= 0) return;
@@ -774,14 +915,18 @@ void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
     m_dy = make_map_2d(d.dy, d.Kb, d.M, d.ld_dy, BLOCK_K, BLOCK_M);
     m_w = make_map_2d(d.w, d.N, d.Kb, d.ld_w, 64, BLOCK_K);
   }
-  static bool configured = false;
-  if (!configured) {
-    check(cudaFuncSetAttribute(lora_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kRingTotal), "cudaFuncSetAttribute(lora_dx)");
-    configured = true;
+  p.paired = lora_dx_pairs(d) ? 1 : 0;
+  p.tma_store = lora_dx_uses_tma_store(d) ? 1 : 0;
+  const CUtensorMap m_out = p.tma_store ? make_map_2d(d.out, d.N, d.M, d.ldc, 64, 64) : m_du;
+  static int max_pairs = 0;  // clusters of 2 resident at once
+  if (max_pairs == 0) {
+    check(cudaFuncSetAttribute(lora_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal), "cudaFuncSetAttribute(lora_dx)");
+    max_pairs = max_active_clusters(lora_dx_kernel, 2, kNumThreads, L::kTotal);
   }
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  launch_k(lora_dx_kernel, grid, kNumThreads, L::kRingTotal, stream, m_dy, m_w, m_du, m_a, p);
+  const int cta_per_unit = p.paired ? 2 : 1;
+  const int work = ceil_div(p.num_m_tiles, cta_per_unit) * p.num_n_tiles;
+  const int grid = std::min(work, p.paired ? max_pairs : num_sms()) * cta_per_unit;
+  launch_k_cluster(cta_per_unit, lora_dx_kernel, grid, kNumThreads, L::kTotal, stream, m_dy, m_w, m_du, m_a, m_out, p);
   RB_CHECK_LAUNCH("lora_dx_kernel");
 }
 

@@ -91,6 +91,30 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// thread-block clusters
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster: arrive (release) and wait (acquire)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset as `bar` in CTA `cta` of the cluster (this CTA included).  Default
+// (.release.cta) semantics: a .cluster release puts a MEMBAR.ALL.GPU before the arrive, which stalls the issuing warp on
+// every k-block; the arrive only reports that this CTA's wgmma reads of a stage, retired by wgmma.wait_group, are done.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------
 // TMA
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -108,6 +132,18 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       " [%0], [%1, {%3, %4}], [%2], %5;"
       :
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
+      : "memory");
+}
+// Same box written to the same shared-memory offset of every CTA in `cta_mask`; each destination's mbarrier at the offset
+// of `bar` receives the bytes as complete_tx.
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int c0, int c1,
+                                                      uint16_t cta_mask, uint64_t hint = kEvictNormal) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask),
+        "l"(hint)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int c0, int c1, int c2,

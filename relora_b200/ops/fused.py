@@ -91,7 +91,8 @@ def gemm(
 ) -> torch.Tensor:
     """``out[M,N] = alpha·(a1·b1ᵀ + a2·b2ᵀ) (+ residual) (+ out)`` on the wgmma kernel.
 
-    ``pair``: accepted and ignored (sm_90 has no CTA-pair MMA; tiles are always single-CTA).
+    ``pair``: CTA pairs, two M tiles of one N tile sharing each B tile through TMA multicast: -1 lets the dispatcher
+    choose (``gemm_pairs``), 0 turns them off, 1 asks for them where the call form allows (the 256-wide tile does not).
     ``fp8``: 1 = ``a1`` / ``b1`` hold E4M3 bytes (K-major), 2 = ``a1`` is E5M2 (gradients); ``alpha_dev``: fp32 device scalar multiplied into ``alpha``.
 
     K-major operands are ``[rows, K]`` row-major; with ``a1_mn`` / ``b1_mn`` the tensor is
