@@ -314,7 +314,11 @@ void rope_inplace(Tensor& buf, int64_t T, int64_t n_rot_heads, int64_t hd, int64
   chk_bf16(buf, "buf"); chk_bf16(cos, "cos"); chk_bf16(sin, "sin");
   chk_2d_rowmajor(buf, "buf");
   TORCH_CHECK(cos.is_contiguous() && sin.is_contiguous() && cos.size(-1) == rotary_dim, "cos/sin must be [n_pos, rotary_dim]");
-  TORCH_CHECK(T + pos0 <= cos.size(0), "rotary table too short");
+  TORCH_CHECK(sin.sizes() == cos.sizes() && T + pos0 <= cos.size(0), "rotary table too short");
+  TORCH_CHECK(rotary_dim > 0 && rotary_dim <= hd && n_rot_heads * hd <= buf.size(1), "rope: rotary_dim <= hd and n_rot_heads * hd <= width");
+  // the scalar kernel (taken when the 16-byte one cannot run) moves element pairs with 4-byte accesses
+  for (const Tensor* t : std::initializer_list<const Tensor*>{&buf, &cos, &sin})
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 3) == 0, "rope: buf, cos and sin must be 4-byte aligned");
   c10::cuda::CUDAGuard guard(buf.device());
   rb::rope_inplace(buf.data_ptr(), buf.stride(0), (int)buf.size(0), (int)T, (int)n_rot_heads, (int)hd, (int)rotary_dim, cos.data_ptr(),
                    sin.data_ptr(), backward, (int)pos0, cur_stream());
@@ -332,7 +336,13 @@ void rope_pack_bwd(const Tensor& dq, const Tensor& dk, const Tensor& dv, Tensor&
   TORCH_CHECK(dk.strides() == dv.strides() && dk.stride(3) == 1, "dk/dv must share strides");
   TORCH_CHECK(nkv != nh || dq.strides() == dk.strides(), "dq/dk/dv must share strides");
   TORCH_CHECK(out.size(0) == (int64_t)B * T && out.size(1) == (nh + 2 * nkv) * hd, "out must be [B*T, (nh+2*nkv)*hd]");
-  for (const Tensor* t : {&dq, &dk, &dv}) TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, "16-byte alignment required");
+  chk_bf16(cos, "cos"); chk_bf16(sin, "sin");
+  TORCH_CHECK(cos.is_contiguous() && sin.is_contiguous() && cos.dim() == 2 && cos.size(1) == rotary_dim && sin.sizes() == cos.sizes(),
+              "rope_pack_bwd: cos/sin must be [n_pos, rotary_dim]");
+  TORCH_CHECK(rotary_dim > 0 && rotary_dim <= hd, "rope_pack_bwd: rotary_dim must be in (0, hd]");
+  TORCH_CHECK(T + pos0 <= cos.size(0), "rope_pack_bwd: rotary table too short for T + pos0");
+  for (const Tensor* t : std::initializer_list<const Tensor*>{&dq, &dk, &dv, &out, &cos, &sin})
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, "rope_pack_bwd: 16-byte aligned operands required");
   c10::cuda::CUDAGuard guard(out.device());
   rb::rope_pack_bwd(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), dq.stride(0), dq.stride(1), dq.stride(2), dk.stride(0), dk.stride(1), dk.stride(2),
                     out.data_ptr(), out.stride(0), B, T, nh, (int)nkv, hd, (int)rotary_dim, cos.data_ptr(), sin.data_ptr(), (int)pos0, cur_stream());

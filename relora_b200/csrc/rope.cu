@@ -50,7 +50,9 @@ __global__ void __launch_bounds__(256) rope_vec_kernel(bf16* __restrict__ buf, l
 bool rope_inplace_vec(void* buf, long long ld, int M, int T, int n_rot_heads, int hd, int rotary_dim, const void* cos, const void* sin,
                       bool backward, int pos0, cudaStream_t s) {
   const int half = rotary_dim / 2;
-  if (half % 8 != 0 || hd % 8 != 0 || ld % 8 != 0 || (reinterpret_cast<uintptr_t>(buf) & 15) != 0) return false;
+  if (half % 8 != 0 || hd % 8 != 0 || ld % 8 != 0 || ((reinterpret_cast<uintptr_t>(buf) | reinterpret_cast<uintptr_t>(cos) |
+                                                         reinterpret_cast<uintptr_t>(sin)) & 15) != 0)
+    return false;
   const long long total = (long long)M * n_rot_heads * (half / 8);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 16);
   launch_k(rope_vec_kernel, grid, 256, 0, s, (bf16*)buf, ld, total, T, n_rot_heads, hd, half, (const bf16*)cos, (const bf16*)sin,

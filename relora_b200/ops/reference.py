@@ -8,6 +8,7 @@ from __future__ import annotations
 import math
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -531,6 +532,509 @@ def assert_attention_close(name: str, got: torch.Tensor, ref: torch.Tensor, boun
             f"got={float(g[idx]):.6g} ref={float(ref[idx]):.6g} tol={float(tol[idx]):.6g} (bound={float(bound[idx]):.6g}, "
             f"score={float(score[idx]):.6g}, floor={float(floor[idx]):.3g})")
     return worst
+
+
+# ----------------------------------------------------------------------------- row-wise kernels (csrc/kernels.h)
+# fp64 evaluations of the contracts of the norm, rotary, activation, loss, embedding, dropout, fp8 and optimizer kernels, written
+# from their documentation.  Each takes the kernel's inputs as stored (and, where a later output is defined in terms of an earlier
+# one, the earlier output as the kernel stored it, like O' in attention_ref) and returns, per output, either ``(ref, bound)`` for
+# assert_rowwise_close or an exact tensor for assert_bitwise_equal.  ``bound`` already carries its coefficient: it is the
+# absolute error allowed beyond the rounding of the output itself.
+#
+# Intermediate roundings are part of the definitions and are reproduced, not absorbed: the bf16 x̂ of RMSNorm (forward and dw),
+# the rounded dz that GELU's dbias sums, the rounded activation that the dropout and E4M3 copies are made from.  Only two
+# constants are empirical.  ROW_C_ACC is the fp32 accumulation error of a sum per unit of Σ|terms| (row statistics, dw / db /
+# dres_sum / dtable / dbias / sumsq / loss_sum), ROW_C_F32 the error of a few fp32 operations and of rsqrtf, __expf,
+# __fdividef, erff, tanhf and powf per unit of the element's magnitude term.  Both are set from the worst element observed
+# on an H100 80GB HBM3 (700 W) over tests/test_rowwise_modes_gpu.py (sweep and executor audit; its "calibration" lines with -s
+# print each family's share of the coefficient), with headroom: sums reached 2.2e-7·Σ|terms| (share 0.229 of 2^-20, RMSNorm dw at
+# M = 1500, H = 8192; LayerNorm dw 0.222) and element-wise fp32 results 9.2e-7 per unit of their magnitude term (share 0.242 of
+# 2^-18, LayerNorm rstd at H = 4096 with a mean offset of 64; tanh-GELU dz 0.142).
+ROW_C_ACC = 2.0 ** -20
+ROW_C_F32 = 2.0 ** -18
+# fp32 results below the normal range may be flushed (ex2.approx.ftz inside __expf, __fdividef past 2^126): at most this much
+ROW_FTZ = 2.0 ** -126
+_BF16_OUT = 2.0 ** -8  # relative rounding of a bf16 output (round to nearest, 8 significant bits)
+_F32_OUT = 2.0 ** -24
+
+
+def _f32(t: torch.Tensor) -> torch.Tensor:
+    return t.to(torch.float32)
+
+
+def _bf16_round(t: torch.Tensor) -> torch.Tensor:
+    """fp32 -> bf16 -> fp32 with round-to-nearest-even (__float2bfloat16_rn)."""
+    return t.to(torch.float32).to(torch.bfloat16).to(torch.float32)
+
+
+def _seed_of(seed) -> int:
+    if seed is None:
+        return 0
+    return (int(seed.reshape(-1)[0].item()) if torch.is_tensor(seed) else int(seed)) & _M32
+
+
+def _keep_f32(p: float) -> float:
+    """The fp32 ``1/(1-p)`` the bindings pass to the kernels."""
+    return float(torch.tensor(1.0 / (1.0 - p), dtype=torch.float32))
+
+
+def dropout_copy_exact(y: torch.Tensor, seed, key: int, p: float, row_offset: int = 0) -> torch.Tensor:
+    """bf16 ``keep ⊙ y · fp32(1/(1-p))`` of a ``[M, H]`` bf16 tensor, mask stream ``mix_seed(seed, key)`` over (row, column),
+    product and rounding in fp32 as the kernels do it: the exact expected dropout copy."""
+    keep = dropout_keep_mask(mix_seed(_seed_of(seed), key), y.shape[0], y.shape[1], p, device=y.device, row_offset=row_offset)
+    return torch.where(keep, _f32(y) * _keep_f32(p), torch.zeros((), device=y.device)).to(torch.bfloat16)
+
+
+def fp8_saturate(x32: torch.Tensor, e5m2: bool = False) -> torch.Tensor:
+    """Saturating round-to-nearest-even of fp32 values to E4M3 (or E5M2), as ``uint8`` bits (``__NV_SATFINITE``)."""
+    fmax = 57344.0 if e5m2 else 448.0
+    return x32.clamp(-fmax, fmax).to(torch.float8_e5m2 if e5m2 else torch.float8_e4m3fn).view(torch.uint8)
+
+
+def fp8_copy_exact(y: torch.Tensor, inv_scale: torch.Tensor, amax_before: torch.Tensor, e5m2: bool = False):
+    """``(q8, amax)`` of a producer's E4M3 side output from its bf16 primary output ``y``: q8 = sat(fp32(y · inv_scale)),
+    amax = max(amax_before, max |y|)."""
+    inv = _f32(inv_scale.reshape(-1)[:1]).to(y.device)
+    q = fp8_saturate(_f32(y) * inv, e5m2)
+    amax = torch.maximum(_f32(amax_before).reshape(-1)[:1].to(y.device), _f32(y).abs().max().reshape(1))
+    return q, amax
+
+
+def rmsnorm_fwd_ref(x: torch.Tensor, w: torch.Tensor, eps: float, rstd_got: torch.Tensor) -> dict:
+    """Contract of ``rmsnorm_fwd(x, w, y, rstd, eps, ...)`` on ``x [M, H]``:
+
+        rstd = 1 / sqrt(Σ_j x_j² / H + eps)        (fp32 sum, rsqrtf)          -> ("rstd": ref, bound)
+        y    = bf16(w · bf16(fp32(x · rstd)))      with the stored fp32 rstd    -> ("y": exact)
+
+    The inner product x·rstd is one fp32 multiplication and w · bf16(..) is exact in fp32, so given the rstd the kernel stored,
+    y has one correct value.  The dropout copies and the E4M3 copy are derived from the stored y (dropout_copy_exact,
+    fp8_copy_exact)."""
+    X = x.to(_F64)
+    r = 1.0 / torch.sqrt((X * X).mean(-1) + eps)
+    rs = _f32(rstd_got).reshape(-1, 1)
+    xh = _bf16_round(_f32(x) * rs)
+    y = (xh * _f32(w).reshape(1, -1)).to(torch.bfloat16)
+    return {"rstd": (r, ROW_C_F32 * r), "y": y}
+
+
+def rmsnorm_bwd_ref(dy, x, w, rstd, dx_add=None, dw_before=None) -> dict:
+    """Contract of ``rmsnorm_bwd(dy, x, w, rstd, dx_add, dx, dw)`` with the stored fp32 ``rstd`` (one per row):
+
+        x̂ = x · rstd,   g = dy · w
+        dx = rstd · (g − x̂ · Σ_j g_j x̂_j / H) + dx_add                         (fp32, one bf16 rounding)
+        dw = dw_before + Σ_rows dy · bf16(fp32(x · rstd))                        (fp32 accumulation)
+
+    The bf16 x̂ inside dw is the one the forward multiplied the weight with; it is reproduced exactly."""
+    rs = _f32(rstd).reshape(-1, 1)
+    X, DY, W, RS = x.to(_F64), dy.to(_F64), w.to(_F64).reshape(1, -1), rs.to(_F64)
+    H = X.shape[1]
+    xh = X * RS
+    g = DY * W
+    dot = (g * xh).sum(-1, keepdim=True) / H
+    adot = (g * xh).abs().sum(-1, keepdim=True) / H
+    dx = RS * (g - xh * dot)
+    bdx = RS * (g.abs() + xh.abs() * adot)
+    if dx_add is not None:
+        dx = dx + dx_add.to(_F64)
+        bdx = bdx + dx_add.to(_F64).abs()
+    xhb = _bf16_round(_f32(x) * rs).to(_F64)
+    t = DY * xhb
+    dw0 = torch.zeros(H, dtype=_F64, device=x.device) if dw_before is None else dw_before.to(_F64)
+    return {"dx": (dx, ROW_C_F32 * bdx), "dw": (dw0 + t.sum(0), ROW_C_ACC * (dw0.abs() + t.abs().sum(0)))}
+
+
+def layernorm_fwd_ref(x, eps: float, mean_got, rstd_got, norms) -> dict:
+    """Contract of ``layernorm_fwd(x, w, b, y, mean, rstd, eps, w2, b2, y2, ...)`` on ``x [M, H]``:
+
+        mean = Σ x / H                                  (fp32)                   -> ("mean": ref, bound)
+        rstd = 1 / sqrt(Σ (x − mean)² / H + eps)        two-pass, the stored mean -> ("rstd": ref, bound)
+        y_n  = (x − mean) · rstd · w_n + b_n            stored mean / rstd, fp32, one bf16 rounding -> ("y0", "y1")
+
+    ``norms``: list of ``(w, b or None)``.  The dropout copies are derived from the stored y (dropout_copy_exact)."""
+    X = x.to(_F64)
+    H = X.shape[1]
+    mu = X.mean(-1)
+    m_got = _f32(mean_got).to(_F64).reshape(-1, 1)
+    var = ((X - m_got) ** 2).mean(-1)
+    r = 1.0 / torch.sqrt(var + eps)
+    res = {"mean": (mu, ROW_C_F32 * X.abs().mean(-1)), "rstd": (r, ROW_C_F32 * r)}
+    rs = _f32(rstd_got).to(_F64).reshape(-1, 1)
+    for n, (w, b) in enumerate(norms):
+        W = w.to(_F64).reshape(1, -1)
+        B = b.to(_F64).reshape(1, -1) if b is not None else torch.zeros(1, H, dtype=_F64, device=x.device)
+        xh = (X - m_got) * rs
+        res[f"y{n}"] = (xh * W + B, ROW_C_F32 * ((xh * W).abs() + B.abs()))
+    return res
+
+
+def layernorm_bwd_ref(x, mean, rstd, norms, dres=None, dres_sums=()) -> dict:
+    """Contract of ``layernorm_bwd`` with the stored fp32 ``mean`` / ``rstd``; ``norms``: list of ``(dy, w, dw_before,
+    db_before or None)`` (one, or two for the dual form):
+
+        x̂ = (x − mean) · rstd,   g_n = dy_n · w_n
+        dx  = dres + Σ_n rstd · (g_n − Σ_j g_n,j / H − x̂ · Σ_j g_n,j x̂_j / H)      (fp32, one bf16 rounding)
+        dw_n = dw_before + Σ_rows dy_n · x̂      db_n = db_before + Σ_rows dy_n
+        dres_sum_k = before_k + Σ_rows dres  for each ``before_k`` in ``dres_sums``"""
+    X = x.to(_F64)
+    H = X.shape[1]
+    xh = (X - _f32(mean).to(_F64).reshape(-1, 1)) * _f32(rstd).to(_F64).reshape(-1, 1)
+    RS = _f32(rstd).to(_F64).reshape(-1, 1)
+    dx = torch.zeros_like(X) if dres is None else dres.to(_F64)
+    bdx = torch.zeros_like(X) if dres is None else dres.to(_F64).abs()
+    res = {}
+    for n, (dy, w, dw0, db0) in enumerate(norms):
+        DY = dy.to(_F64)
+        g = DY * w.to(_F64).reshape(1, -1)
+        sg, sgx = g.sum(-1, keepdim=True) / H, (g * xh).sum(-1, keepdim=True) / H
+        dx = dx + RS * (g - sg - xh * sgx)
+        bdx = bdx + RS * (g.abs() + g.abs().sum(-1, keepdim=True) / H + xh.abs() * (g * xh).abs().sum(-1, keepdim=True) / H)
+        for name, before, t in ((f"dw{n}", dw0, DY * xh), (f"db{n}", db0, DY)):
+            if before is not None:
+                b0 = before.to(_F64)
+                res[name] = (b0 + t.sum(0), ROW_C_ACC * (b0.abs() + t.abs().sum(0)))
+    res["dx"] = (dx, ROW_C_F32 * bdx)
+    for k, before in enumerate(dres_sums):
+        b0, D = before.to(_F64), dres.to(_F64)
+        res[f"dres_sum{k}"] = (b0 + D.sum(0), ROW_C_ACC * (b0.abs() + D.abs().sum(0)))
+    return res
+
+
+def cross_entropy_ref(logits: torch.Tensor, labels: torch.Tensor, V: int, grad_scale: float, ignore_index: int,
+                      loss_before, count_before) -> dict:
+    """Contract of ``cross_entropy_fwd_bwd(logits, labels, V, grad_scale, ignore_index, loss_sum, count)`` on the bf16
+    ``logits[:, :V]`` as stored (row pitch ≥ V; the columns [V, ld) are neither read nor written):
+
+        row with label y ≠ ignore_index:  lse = log Σ_j exp(x_j),  loss_sum += lse − x_y,  count += 1
+                                          x_j <- bf16(grad_scale · (softmax_j − [j = y]))
+        ignored row:                      x_j <- 0 exactly
+
+    Bounds with m the row maximum and ρ_j = 1 + |x_j − m| (__expf's argument is rounded relative to its size): the gradient
+    ROW_C_F32·|gs|·p_j·(ρ_j + Σ_k p_k ρ_k) + |gs|·ROW_FTZ, the loss ROW_C_F32·(|lse| + |m| + |x_y| + Σ_k p_k ρ_k) per row plus
+    ROW_C_ACC over the rows' sum.  ``count`` is exact."""
+    X = logits[:, :V].to(_F64)
+    lab = labels.to(torch.int64).reshape(-1).to(X.device)
+    valid = lab != ignore_index
+    m = X.max(-1, keepdim=True).values
+    e = torch.exp(X - m)
+    se = e.sum(-1, keepdim=True)
+    P = e / se
+    lse = m + torch.log(se)
+    rho = 1.0 + (X - m).abs()
+    prho = (P * rho).sum(-1, keepdim=True)
+    onehot = torch.zeros_like(X)
+    lab_c = lab.clamp(0, V - 1)
+    onehot.scatter_(1, lab_c.view(-1, 1), 1.0)
+    gs = float(grad_scale)
+    vm = valid.view(-1, 1).to(_F64)
+    grad = gs * (P - onehot) * vm
+    bgrad = (ROW_C_F32 * abs(gs) * P * (rho + prho) + abs(gs) * ROW_FTZ) * vm
+    xl = X.gather(1, lab_c.view(-1, 1))
+    row_loss = ((lse - xl) * vm).reshape(-1)
+    row_b = (ROW_C_F32 * (lse.abs() + m.abs() + xl.abs() + prho) * vm).reshape(-1)
+    l0 = _f32(loss_before).reshape(-1)[0].to(_F64)
+    total = l0 + row_loss.sum()
+    loss_bound = ROW_C_ACC * (l0.abs() + (row_loss.abs()).sum()) + row_b.sum()
+    count = _f32(count_before).reshape(-1)[0] + float(int(valid.sum()))
+    return {"grad": (grad, bgrad), "loss_sum": (total.reshape(1), loss_bound.reshape(1)), "count": count.reshape(1)}
+
+
+def _rotate(a, b, c, s):
+    """(a c − b s, b c + a s) and its magnitude (|a c| + |b s|, |b c| + |a s|) in fp64."""
+    return a * c - b * s, b * c + a * s, (a * c).abs() + (b * s).abs(), (b * c).abs() + (a * s).abs()
+
+
+def rope_inplace_ref(buf: torch.Tensor, T: int, n_rot_heads: int, hd: int, rotary_dim: int, cos, sin, backward: bool, pos0: int):
+    """Contract of ``rope_inplace(buf, T, n_rot_heads, hd, rotary_dim, cos, sin, backward, pos0)`` on ``buf [M, ≥ n_rot_heads·hd]``
+    as it was before the call.  Row r sits at position r mod T + pos0; head h < n_rot_heads, i < rotary_dim/2:
+
+        (a, b) = (x[h·hd + i], x[h·hd + i + rotary_dim/2]) -> (a c − b s, b c + a s),  c = cos[pos, i],  s = ±sin[pos, i]
+
+    (s negated for the backward), in fp32 with one bf16 rounding.  Returns ``(mask, ref, bound)`` over buf's columns: where
+    ``mask`` is False the element must keep its bits."""
+    return _rope_ref(buf, T, [h * hd for h in range(n_rot_heads)], rotary_dim, cos, sin, -1.0 if backward else 1.0, pos0)
+
+
+def _rope_ref(buf, T, starts, rot, cos, sin, sgn, pos0):
+    X = buf.to(_F64)
+    M, W = X.shape
+    half = rot // 2
+    pos = torch.arange(M, device=buf.device) % T + pos0
+    c = cos.to(_F64)[pos][:, :half]
+    s = sgn * sin.to(_F64)[pos][:, :half]
+    ref, bound = X.clone(), torch.zeros_like(X)
+    mask = torch.zeros(M, W, dtype=torch.bool, device=buf.device)
+    for s0 in starts:
+        a, b = X[:, s0:s0 + half], X[:, s0 + half:s0 + rot]
+        y1, y2, b1, b2 = _rotate(a, b, c, s)
+        ref[:, s0:s0 + half], ref[:, s0 + half:s0 + rot] = y1, y2
+        bound[:, s0:s0 + half], bound[:, s0 + half:s0 + rot] = ROW_C_F32 * b1, ROW_C_F32 * b2
+        mask[:, s0:s0 + rot] = True
+    return mask, ref, bound
+
+
+def neox_rope_ref(qkv: torch.Tensor, T: int, nh: int, hd: int, rot: int, cos, sin, pos0: int, inverse: bool):
+    """Contract of ``neox_rope(qkv, T, nh, hd, rot, cos, sin, pos0, inverse)`` on the GPT-NeoX ``[rows, nh·(q|k|v)·hd]`` layout
+    with fp32 tables ``[n_pos, rot]``: the first ``rot`` dims of each q and k head rotate as in :func:`rope_inplace_ref`; v and
+    the dims past ``rot`` keep their bits.  Returns ``(mask, ref, bound)``."""
+    starts = [h * 3 * hd + w * hd for h in range(nh) for w in (0, 1)]
+    return _rope_ref(qkv, T, starts, rot, cos, sin, -1.0 if inverse else 1.0, pos0)
+
+
+def rope_pack_bwd_ref(dq, dk, dv, rotary_dim: int, cos, sin, pos0: int):
+    """Contract of ``rope_pack_bwd(dq, dk, dv, out, rotary_dim, cos, sin, pos0, nkv)``: ``dq [B, nh, T, hd]``, ``dk / dv
+    [B, nkv, T, hd]`` (any strides) gathered into ``out [B·T, (nh + 2·nkv)·hd]`` = [q heads | k heads | v heads], q and k
+    rotated back (s -> −s, position t + pos0) in their first ``rotary_dim`` dims, everything else copied.  Returns
+    ``(exact_mask, ref, bound)``: where ``exact_mask`` is set the value is a copy and must match bit for bit."""
+    B, nh, T, hd = dq.shape
+    nkv = dk.shape[1]
+    rows = lambda t: t.permute(0, 2, 1, 3).reshape(B * T, -1)  # noqa: E731  [B·T, heads·hd]
+    X = torch.cat([rows(dq), rows(dk), rows(dv)], 1)
+    mask, ref, bound = _rope_ref(X, T, [h * hd for h in range(nh + nkv)], rotary_dim, cos, sin, -1.0, pos0)
+    return ~mask, ref, bound
+
+
+def swiglu_fwd_ref(gu: torch.Tensor, F: int) -> tuple:
+    """Contract of ``swiglu_fwd(gu, h, ...)``: ``h = bf16(silu(g) · u)`` with g = gu[:, :F], u = gu[:, F:2F], computed as
+    g / (1 + __expf(−g)) · u.  Bound ROW_C_F32·|h|·(1 + |g|) (__expf's argument); where 1 + e^{−g} passes 2^126 (g < −87)
+    __fdividef returns 0, so there the whole value is allowed.  The dropout / E4M3 copies are derived from the stored h."""
+    G, U = gu[:, :F].to(_F64), gu[:, F:2 * F].to(_F64)
+    sg = torch.sigmoid(G)
+    h = G * sg * U
+    bound = ROW_C_F32 * h.abs() * (1.0 + G.abs()) + torch.where(G < -87.0, h.abs(), torch.zeros_like(h))
+    return h, bound
+
+
+def swiglu_bwd_ref(dh: torch.Tensor, gu: torch.Tensor, F: int) -> dict:
+    """Contract of ``swiglu_bwd(dh, gu, dgu)``: with σ = sigmoid(g), silu = g·σ (σ = __fdividef(1, 1 + __expf(−g))):
+
+        dgu[:, :F] = dh · u · (σ + silu · (1 − σ))        dgu[:, F:] = dh · silu
+
+    Bounds as :func:`swiglu_fwd_ref` (magnitudes σ(1 + |g|(1 − σ))·|dh u| and |dh silu|)."""
+    G, U, D = gu[:, :F].to(_F64), gu[:, F:2 * F].to(_F64), dh.to(_F64)
+    sg = torch.sigmoid(G)
+    silu = G * sg
+    dg = D * U * (sg + silu * (1.0 - sg))
+    du = D * silu
+    flush = G < -87.0
+    z = torch.zeros_like(dg)
+    bdg = ROW_C_F32 * (D * U).abs() * sg * (1.0 + G.abs() * (1.0 - sg)) * (1.0 + G.abs()) + torch.where(flush, dg.abs(), z)
+    bdu = ROW_C_F32 * du.abs() * (1.0 + G.abs()) + torch.where(flush, du.abs(), z)
+    return {"dg": (dg, bdg), "du": (du, bdu)}
+
+
+_SQRT_2_OVER_PI = math.sqrt(2.0 / math.pi)
+
+
+def gelu_fwd_ref(z: torch.Tensor, tanh_approx: bool) -> tuple:
+    """Contract of ``gelu_fwd(z, a, tanh_approx)``: a = bf16(0.5 z (1 + erf(z/√2))), or with the tanh form
+    0.5 z (1 + tanh(√(2/π)(z + 0.044715 z³))), fp32 erff / tanhf.  The absolute error of 1 + erf (or 1 + tanh) is a few fp32
+    ulps of 1 (and, for tanh, of the argument u times 1 − t²), so the bound is ROW_C_F32·0.5|z|·(1 + |u|(1 − t²))."""
+    Z = z.to(_F64)
+    if tanh_approx:
+        u = _SQRT_2_OVER_PI * (Z + 0.044715 * Z ** 3)
+        t = torch.tanh(u)
+        a = 0.5 * Z * (1.0 + t)
+        mag = 0.5 * Z.abs() * (1.0 + u.abs() * (1.0 - t * t))
+    else:
+        a = 0.5 * Z * torch.erfc(-Z / math.sqrt(2.0))  # 1 + erf without its cancellation for z << 0
+        mag = 0.5 * Z.abs() * 2.0
+    return a, ROW_C_F32 * (mag + a.abs())
+
+
+def gelu_bwd_ref(da: torch.Tensor, z: torch.Tensor, tanh_approx: bool) -> tuple:
+    """Contract of ``gelu_bwd(da, z, dz, tanh_approx)``: dz = bf16(da · GELU'(z)); erf form
+    GELU'(z) = 0.5 (1 + erf(z/√2)) + z φ(z) with φ from __expf(−z²/2), tanh form
+    0.5 (1 + t) + 0.5 z (1 − t²) √(2/π)(1 + 3·0.044715 z²).  Bound ROW_C_F32·|da|·(1 + |z|·d(z)·(1 + z²)), d the size of the
+    exponential / sech² factor.  ``dbias`` (column sum of the *rounded* dz) is checked with :func:`colsum_ref` on the dz the
+    kernel stored."""
+    Z, DA = z.to(_F64), da.to(_F64)
+    if tanh_approx:
+        u = _SQRT_2_OVER_PI * (Z + 0.044715 * Z ** 3)
+        t = torch.tanh(u)
+        d = 0.5 * (1.0 + t) + 0.5 * Z * (1.0 - t * t) * _SQRT_2_OVER_PI * (1.0 + 3.0 * 0.044715 * Z * Z)
+        fac = (1.0 - t * t) * (1.0 + u.abs())
+    else:
+        phi = torch.exp(-0.5 * Z * Z) / math.sqrt(2.0 * math.pi)
+        d = 0.5 * torch.erfc(-Z / math.sqrt(2.0)) + Z * phi
+        fac = phi
+    return DA * d, ROW_C_F32 * DA.abs() * (1.0 + Z.abs() * fac * (1.0 + Z * Z))
+
+
+def colsum_ref(x: torch.Tensor, before: torch.Tensor) -> tuple:
+    """``out = before + Σ_rows x`` (``colsum``, the dbias of ``gelu_bwd`` over the stored dz), fp32 accumulation."""
+    X, b0 = x.to(_F64), before.to(_F64)
+    return b0 + X.sum(0), ROW_C_ACC * (b0.abs() + X.abs().sum(0))
+
+
+def embedding_bwd_ref(ids: torch.Tensor, dout: torch.Tensor, dtable_before: torch.Tensor, padding_idx: int) -> tuple:
+    """``embedding_bwd``: dtable[id] += dout row for every position whose id is not ``padding_idx`` (fp32 atomics)."""
+    idx = ids.reshape(-1).to(torch.int64)
+    D = dout.reshape(idx.numel(), -1).to(_F64)
+    keep = idx != padding_idx
+    acc = torch.zeros(dtable_before.shape, dtype=_F64, device=D.device)
+    mag = torch.zeros_like(acc)
+    acc.index_add_(0, idx[keep], D[keep])
+    mag.index_add_(0, idx[keep], D[keep].abs())
+    b0 = dtable_before.to(_F64)
+    return b0 + acc, ROW_C_ACC * (b0.abs() + mag)
+
+
+def embedding_bwd_sorted_exact(sorted_ids: torch.Tensor, perm: torch.Tensor, dout: torch.Tensor, dtable_before: torch.Tensor,
+                               padding_idx: int) -> torch.Tensor:
+    """``embedding_bwd_sorted(sorted_ids, perm, dout, dtable, padding_idx)``: for every run of equal ids in ``sorted_ids``, the
+    fp32 sum of the rows ``dout[perm[k]]`` in run order starting from 0, then one fp32 add into the prior table row (a stable
+    sort makes the run order the position order).  Plain fp32 adds, no FMA: reproduced bit for bit."""
+    sid = sorted_ids.reshape(-1).to(torch.int64).cpu()
+    pm = perm.reshape(-1).to(torch.int64).cpu()
+    D = _f32(dout.reshape(sid.numel(), -1)).cpu()
+    out = _f32(dtable_before).cpu().clone()
+    uniq, counts = torch.unique_consecutive(sid, return_counts=True)
+    starts = torch.cumsum(counts, 0) - counts
+    sel = uniq != padding_idx
+    uniq, counts, starts = uniq[sel], counts[sel], starts[sel]
+    acc = torch.zeros(uniq.numel(), D.shape[1], dtype=torch.float32)
+    for k in range(int(counts.max()) if counts.numel() else 0):
+        live = counts > k
+        acc[live] = acc[live] + D[pm[starts[live] + k]]
+    out[uniq] = out[uniq] + acc
+    return out.to(dtable_before.device)
+
+
+def dropout_combine_ref(base, parts_groups, seed, keys, p: float) -> tuple:
+    """``dropout_combine(base, parts, out, seed, keys, p)``: out = bf16(base + Σ_g keep_g ⊙ parts_g / (1 − p)), fp32."""
+    M, H = parts_groups[0].shape
+    acc = torch.zeros(M, H, dtype=_F64, device=parts_groups[0].device) if base is None else base.to(_F64).reshape(M, H)
+    mag = acc.abs()
+    inv = _keep_f32(p)
+    for g, part in enumerate(parts_groups):
+        keep = dropout_keep_mask(mix_seed(_seed_of(seed), keys[g]), M, H, p, device=part.device)
+        t = part.to(_F64) * inv * keep
+        acc, mag = acc + t, mag + t.abs()
+    return acc, ROW_C_F32 * mag
+
+
+def adamw_ref(p, g, m, v, *, lr, b1, b2, eps, wd, step, grad_scale: float = 1.0) -> dict:
+    """Contract of ``adamw_flat(p, g, m, v, lr, b1, b2, eps, wd, step, grad_scale, grad_scale_host, skip, step_dev)`` with the
+    hyperparameters as the fp32 values the kernel receives and ``grad_scale`` the product of the device and host scales:
+
+        g' = g·gs,  m' = b1 m + (1 − b1) g',  v' = b2 v + (1 − b2) g'²              (stored in m's / v's dtype)
+        p' = bf16(p (1 − lr wd) − lr/(1 − b1^t) · m' / (√v' / √(1 − b2^t) + eps))    (from the unrounded m', v')
+
+    Bounds: ROW_C_F32 times the magnitudes of the terms; powf's relative error ε (inside ROW_C_F32) in b^t becomes
+    ε·b^t/(1 − b^t) in the bias corrections, which is large at small t, so that factor is carried explicitly."""
+    f = lambda a: float(torch.tensor(a, dtype=torch.float32))  # noqa: E731
+    lr, b1, b2, eps, wd, gs = f(lr), f(b1), f(b2), f(eps), f(wd), f(grad_scale)
+    G, P, Mo, Vo = g.to(_F64) * gs, p.to(_F64), m.to(_F64), v.to(_F64)
+    m1 = b1 * Mo + (1.0 - b1) * G
+    v1 = b2 * Vo + (1.0 - b2) * G * G
+    bm = b1 * Mo.abs() + (1.0 - b1) * G.abs()
+    bc1, bc2 = 1.0 - b1 ** step, 1.0 - b2 ** step
+    k1, k2 = 1.0 + b1 ** step / bc1, 1.0 + b2 ** step / bc2
+    denom = torch.sqrt(v1) / math.sqrt(bc2) + eps
+    upd = (lr / bc1) * m1 / denom
+    decay = 1.0 - lr * wd
+    pn = P * decay - upd
+    bp = ROW_C_F32 * (P.abs() * abs(decay) + (lr / bc1) * bm / denom * (k1 + k2))
+    return {"p": (pn, bp), "m": (m1, ROW_C_F32 * bm), "v": (v1, ROW_C_F32 * v1)}
+
+
+def sumsq_ref(x: torch.Tensor, before: torch.Tensor) -> tuple:
+    """``sumsq(x, out)``: out = before + Σ x², fp32 accumulation."""
+    X, b0 = x.to(_F64).reshape(-1), _f32(before).reshape(-1)[:1].to(_F64)
+    s = (X * X).sum()
+    return b0 + s, ROW_C_ACC * (b0.abs() + s)
+
+
+def fp8_quantize_weight_exact(w: torch.Tensor):
+    """``fp8_quantize_weight(w, w8, scratch, scale, inv_scale, w8t)``: amax = max|w|, scale = max(amax, 1e-12)/448,
+    inv_scale = 1/scale (IEEE fp32), w8 = sat_e4m3(fp32(w · inv_scale)), w8t its transpose.  Returns the exact
+    ``(amax, scale, inv_scale, w8, w8t)``."""
+    W = _f32(w)
+    amax = W.abs().max().reshape(1)
+    # numpy: a torch division by a Python scalar multiplies by the reciprocal, one ulp off the kernel's IEEE division
+    a = amax.cpu().numpy()
+    scale = np.maximum(a, np.float32(1e-12)) / np.float32(448.0)
+    inv = np.float32(1.0) / scale
+    scale, inv = torch.from_numpy(scale).to(w.device), torch.from_numpy(inv).to(w.device)
+    q = fp8_saturate(W * inv)
+    return amax, scale, inv, q, q.t().contiguous()
+
+
+def fp8_prep_exact(state, w_scale, margin: float, n_e4m3: int) -> dict:
+    """``fp8_prep(state, w_scale, inv_sx, alpha_main, alpha_inv, margin, n_e4m3)`` per site i (all fp32, IEEE division):
+
+        prev = state[i,1] > 0 ? state[i,1] : state[i,0];   state[i] <- (prev, 0)
+        sx = max(prev, 1e-12) · margin / fmax_i   (fmax 448 for i < n_e4m3, else 57344)
+        inv_sx = 1/sx,  alpha_main = sx · w_scale[i],  alpha_inv = 1/alpha_main"""
+    S = _f32(state).reshape(-1, 2)
+    n = S.shape[0]
+    cur, old = S[:, 1], S[:, 0]
+    prev = torch.where(cur > 0, cur, old)
+    fmax = torch.where(torch.arange(n, device=S.device) < n_e4m3, torch.tensor(448.0, device=S.device),
+                       torch.tensor(57344.0, device=S.device))
+    sx = torch.clamp(prev, min=torch.tensor(1e-12, dtype=torch.float32, device=S.device)) * torch.tensor(
+        margin, dtype=torch.float32) / fmax
+    one = torch.tensor(1.0, dtype=torch.float32, device=S.device)
+    a = sx * _f32(w_scale).reshape(-1)
+    return {"state": torch.stack([prev, torch.zeros_like(prev)], 1).reshape(state.shape), "inv_sx": one / sx,
+            "alpha_main": a, "alpha_inv": one / a}
+
+
+def assert_rowwise_close(name: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> float:
+    """Element-wise check of a row-wise kernel output against its fp64 contract:
+
+        |got − ref| ≤ c_out·|ref| + bound
+
+    ``c_out`` is the output rounding (2⁻⁸ for bf16, 2⁻²⁴ for fp32); ``bound`` comes from the ``*_ref`` function with its
+    coefficient applied.  A NaN fails.  Returns the worst ratio of error to tolerance (<= 1 when it passes); the failure
+    message names the worst element by index."""
+    g = got.to(_F64)
+    ref = ref.to(g.device).expand_as(g)
+    bound = bound.to(g.device).expand_as(g)
+    c_out = _BF16_OUT if got.dtype == torch.bfloat16 else _F32_OUT
+    err = (g - ref).abs()
+    tol = c_out * ref.abs() + bound
+    ratio = torch.where(tol > 0, err / tol.clamp(min=1e-300), torch.where(err == 0, 0.0, math.inf))
+    ratio = torch.nan_to_num(ratio, nan=math.inf, posinf=math.inf)
+    if ratio.numel() == 0:
+        return 0.0
+    flat = int(torch.argmax(ratio))
+    idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(flat), ratio.shape))
+    worst = float(ratio[idx])
+    if not worst <= 1.0:
+        n_bad = int((ratio > 1.0).sum())
+        raise AssertionError(
+            f"{name} out of tolerance at {n_bad} of {ratio.numel()} elements; worst ratio {worst:.3g} at {idx}: "
+            f"got={float(g[idx]):.6g} ref={float(ref[idx]):.6g} tol={float(tol[idx]):.6g} (bound={float(bound[idx]):.6g})")
+    return worst
+
+
+def rowwise_excess(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> float:
+    """Worst (|got − ref| − c_out·|ref|)⁺ / bound: how much of the empirical coefficient inside ``bound`` an output used."""
+    g = got.to(_F64)
+    c_out = _BF16_OUT if got.dtype == torch.bfloat16 else _F32_OUT
+    ex = ((g - ref.to(g.device)).abs() - c_out * ref.to(g.device).abs()).clamp(min=0)
+    b = bound.to(g.device).expand_as(ex)
+    r = torch.where(b > 0, ex / b.clamp(min=1e-300), torch.zeros_like(ex))
+    return float(r.max()) if r.numel() else 0.0
+
+
+def _bits(t: torch.Tensor) -> torch.Tensor:
+    return t.contiguous().view({1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[t.element_size()])
+
+
+def assert_bitwise_equal(name: str, got: torch.Tensor, ref: torch.Tensor) -> None:
+    """Exact contracts: every element of ``got`` has the bits of ``ref``; the message names the first one that does not."""
+    ref = ref.to(got.device)
+    if got.shape != ref.shape or got.dtype != ref.dtype:
+        raise AssertionError(f"{name}: got {tuple(got.shape)} {got.dtype}, expected {tuple(ref.shape)} {ref.dtype}")
+    diff = _bits(got) != _bits(ref)
+    if bool(diff.any()):
+        idx = tuple(int(i) for i in diff.nonzero()[0])
+        n_bad = int(diff.sum())
+        gv = got[idx].float().item() if got.is_floating_point() else got[idx].item()
+        rv = ref[idx].float().item() if ref.is_floating_point() else ref[idx].item()
+        raise AssertionError(f"{name} differs at {n_bad} of {got.numel()} elements; first at {idx}: got={gv!r} expected={rv!r}")
 
 
 # ----------------------------------------------------------------------------- merge
