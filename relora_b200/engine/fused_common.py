@@ -1,31 +1,129 @@
 """Model-independent machinery of the whole-model fused executors (:mod:`.fused_llama`, :mod:`.fused_pythia`).
 
-An executor subclass owns the model-specific buffers and the ``_alloc`` / ``_forward`` / ``_backward`` of one micro-batch; this
-base class provides the rest:
+An executor subclass owns what depends on the model: its checks of a model's shapes, the order of its trainable parameters and
+their stacked views, its own buffers (``_alloc_layers``) and the ``_forward`` / ``_backward`` of one micro-batch.  This module
+provides the rest:
 
-* the gradient transport (NVLink peer-memory kernels when symmetric memory is available, NCCL otherwise), the flat parameter store
-  with stacked views, ``GradSync`` and ``FlatAdamW``;
-* ``update()`` (NCCL or the peer-memory kernel chain);
+* the checks every ``supports`` / ``supports_full_rank`` shares: the ReLoRA wrapper, fp8 in full-rank training, the native
+  attention head dim and, last, the device;
+* the constructor preamble (sizes, ReLoRA rank / dropout / scale, attention backend, side stream, environment knobs), the gradient
+  transport (NVLink peer-memory kernels when symmetric memory is available, NCCL otherwise), the flat parameter store with stacked
+  views, ``GradSync`` and ``FlatAdamW``;
+* the buffers both executors share, the per-layer slot selection, the SDPA fallback attention and the embedding backward;
+* ``update()`` (NCCL or the peer-memory kernel chain) and ``merge_and_reinit()``;
 * one CUDA graph per micro-batch shape, capture / replay and launch counting;
 * the LoRA group forward / backward on the wgmma GEMM and the fused input-gradient kernel, and the chunked LM head + CE.
 """
 from __future__ import annotations
 
+import math
+import os
 from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
+import torch.nn.functional as F_
 
 from ..ops import fused
 from ..parallel.flat import FlatAdamW, FlatParamStore
-from ..parallel.grad_sync import GradSync
+from ..parallel.grad_sync import GradSync, broadcast_params
+from ..relora import ReLoRaModel
 from .stepper import UpdateInfo
 
 BF = torch.bfloat16
 
 
+# ---------------------------------------------------------------------- checks shared by every supports() / supports_full_rank()
+# Each returns why the executor declines ``model``, or None.
+def relora_refusal(model, inner_cls, other_model: str) -> Optional[str]:
+    """The ReLoRA wrapper: a ``ReLoRaModel`` around an ``inner_cls`` (else ``other_model``) on the plain recipe."""
+    if not isinstance(model, ReLoRaModel):
+        return "full-rank training uses the module path"
+    if not isinstance(model.wrapped_model, inner_cls):
+        return other_model
+    if model.lora_only or model.trainable_scaling or model._config.quantize is not None:
+        return "lora_only / trainable scaling / quantized frozen weights use the module path"
+    return None
+
+
+def full_rank_refusal(model, cls, other_model: str, args) -> Optional[str]:
+    """A bare ``cls`` (else ``other_model``), and no fp8 frozen-weight recipe: full-rank training has no frozen weights."""
+    if not isinstance(model, cls):
+        return other_model
+    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return f"--frozen_dtype {args.frozen_dtype} has no frozen weights to act on in full-rank training"
+    return None
+
+
+def native_attention_refusal(hd: int, args) -> Optional[str]:
+    attention = getattr(args, "attention", "auto")
+    if attention == "native" and fused.attention_backend(hd, attention) != "native":
+        return f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM}, got {hd}"
+    return None
+
+
+def device_refusal(model) -> Optional[str]:
+    """Checked after the shapes, so their reasons are visible on a CPU model."""
+    p = next(model.parameters())
+    return None if p.is_cuda and p.dtype == BF else "needs CUDA + bfloat16"
+
+
+class LayerViews:
+    """Views of one layer's parameters and gradients, None where a mode has no such tensor (the LoRA factors in full-rank training,
+    the projection-weight gradients under ReLoRA).  Each executor lists its view names in ``__slots__``, so a misspelt name fails."""
+
+    __slots__ = ()
+
+    def __init__(self):
+        for k in self.__slots__:
+            setattr(self, k, None)
+
+
 class FusedStepperBase:
     # ------------------------------------------------------------------ construction helpers
+    def __init__(self, model, info, supports, supports_full_rank, *, grad_accumulation: int, clip_grad_norm: float,
+                 cuda_graphs: bool, ce_chunk: int, overlap_wgrad: bool, attention: str, deterministic: bool):
+        """Settings and sizes every executor has; ``supports`` / ``supports_full_rank`` are the executor's checks of a ReLoRA model
+        and of a bare one (full-rank training)."""
+        self.full = not isinstance(model, ReLoRaModel)
+        ok, why = supports_full_rank(model) if self.full else supports(model)
+        if not ok:
+            raise RuntimeError(why)
+        self.model, self.info = model, info
+        self.inner = model if self.full else model.wrapped_model
+        self.C = fused._C()
+        self.ga = grad_accumulation
+        self.clip = clip_grad_norm
+        self.use_graphs = cuda_graphs
+        self.ce_chunk = ce_chunk
+        cfg = self.inner.config
+        self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
+        self.hd = self.h // self.nh
+        self.L = cfg.num_hidden_layers
+        self.r = 0 if self.full else model.r
+        self.p = 0.0 if self.full else float(model.lora_dropout)
+        self.scale = 1.0 if self.full else float(model.lora_alpha) / model.r
+        self.device = info.device
+        broadcast_params(model)
+        attention = os.environ.get("RELORA_B200_ATTENTION", attention)
+        # auto: this repo's wgmma kernels (csrc/attention.cu) for head_dim <= 64 -- the hot path then contains no library
+        # attention call -- and torch SDPA (cuDNN) above; native: the kernels up to head_dim 256; sdpa: torch SDPA
+        # (bench/attn_bench.py times both)
+        self.native_attn = fused.attention_backend(self.hd, attention) == "native"
+        if attention == "native" and not self.native_attn:
+            raise RuntimeError(f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM} (multiple of 8), "
+                               f"got {self.hd}")
+        self._attn_saved: List = []  # SDPA: (o, q, k, v) of every layer of the training forward
+        self.side = torch.cuda.Stream(device=self.device) if overlap_wgrad else None
+        self.fp8 = self.fp8_bwd = False  # E4M3 frozen weights (csrc/fp8.cu): an executor that has them turns them on
+        self.fused_dx = True
+        # stacked output width from which the LoRA input gradient uses two kernels (see _lora_group_bwd); 0: the executor's default
+        self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0"))
+        # --deterministic asks for fixed summation orders; each executor sets which of its GEMMs give up split-K (wgrad_split_k)
+        self.deterministic = deterministic or os.environ.get("RELORA_B200_DETERMINISTIC", "0") == "1"
+        # embedding backward without atomics (default); RELORA_B200_ATOMIC_EMBEDDING=1 selects the atomicAdd scatter
+        self.deterministic_embedding = os.environ.get("RELORA_B200_ATOMIC_EMBEDDING", "0") != "1"
+
     def _init_transport(self, info, transport: str) -> None:
         """NVLink peer-memory kernels when symmetric memory is available (``self.comm``), NCCL otherwise (``self.comm = None``)."""
         self.comm = None
@@ -44,8 +142,18 @@ class FusedStepperBase:
             elif transport == "p2p":
                 raise RuntimeError("--comm p2p needs torch symmetric memory over an NCCL process group")
 
-    def _init_store(self, named: List[Tuple[str, torch.nn.Parameter]], padded: Optional[Dict[int, Tuple[int, int]]] = None) -> None:
-        """Flat fp32-gradient store over ``named`` (in that order); ``padded`` maps parameters to zero-padded storage shapes."""
+    def _build_store(self, params: List[torch.nn.Parameter], transport: str,
+                     padded: Optional[Dict[int, Tuple[int, int]]] = None) -> None:
+        """Gradient transport and flat fp32-gradient store over ``params``, which must be every trainable parameter of the model.
+        Their order is the store's layout (stacked views, checkpoints, ZeRO shards and the peer-memory update depend on it);
+        ``padded`` maps parameters to zero-padded storage shapes."""
+        name_of = {id(p): n for n, p in self.model.named_parameters()}
+        named = [(name_of[id(p)], p) for p in params]
+        seen = {id(p) for p in params}
+        extra = [n for n, p in self.model.named_parameters() if p.requires_grad and id(p) not in seen]
+        if extra:
+            raise RuntimeError(f"unexpected trainable parameters for the fused executor: {extra}")
+        self._init_transport(self.info, transport)
         self.store = FlatParamStore(named, world_size=self.info.world_size, grad_dtype=torch.float32, bind_grads=False,
                                     allocator=self.comm.allocator() if self.comm is not None else None,
                                     storage_shapes=padded or {})
@@ -88,17 +196,82 @@ class FusedStepperBase:
         self._wg_done: Dict[str, torch.cuda.Event] = {}
 
     # ------------------------------------------------------------------ hooks of the subclasses
-    def _alloc(self, B: int, T: int) -> None:
-        raise NotImplementedError
-
-    def _micro_body(self) -> None:
+    def _alloc_layers(self, B: int, T: int) -> None:
+        """The executor's own buffers for a [B, T] micro-batch (``_alloc`` has set ``B_`` / ``T_`` / ``M_`` and ``x_in``)."""
         raise NotImplementedError
 
     def _before_micro(self) -> None:
         """Runs before a micro-step (outside the CUDA graph)."""
 
+    # ------------------------------------------------------------------ one micro-batch
+    def _alloc(self, B: int, T: int) -> None:
+        dev, L, h = self.device, self.L, self.h
+        M = B * T
+        self.B_, self.T_, self.M_ = B, T, M
+        self.ids = torch.zeros(B, T, dtype=torch.long, device=dev)
+        self.labels = torch.zeros(M, dtype=torch.long, device=dev)
+        self.x_in = torch.empty(L + 1, M, h, dtype=BF, device=dev)  # layer inputs, saved for the backward ([0], [1] in evaluation)
+        self._alloc_layers(B, T)
+        if self.native_attn:
+            self.attn_o = torch.empty(L, M, h, dtype=BF, device=dev)
+            self.lse = torch.empty(L, B, self.nh, T, dtype=torch.float32, device=dev)
+            self.delta = torch.empty(B, self.nh, T, dtype=torch.float32, device=dev)
+        ldv = (self.V + 7) // 8 * 8
+        self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
+        self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.count = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
+        self._shape = (B, T)
+
+    def _layer_slots(self, train: bool):
+        """(l, views, slot, x, x_next) per layer of the forward: ``slot`` indexes the per-layer saved activations and ``x`` /
+        ``x_next`` are the layer's input and output.  Training keeps every layer's; evaluation reuses slot 0 and alternates two
+        residual buffers."""
+        for l, S in enumerate(self.layers):
+            if train:
+                yield l, S, l, self.x_in[l], self.x_in[l + 1]
+            else:
+                yield l, S, 0, self.x_in[l % 2], self.x_in[(l + 1) % 2]
+
+    def _sdpa(self, q, k, v, train: bool, **kw):
+        """Causal torch SDPA over [B, heads, T, head_dim] views (the attention where the wgmma kernels are not used); in training
+        the call's autograd graph is kept for ``_sdpa_bwd``."""
+        if not train:
+            return F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **kw)
+        q, k, v = (t.detach().requires_grad_() for t in (q, k, v))
+        with torch.enable_grad():
+            o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **kw)
+        self._attn_saved.append((o, q, k, v))
+        return o.detach()
+
+    def _sdpa_bwd(self, l: int):
+        """(dq, dk, dv) of layer ``l``'s SDPA call for the attention-output gradient in ``dattn``."""
+        o, q, k, v = self._attn_saved[l]
+        return torch.autograd.grad(o, (q, k, v), self.dattn.view(self.B_, self.T_, self.nh, self.hd).transpose(1, 2))
+
+    def _embedding_bwd_and_join(self, dx, tags) -> None:
+        """The embedding gradient from ``dx`` (the gradient of the first layer's input), then the main stream waits for every
+        side-stream weight gradient (``tags``, in that order)."""
+        if self.deterministic_embedding:
+            # stable sort of the token ids (12 K keys) -> one writer per table row, fixed summation order: bit-reproducible
+            sorted_ids, perm = torch.sort(self.ids.view(-1), stable=True)
+            self.C.embedding_bwd_sorted(sorted_ids, perm, dx, self.gW_emb, self.pad_idx)
+        else:
+            self.C.embedding_bwd(self.ids.view(-1), dx, self.gW_emb, self.pad_idx)
+        for tag in tags:
+            self._join(tag)
+        self._attn_saved.clear()
+
+    def _micro_body(self) -> None:
+        self._set_labels()
+        self._forward(True)
+        self._loss_and_head_backward(True)
+        self._backward()
+        self.C.seed_advance(self.seed)
+
     def _eval_body(self) -> None:
-        raise NotImplementedError
+        self._forward(False)
+        self._loss_and_head_backward(False)
 
     # ------------------------------------------------------------------ LoRA groups
     def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False, bias=None, Nq=None):
@@ -356,19 +529,21 @@ class FusedStepperBase:
         return UpdateInfo(total, False)
 
     @torch.no_grad()
-    def _merge_modules(self, blocks):
-        """W += s·B@A for every (module, (B, A, W)) of ``blocks`` (wgmma GEMM accumulating into W in fp32), then the hash re-init
-        of the module path: A ~ U(±1/√in) keyed by (seed, restart, module index), B = 0."""
-        import math
-
+    def merge_and_reinit(self):
+        """W += s·B@A for every module of every layer and its (B, A, W) block (``mods`` / ``merge`` of the layer views; wgmma GEMM
+        accumulating into W in fp32), then the hash re-init of the module path: A ~ U(±1/√in) keyed by (seed, restart, module
+        index), B = 0."""
+        if self.full:
+            raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
         from ..ops import reference as ref
 
         g, r = fused.gemm, self.r
-        for m, (Bm, Am, Wm) in blocks:
-            g(Bm, Am, Wm, M=Wm.shape[0], N=Wm.shape[1], K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
-            sd = ref.mix_seed(self.model.seed, self.model.n_restarts, m.module_index)
-            self.C.fill_uniform_hash(m.lora_A.weight.data, sd, 1.0 / math.sqrt(m.in_features))
-            m.lora_B.weight.data.zero_()
+        for S in self.layers:
+            for m, (Bm, Am, Wm) in zip(S.mods, S.merge):
+                g(Bm, Am, Wm, M=Wm.shape[0], N=Wm.shape[1], K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
+                sd = ref.mix_seed(self.model.seed, self.model.n_restarts, m.module_index)
+                self.C.fill_uniform_hash(m.lora_A.weight.data, sd, 1.0 / math.sqrt(m.in_features))
+                m.lora_B.weight.data.zero_()
         self.model.n_restarts += 1
 
     def launches_in_window(self, n_steps: int) -> int:

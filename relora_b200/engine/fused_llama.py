@@ -31,27 +31,23 @@ import os
 from typing import Dict, List, Tuple
 
 import torch
-import torch.nn.functional as F_
 
 from ..models.llama import LlamaForCausalLM, num_kv_heads
 from ..ops import fused, native
 from ..parallel.dist import DistInfo
 from ..parallel.flat import _ALIGN as _STORE_ALIGN
-from ..parallel.grad_sync import broadcast_params
-from ..relora import ReLoRaLinear, ReLoRaModel
-from .fused_common import FusedStepperBase
+from ..relora import ReLoRaLinear
+from .fused_common import (FusedStepperBase, LayerViews, device_refusal, full_rank_refusal, native_attention_refusal,
+                           relora_refusal)
 
 BF = torch.bfloat16
 
 
 def supports(model, args=None) -> Tuple[bool, str]:
-    if not isinstance(model, ReLoRaModel):
-        return False, "full-rank training uses the module path"
+    why = relora_refusal(model, LlamaForCausalLM, "only Llama is fused")
+    if why:
+        return False, why
     inner = model.wrapped_model
-    if not isinstance(inner, LlamaForCausalLM):
-        return False, "only Llama is fused"
-    if model.lora_only or model.trainable_scaling or model._config.quantize is not None:
-        return False, "lora_only / trainable scaling / quantized frozen weights use the module path"
     cfg = inner.config
     h, f, nh = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads
     nkv = num_kv_heads(cfg)
@@ -67,9 +63,10 @@ def supports(model, args=None) -> Tuple[bool, str]:
         return False, f"hidden ({h}) and rank ({r}) must be multiples of 128 for stacked groups"
     if hd % 8 or hd % 4:
         return False, "head_dim must be a multiple of 8"
-    p = next(inner.parameters())
-    if not p.is_cuda or p.dtype != BF:
-        return False, "needs CUDA + bfloat16"
+    # --attention native is not checked here but in the constructor: declining would send such a model to the module path
+    why = device_refusal(inner)
+    if why:
+        return False, why
     for m in inner.modules():
         if isinstance(m, ReLoRaLinear) and m.bias is not None:
             return False, "biased projections use the module path"
@@ -77,12 +74,10 @@ def supports(model, args=None) -> Tuple[bool, str]:
 
 
 def supports_full_rank(model, args=None) -> Tuple[bool, str]:
-    """Whether the executor can train ``model`` (an unwrapped Llama) full-rank, and if not, why.  The device and dtype are
-    checked last, so every other reason is visible on a CPU model."""
-    if not isinstance(model, LlamaForCausalLM):
-        return False, "only Llama is fused for full-rank training"
-    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
-        return False, f"--frozen_dtype {args.frozen_dtype} has no frozen weights to act on in full-rank training"
+    """Whether the executor can train ``model`` (an unwrapped Llama) full-rank, and if not, why."""
+    why = full_rank_refusal(model, LlamaForCausalLM, "only Llama is fused for full-rank training", args)
+    if why:
+        return False, why
     cfg = model.config
     h, nh = cfg.hidden_size, cfg.num_attention_heads
     hd = h // nh
@@ -98,29 +93,20 @@ def supports_full_rank(model, args=None) -> Tuple[bool, str]:
         return False, f"hidden ({h}) is above the RMSNorm kernels' 8192"
     if hd % 8:
         return False, f"head_dim ({hd}) must be a multiple of 8 for the attention and RoPE kernels"
-    attention = getattr(args, "attention", "auto")
-    if attention == "native" and fused.attention_backend(hd, attention) != "native":
-        return False, f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM}, got {hd}"
+    why = native_attention_refusal(hd, args)
+    if why:
+        return False, why
     for m in model.modules():
         if isinstance(m, torch.nn.Linear) and m.bias is not None:
             return False, "biased projections use the module path"
-    p = next(model.parameters())
-    if not p.is_cuda or p.dtype != BF:
-        return False, "needs CUDA + bfloat16"
-    return True, "ok"
+    why = device_refusal(model)
+    return (False, why) if why else (True, "ok")
 
 
-class _Layer:
-    """Stacked views of one decoder layer's parameters and gradients (None where a mode has no such tensor: the LoRA factors
-    in full-rank training, the projection-weight gradients under ReLoRA)."""
-
+class _Layer(LayerViews):
     __slots__ = ("Wqkv", "Wo", "Wgu", "Wd", "A_qkv", "B_qkv", "A_o", "B_o", "A_gu", "B_gu", "A_d", "B_d", "w1", "w2",
                  "gA_qkv", "gB_qkv", "gA_o", "gB_o", "gA_gu", "gB_gu", "gA_d", "gB_d", "gw1", "gw2", "keys_qkv", "key_o",
                  "keys_gu", "key_d", "mods", "merge", "gWqkv", "gWo", "gWgu", "gWd")
-
-    def __init__(self):
-        for k in self.__slots__:
-            setattr(self, k, None)
 
 
 class FusedLlamaStepper(FusedStepperBase):
@@ -130,38 +116,22 @@ class FusedLlamaStepper(FusedStepperBase):
 
     def __init__(self, model, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
-                 transport: str = "nccl", native=None, symm_factory=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
+                 transport: str = "nccl", native=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
                  overlap_wgrad: bool = True, attention: str = "auto", fp8: bool = False, fp8_backward: bool = False,
                  deterministic: bool = False):
-        self.full = not isinstance(model, ReLoRaModel)
-        ok, why = supports_full_rank(model) if self.full else supports(model)
-        if not ok:
-            raise RuntimeError(why)
+        super().__init__(model, info, supports, supports_full_rank, grad_accumulation=grad_accumulation,
+                         clip_grad_norm=clip_grad_norm, cuda_graphs=cuda_graphs, ce_chunk=ce_chunk, overlap_wgrad=overlap_wgrad,
+                         attention=attention, deterministic=deterministic)
         if self.full and fp8:
             raise RuntimeError("--frozen_dtype fp8 has no frozen weights to act on in full-rank training")
         if fp8 and num_kv_heads(model.wrapped_model.config) != model.wrapped_model.config.num_attention_heads:
             raise RuntimeError("--frozen_dtype fp8 with grouped-query attention uses the module path (the fp8 weight copies are [3h, h])")
-        self.model, self.info = model, info
-        self.inner: LlamaForCausalLM = model if self.full else model.wrapped_model
-        self.C = fused._C()
-        self.ga = grad_accumulation
-        self.clip = clip_grad_norm
-        self.use_graphs = cuda_graphs
-        self.ce_chunk = ce_chunk
         cfg = self.inner.config
-        self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
-        self.hd = self.h // self.nh
         self.nkv = num_kv_heads(cfg)
         self.kv = self.nkv * self.hd  # width of the k and v projections (h without grouped-query attention)
         self.qkv_w = self.h + 2 * self.kv  # packed [q | k | v] row
         self.fp = (self.f + 127) // 128 * 128  # padded intermediate size (zero rows / columns keep every GEMM extent a multiple of the 128-wide tile)
-        self.r = 0 if self.full else model.r
-        self.L = cfg.num_hidden_layers
         self.eps = cfg.rms_norm_eps
-        self.p = 0.0 if self.full else float(model.lora_dropout)
-        self.scale = 1.0 if self.full else float(model.lora_alpha) / model.r
-        self.device = info.device
-        broadcast_params(model)
 
         # ---------------------------------------------------------------- stacked frozen weights (ReLoRA)
         dev = self.device
@@ -185,35 +155,20 @@ class FusedLlamaStepper(FusedStepperBase):
                     self._rehome(mlp.down_proj.weight, self.Wd[l][:, :f])
 
         # ---------------------------------------------------------------- flat trainable store (stack-friendly order)
-        named: List[Tuple[str, torch.nn.Parameter]] = []
-        name_of = {id(p): n for n, p in model.named_parameters()}
-
-        def add(p):
-            named.append((name_of[id(p)], p))
-
+        params: List[torch.nn.Parameter] = []
         for layer in layers:
             at, mlp = layer.self_attn, layer.mlp
             if self.full:
-                for m in (at.q_proj, at.k_proj, at.v_proj, at.o_proj, mlp.gate_proj, mlp.up_proj, mlp.down_proj):
-                    add(m.weight)
+                params += [m.weight for m in (at.q_proj, at.k_proj, at.v_proj, at.o_proj, mlp.gate_proj, mlp.up_proj, mlp.down_proj)]
             else:
-                for m in (at.q_proj, at.k_proj, at.v_proj):
-                    add(m.lora_A.weight)
-                for m in (at.q_proj, at.k_proj, at.v_proj):
-                    add(m.lora_B.weight)
-                add(at.o_proj.lora_A.weight); add(at.o_proj.lora_B.weight)
-                add(mlp.gate_proj.lora_A.weight); add(mlp.up_proj.lora_A.weight)
-                add(mlp.gate_proj.lora_B.weight); add(mlp.up_proj.lora_B.weight)
-                add(mlp.down_proj.lora_A.weight); add(mlp.down_proj.lora_B.weight)
-            add(layer.input_layernorm.weight); add(layer.post_attention_layernorm.weight)
-        add(self.inner.model.embed_tokens.weight)
-        add(self.inner.model.norm.weight)
-        add(self.inner.lm_head.weight)
-        seen = {id(p) for _, p in named}
-        extra = [(n, p) for n, p in model.named_parameters() if p.requires_grad and id(p) not in seen]
-        if extra:
-            raise RuntimeError(f"unexpected trainable parameters for the fused executor: {[n for n, _ in extra]}")
-        self._init_transport(info, transport)
+                params += [m.lora_A.weight for m in (at.q_proj, at.k_proj, at.v_proj)]
+                params += [m.lora_B.weight for m in (at.q_proj, at.k_proj, at.v_proj)]
+                params += [at.o_proj.lora_A.weight, at.o_proj.lora_B.weight]
+                params += [mlp.gate_proj.lora_A.weight, mlp.up_proj.lora_A.weight]
+                params += [mlp.gate_proj.lora_B.weight, mlp.up_proj.lora_B.weight]
+                params += [mlp.down_proj.lora_A.weight, mlp.down_proj.lora_B.weight]
+            params += [layer.input_layernorm.weight, layer.post_attention_layernorm.weight]
+        params += [self.inner.model.embed_tokens.weight, self.inner.model.norm.weight, self.inner.lm_head.weight]
         padded: Dict[int, Tuple[int, int]] = {}
         if fp != f:
             for layer in layers:
@@ -226,7 +181,7 @@ class FusedLlamaStepper(FusedStepperBase):
                 padded[id(mlp.gate_proj.lora_B.weight)] = (fp, r)
                 padded[id(mlp.up_proj.lora_B.weight)] = (fp, r)
                 padded[id(mlp.down_proj.lora_A.weight)] = (r, fp)
-        self._init_store(named, padded)
+        self._build_store(params, transport, padded)
         pv = self._stacked_view  # stacked view over `rows_mult` adjacent parameters (params and grads)
 
         self.layers: List[_Layer] = []
@@ -283,7 +238,6 @@ class FusedLlamaStepper(FusedStepperBase):
 
         # ---------------------------------------------------------------- optimizer / comm
         self._init_optimizer(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, zero=zero, native=native)
-        self._attn_saved: List = []
         # ---- fp8 frozen-weight path: E4M3 copies of the stacked weights + per-site activation scales (csrc/fp8.cu)
         self.fp8 = not self.full and (bool(fp8) or os.environ.get("RELORA_B200_FP8", "0") == "1")
         if self.fp8:
@@ -305,27 +259,14 @@ class FusedLlamaStepper(FusedStepperBase):
             self._fp8_calibrated = False
             self._quantize_weights()
         self._fp8_calibrating = False
-        if not self.fp8:
-            self.fp8_bwd = False
-        attention = os.environ.get("RELORA_B200_ATTENTION", attention)
-        # auto: this repo's wgmma kernels (csrc/attention.cu) for head_dim <= 64 -- the hot path then contains no library
-        # attention call -- and torch SDPA (cuDNN) above; native: the kernels up to head_dim 256; sdpa: torch SDPA
-        # (bench/attn_bench.py times both)
-        self.native_attn = fused.attention_backend(self.hd, attention) == "native"
-        if attention == "native" and not self.native_attn:
-            raise RuntimeError(f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM} (multiple of 8), "
-                               f"got {self.hd}")
-        self.side = torch.cuda.Stream(device=dev) if overlap_wgrad else None
         self.fused_dx = os.environ.get("RELORA_B200_FUSED_DX", "1") != "0"
         # stacked output width from which dx uses two kernels (frozen-path GEMM on 256-wide tiles + a mask-and-add pass) instead of
         # the one-kernel form; the thresholds (4096 bf16, 2048 with fp8 input-gradient GEMMs) have not been re-tuned on the H100.
-        self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0")) or (2048 if self.fp8_bwd else 4096)
+        self.dx_split_k = self.dx_split_k or (2048 if self.fp8_bwd else 4096)
         # --deterministic: the stacked dA / dB weight-gradient GEMMs run without split-K (one CTA owns an output tile for the whole token
         # reduction: fixed summation order instead of fp32 atomics from several CTAs).  Remaining order-dependent reductions are the
         # [h]-sized norm-weight gradients (block partials combined with vector atomics).
-        self.wgrad_split_k = 1 if (deterministic or os.environ.get("RELORA_B200_DETERMINISTIC", "0") == "1") else 0
-        # embedding backward without atomics (default); RELORA_B200_ATOMIC_EMBEDDING=1 selects the atomicAdd scatter
-        self.deterministic_embedding = os.environ.get("RELORA_B200_ATOMIC_EMBEDDING", "0") != "1"
+        self.wgrad_split_k = 1 if self.deterministic else 0
 
     # ------------------------------------------------------------------ plumbing
     @staticmethod
@@ -343,14 +284,9 @@ class FusedLlamaStepper(FusedStepperBase):
                                            self.w_inv_scale[l, s_i:s_i + 1], self.W8T[s_i][l] if self.fp8_bwd else None)
         self._w_scale2[1].copy_(self._w_scale2[0])
 
-    def _alloc(self, B: int, T: int):
-        dev, h, f, r, L = self.device, self.h, self.fp, self.r, self.L  # f: padded intermediate size
-        M = B * T
+    def _alloc_layers(self, B: int, T: int):
+        dev, h, f, r, L, M = self.device, self.h, self.fp, self.r, self.L, self.M_  # f: padded intermediate size
         e = lambda *s: torch.empty(*s, dtype=BF, device=dev)  # noqa: E731
-        self.B_, self.T_, self.M_ = B, T, M
-        self.ids = torch.zeros(B, T, dtype=torch.long, device=dev)
-        self.labels = torch.zeros(M, dtype=torch.long, device=dev)
-        self.x_in = e(L + 1, M, h)
         self.x1 = e(L, M, h)
         self.rstd1 = torch.empty(L, M, dtype=torch.float32, device=dev)
         self.rstd2 = torch.empty(L, M, dtype=torch.float32, device=dev)
@@ -389,17 +325,7 @@ class FusedLlamaStepper(FusedStepperBase):
             self.x8_f = torch.empty(M, f, dtype=torch.uint8, device=dev)
             if self.fp8_bwd:
                 self.dy8 = {w: torch.empty(M, w, dtype=torch.uint8, device=dev) for w in {h, 3 * h, 2 * f}}
-        if self.native_attn:
-            self.attn_o = e(L, M, h)
-            self.lse = torch.empty(L, B, self.nh, T, dtype=torch.float32, device=dev)
-            self.delta = torch.empty(B, self.nh, T, dtype=torch.float32, device=dev)
         self.parts = None if self.full else e(M, max(3 * h, f))
-        ldv = (self.V + 7) // 8 * 8
-        self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
-        self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.count = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
-        self._shape = (B, T)
 
     # ------------------------------------------------------------------ forward + backward of one micro-batch
     def _attention(self, qkv: torch.Tensor, train: bool, sl: int = 0):
@@ -421,14 +347,7 @@ class FusedLlamaStepper(FusedStepperBase):
             v3 = qkv.view(B, T, nh + 2 * self.nkv, hd)
             q, k, v = (v3[:, :, a:b].transpose(1, 2) for a, b in ((0, nh), (nh, nh + self.nkv), (nh + self.nkv, nh + 2 * self.nkv)))
             gqa = {"enable_gqa": True}
-        if train:
-            q, k, v = (t.detach().requires_grad_() for t in (q, k, v))
-            with torch.enable_grad():
-                o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **gqa)
-            self._attn_saved.append((o, q, k, v))
-        else:
-            o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **gqa)
-        return o.detach().transpose(1, 2).reshape(self.M_, self.h)
+        return self._sdpa(q, k, v, train, **gqa).transpose(1, 2).reshape(self.M_, self.h)
 
     def _q8(self, l, s_i, K):
         """(q8, inv_scale, amax_cur) arguments that make a producer kernel also emit the E4M3 copy of its output."""
@@ -440,12 +359,11 @@ class FusedLlamaStepper(FusedStepperBase):
         C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
         p = self.p if train else 0.0
         seed = self.seed
+        if train and self.fp8 and not self._fp8_calibrating:
+            self._fp8_prep()
         C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
         self._attn_saved.clear()
-        for l, S in enumerate(self.layers):
-            sl = l if train else 0
-            x = self.x_in[l] if train else self.x_in[l % 2]
-            x_next = self.x_in[l + 1] if train else self.x_in[(l + 1) % 2]
+        for l, S, sl, x, x_next in self._layer_slots(train):
             x1 = self.x1[sl]
             qkv, gu = self.qkv[sl], self.gu[sl]
             # ---- attention block
@@ -489,9 +407,8 @@ class FusedLlamaStepper(FusedStepperBase):
                 if train:
                     self.xd_d[sl].copy_(self.hmid)
             self._lora_group_fwd(self.hmid, xd_d, S.A_d, S.B_d, S.Wd, self.u_d[sl], x_next, G=1, K=f, Ng=h, residual=x1, site=(l, 3), prequant=True)
-        x_last = self.x_in[self.L] if train else self.x_in[self.L % 2]
-        C.rmsnorm_fwd(x_last, self.w_norm, self.xf, self.rstd_f, self.eps, None, None, [], 0.0)
-        return x_last
+        C.rmsnorm_fwd(x_next, self.w_norm, self.xf, self.rstd_f, self.eps, None, None, [], 0.0)
+        return x_next
 
     def _backward(self):
         C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
@@ -525,8 +442,7 @@ class FusedLlamaStepper(FusedStepperBase):
                 C.rope_inplace(self.dqkv, T, nh + self.nkv, hd, hd, self.cos, self.sin, True, 0)  # back through the rotation of q, k
                 dq = None
             else:
-                o, q, k, v = self._attn_saved[l]
-                dq, dk, dv = torch.autograd.grad(o, (q, k, v), self.dattn.view(B, T, nh, hd).transpose(1, 2))
+                dq, dk, dv = self._sdpa_bwd(l)
                 self._join("qkv")  # the previous layer's qkv weight gradients read dqkv / du_qkv
             if dq is None:
                 pass
@@ -547,15 +463,9 @@ class FusedLlamaStepper(FusedStepperBase):
             self._join("d")  # this layer's down_proj weight gradients read the buffer written next
             C.rmsnorm_bwd(self.dxn2, self.x_in[l], S.w1, self.rstd1[l], dx, dx_other, S.gw1, ws, tk)
             dx, dx_other = dx_other, dx
-        if self.deterministic_embedding:
-            # stable sort of the token ids (12 K keys) -> one writer per table row, fixed summation order: bit-reproducible
-            sorted_ids, perm = torch.sort(self.ids.view(-1), stable=True)
-            C.embedding_bwd_sorted(sorted_ids, perm, dx, self.gW_emb, self.pad_idx)
-        else:
-            C.embedding_bwd(self.ids.view(-1), dx, self.gW_emb, self.pad_idx)
-        for tag in ("d", "gu", "o", "qkv"):
-            self._join(tag)
-        self._attn_saved.clear()
+        self._embedding_bwd_and_join(dx, ("d", "gu", "o", "qkv"))
+        if self.fp8_bwd:
+            self._fp8_bwd_calibrated = True  # the first backward ran in bf16 and recorded the gradient amax of every site
 
     def _fp8_calibrate(self):
         """Bootstrap of the delayed activation scales: one bf16 forward that only *records* every site's amax.  (Starting the
@@ -568,17 +478,10 @@ class FusedLlamaStepper(FusedStepperBase):
             self._fp8_calibrating = False
         self._fp8_calibrated = True
 
-    def _micro_body(self):
-        self._set_labels()
-        if self.fp8:  # rotate the activation amax state, derive this micro-step's scales
-            self.C.fp8_prep(self._act_state2, self._w_scale2, self._inv_sx2, self._alpha_main2, self._alpha_inv2, self.fp8_margin,
-                            4 * self.L)
-        self._forward(True)
-        self._loss_and_head_backward(True)
-        self._backward()
-        if self.fp8_bwd:
-            self._fp8_bwd_calibrated = True  # the first backward ran in bf16 and recorded the gradient amax of every site
-        self.C.seed_advance(self.seed)
+    def _fp8_prep(self):
+        """Rotates the activation amax state and derives the scales of a micro-step (a training forward starts with it)."""
+        self.C.fp8_prep(self._act_state2, self._w_scale2, self._inv_sx2, self._alpha_main2, self._alpha_inv2, self.fp8_margin,
+                        4 * self.L)
 
     # ------------------------------------------------------------------ public stepper interface
     def _before_micro(self):
@@ -589,16 +492,12 @@ class FusedLlamaStepper(FusedStepperBase):
         if self.fp8 and not self._fp8_calibrated:
             # evaluation before the first training step: bootstrap the activation scales exactly like micro_step does
             self._fp8_calibrate()
-            self.C.fp8_prep(self._act_state2, self._w_scale2, self._inv_sx2, self._alpha_main2, self._alpha_inv2, self.fp8_margin,
-                            4 * self.L)
-        self._forward(False)
-        self._loss_and_head_backward(False)
+            self._fp8_prep()
+        super()._eval_body()
 
     @torch.no_grad()
     def merge_and_reinit(self):
-        """W += s·B@A on the stacked buffers (wgmma GEMM accumulating into W in fp32), then hash re-init."""
-        if self.full:
-            raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
-        self._merge_modules([blk for S in self.layers for blk in zip(S.mods, S.merge)])
+        """The merge of every stacked block (see the base class), then the E4M3 copies of the merged weights."""
+        super().merge_and_reinit()
         if self.fp8:
             self._quantize_weights()

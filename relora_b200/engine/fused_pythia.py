@@ -28,107 +28,69 @@ Sequential residual: x1 = x + dense(attn(LN1 x)) + b_o ;  x_next = x1 + mlp(LN2 
 from __future__ import annotations
 
 import math
-import os
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F_
 
 from ..models.pythia import GPTNeoXForCausalLM
-from ..ops import fused
 from ..parallel.dist import DistInfo
-from ..parallel.grad_sync import broadcast_params
-from ..relora import ReLoRaModel
-from .fused_common import FusedStepperBase
+from .fused_common import (FusedStepperBase, LayerViews, device_refusal, full_rank_refusal, native_attention_refusal,
+                           relora_refusal)
 
 BF = torch.bfloat16
 MAX_HIDDEN = 2048  # the executor LayerNorm backward keeps its block partials of five [H] vectors in 48 KB of shared memory
 
 
-def supports(model, args=None) -> Tuple[bool, str]:
-    """(True, "ok") when the Pythia executor can train ``model``, else (False, why).  The configuration is checked before the device,
-    so the reason does not depend on where the model lives."""
-    if not isinstance(model, ReLoRaModel):
-        return False, "full-rank training uses the module path"
-    inner = model.wrapped_model
-    if not isinstance(inner, GPTNeoXForCausalLM):
-        return False, "not a GPT-NeoX (Pythia) model"
-    if model.lora_only or model.trainable_scaling or model._config.quantize is not None:
-        return False, "lora_only / trainable scaling / quantized frozen weights use the module path"
-    if args is not None and getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
-        return False, "fp8 frozen weights are not supported for Pythia"
-    cfg = inner.config
+def _neox_refusal(model, r=None) -> Optional[str]:
+    """Why the executor declines the GPT-NeoX ``model`` (LoRA rank ``r``; None in full-rank training) for its configuration, or
+    None."""
+    cfg = model.config
     if float(getattr(cfg, "hidden_dropout", 0.0)) != 0.0 or float(getattr(cfg, "attention_dropout", 0.0)) != 0.0:
-        return False, "hidden / attention dropout must be 0"
-    layer0 = inner.gpt_neox.layers[0]
+        return "hidden / attention dropout must be 0"
+    layer0 = model.gpt_neox.layers[0]
     if not isinstance(layer0.mlp.act, nn.GELU):
-        return False, "only the GELU activation is fused"
-    h, f, nh, r = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, model.r
-    if h % 128 or r % 128 or f % 128:
-        return False, f"hidden ({h}), intermediate ({f}) and rank ({r}) must be multiples of 128"
+        return "only the GELU activation is fused"
+    h, f, nh = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads
+    if r is None and (h % 128 or f % 128):
+        return f"hidden ({h}) and intermediate ({f}) must be multiples of 128"
+    if r is not None and (h % 128 or r % 128 or f % 128):
+        return f"hidden ({h}), intermediate ({f}) and rank ({r}) must be multiples of 128"
     if h > MAX_HIDDEN:
-        return False, f"hidden ({h}) must be <= {MAX_HIDDEN} (LayerNorm kernel limit)"
+        return f"hidden ({h}) must be <= {MAX_HIDDEN} (LayerNorm kernel limit)"
     hd = h // nh
     if hd % 8:
-        return False, "head_dim must be a multiple of 8"
+        return f"head_dim ({hd}) must be a multiple of 8 for the attention and rotary kernels"
     if layer0.attention.rotary_ndims % 2:
-        return False, "the number of rotary dims must be even"
+        return "the number of rotary dims must be even"
     at, mlp = layer0.attention, layer0.mlp
     if any(m.bias is None for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)):
-        return False, "projections without bias use the module path"
-    p = next(inner.parameters())
-    if not p.is_cuda or p.dtype != BF:
-        return False, "needs CUDA + bfloat16"
-    return True, "ok"
+        return "projections without bias use the module path"
+    return None
+
+
+def supports(model, args=None) -> Tuple[bool, str]:
+    """(True, "ok") when the Pythia executor can train ``model``, else (False, why)."""
+    why = relora_refusal(model, GPTNeoXForCausalLM, "not a GPT-NeoX (Pythia) model")
+    if why is None and getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        why = "fp8 frozen weights are not supported for Pythia"
+    why = why or _neox_refusal(model.wrapped_model, model.r) or device_refusal(model.wrapped_model)
+    return (False, why) if why else (True, "ok")
 
 
 def supports_full_rank(model, args=None) -> Tuple[bool, str]:
-    """Whether the executor can train ``model`` (an unwrapped GPT-NeoX) full-rank, and if not, why.  The device and dtype are
-    checked last, so every other reason is visible on a CPU model."""
-    if not isinstance(model, GPTNeoXForCausalLM):
-        return False, "only GPT-NeoX (Pythia) is fused for full-rank training here"
-    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
-        return False, f"--frozen_dtype {args.frozen_dtype} has no frozen weights to act on in full-rank training"
-    cfg = model.config
-    if float(getattr(cfg, "hidden_dropout", 0.0)) != 0.0 or float(getattr(cfg, "attention_dropout", 0.0)) != 0.0:
-        return False, "hidden / attention dropout must be 0"
-    layer0 = model.gpt_neox.layers[0]
-    if not isinstance(layer0.mlp.act, nn.GELU):
-        return False, "only the GELU activation is fused"
-    h, f, nh = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads
-    if h % 128 or f % 128:
-        return False, f"hidden ({h}) and intermediate ({f}) must be multiples of 128"
-    if h > MAX_HIDDEN:
-        return False, f"hidden ({h}) must be <= {MAX_HIDDEN} (LayerNorm kernel limit)"
-    hd = h // nh
-    if hd % 8:
-        return False, f"head_dim ({hd}) must be a multiple of 8 for the attention and rotary kernels"
-    if layer0.attention.rotary_ndims % 2:
-        return False, "the number of rotary dims must be even"
-    at, mlp = layer0.attention, layer0.mlp
-    if any(m.bias is None for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)):
-        return False, "projections without bias use the module path"
-    attention = getattr(args, "attention", "auto")
-    if attention == "native" and fused.attention_backend(hd, attention) != "native":
-        return False, f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM}, got {hd}"
-    p = next(model.parameters())
-    if not p.is_cuda or p.dtype != BF:
-        return False, "needs CUDA + bfloat16"
-    return True, "ok"
+    """Whether the executor can train ``model`` (an unwrapped GPT-NeoX) full-rank, and if not, why."""
+    why = full_rank_refusal(model, GPTNeoXForCausalLM, "only GPT-NeoX (Pythia) is fused for full-rank training here", args)
+    why = why or _neox_refusal(model) or native_attention_refusal(model.config.hidden_size // model.config.num_attention_heads, args)
+    why = why or device_refusal(model)
+    return (False, why) if why else (True, "ok")
 
 
-class _Layer:
-    """Views of one GPT-NeoX layer's parameters and gradients (None where a mode has no such tensor: the LoRA factors in full-rank
-    training, the projection-weight gradients under ReLoRA)."""
-
+class _Layer(LayerViews):
     __slots__ = ("W_qkv", "W_o", "W_h", "W_4", "A_qkv", "B_qkv", "b_qkv", "A_o", "B_o", "b_o", "A_h", "B_h", "b_h", "A_4", "B_4", "b_4",
                  "w1", "c1", "w2", "c2", "gA_qkv", "gB_qkv", "gb_qkv", "gA_o", "gB_o", "gb_o", "gA_h", "gB_h", "gb_h", "gA_4", "gB_4",
-                 "gb_4", "gw1", "gc1", "gw2", "gc2", "key_qkv", "key_o", "key_h", "key_4", "mods", "gW_qkv", "gW_o", "gW_h", "gW_4")
-
-    def __init__(self):
-        for k in self.__slots__:
-            setattr(self, k, None)
+                 "gb_4", "gw1", "gc1", "gw2", "gc2", "key_qkv", "key_o", "key_h", "key_4", "mods", "merge", "gW_qkv", "gW_o", "gW_h",
+                 "gW_4")
 
 
 class FusedPythiaStepper(FusedStepperBase):
@@ -138,29 +100,11 @@ class FusedPythiaStepper(FusedStepperBase):
 
     def __init__(self, model, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
-                 transport: str = "nccl", native=None, symm_factory=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
+                 transport: str = "nccl", native=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
                  overlap_wgrad: bool = True, attention: str = "auto", deterministic: bool = False):
-        self.full = not isinstance(model, ReLoRaModel)
-        ok, why = supports_full_rank(model) if self.full else supports(model)
-        if not ok:
-            raise RuntimeError(why)
-        self.model, self.info = model, info
-        self.inner: GPTNeoXForCausalLM = model if self.full else model.wrapped_model
-        self.C = fused._C()
-        self.ga = grad_accumulation
-        self.clip = clip_grad_norm
-        self.use_graphs = cuda_graphs
-        self.ce_chunk = ce_chunk
-        cfg = self.inner.config
-        self.h, self.f, self.nh, self.V = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.vocab_size
-        self.hd = self.h // self.nh
-        self.r = 0 if self.full else model.r
-        self.L = cfg.num_hidden_layers
-        self.p = 0.0 if self.full else float(model.lora_dropout)
-        self.scale = 1.0 if self.full else float(model.lora_alpha) / model.r
-        self.device = info.device
-        self.fp8 = self.fp8_bwd = False
-        broadcast_params(model)
+        super().__init__(model, info, supports, supports_full_rank, grad_accumulation=grad_accumulation,
+                         clip_grad_norm=clip_grad_norm, cuda_graphs=cuda_graphs, ce_chunk=ce_chunk, overlap_wgrad=overlap_wgrad,
+                         attention=attention, deterministic=deterministic)
         neox = self.inner.gpt_neox
         layers = neox.layers
         self.parallel = bool(layers[0].use_parallel_residual)
@@ -172,30 +116,15 @@ class FusedPythiaStepper(FusedStepperBase):
         self.rotary = at0.rotary_emb
 
         # ---------------------------------------------------------------- flat trainable store
-        named: List[Tuple[str, torch.nn.Parameter]] = []
-        name_of = {id(p): n for n, p in model.named_parameters()}
-
-        def add(p):
-            named.append((name_of[id(p)], p))
-
+        params: List[torch.nn.Parameter] = []
         for layer in layers:
             at, mlp = layer.attention, layer.mlp
             for m in (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h):
-                if self.full:
-                    add(m.weight); add(m.bias)
-                else:
-                    add(m.lora_A.weight); add(m.lora_B.weight); add(m.bias)
+                params += [m.weight, m.bias] if self.full else [m.lora_A.weight, m.lora_B.weight, m.bias]
             for ln in (layer.input_layernorm, layer.post_attention_layernorm):
-                add(ln.weight); add(ln.bias)
-        add(neox.embed_in.weight)
-        add(neox.final_layer_norm.weight); add(neox.final_layer_norm.bias)
-        add(self.inner.embed_out.weight)
-        seen = {id(p) for _, p in named}
-        extra = [(n, p) for n, p in model.named_parameters() if p.requires_grad and id(p) not in seen]
-        if extra:
-            raise RuntimeError(f"unexpected trainable parameters for the fused executor: {[n for n, _ in extra]}")
-        self._init_transport(info, transport)
-        self._init_store(named)
+                params += [ln.weight, ln.bias]
+        params += [neox.embed_in.weight, neox.final_layer_norm.weight, neox.final_layer_norm.bias, self.inner.embed_out.weight]
+        self._build_store(params, transport)
         pv = self._stacked_view
 
         self.layers: List[_Layer] = []
@@ -227,41 +156,29 @@ class FusedPythiaStepper(FusedStepperBase):
             S.w2, S.gw2 = pv(layer.post_attention_layernorm.weight)
             S.c2, S.gc2 = pv(layer.post_attention_layernorm.bias)
             S.mods = (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)
+            if not self.full:  # (B, A, W) blocks of the merge GEMM  W += s·B·A
+                S.merge = [(m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data) for m in S.mods]
             self.layers.append(S)
         self.W_emb, self.gW_emb = pv(neox.embed_in.weight)
+        self.pad_idx = -1
         self.w_norm, self.gw_norm = pv(neox.final_layer_norm.weight)
         self.c_norm, self.gc_norm = pv(neox.final_layer_norm.bias)
         self.W_head, self.gW_head = pv(self.inner.embed_out.weight)
 
         # ---------------------------------------------------------------- optimizer / comm
         self._init_optimizer(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, zero=zero, native=native)
-        self._attn_saved: List = []
-        attention = os.environ.get("RELORA_B200_ATTENTION", attention)
-        self.native_attn = fused.attention_backend(self.hd, attention) == "native"
-        if attention == "native" and not self.native_attn:
-            raise RuntimeError(f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM} (multiple of 8), "
-                               f"got {self.hd}")
-        self.side = torch.cuda.Stream(device=self.device) if overlap_wgrad else None
-        self.fused_dx = True
-        self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0")) or 4096
-        # --deterministic (full-rank training only): the weight-gradient GEMMs run without split-K, so one CTA owns an output tile
-        # for the whole token reduction.  The 1-D gradients (LayerNorm γ / β and the projection biases) stay column sums whose
-        # block partials meet in fp32 atomics.
-        det = deterministic or os.environ.get("RELORA_B200_DETERMINISTIC", "0") == "1"
-        self.wgrad_split_k = 1 if (self.full and det) else 0
-        self.deterministic_embedding = os.environ.get("RELORA_B200_ATOMIC_EMBEDDING", "0") != "1"
+        self.dx_split_k = self.dx_split_k or 4096
+        # --deterministic (full-rank training only; ReLoRA ignores it): the weight-gradient GEMMs run without split-K, so one CTA owns
+        # an output tile for the whole token reduction.  The 1-D gradients (LayerNorm γ / β and the projection biases) stay column
+        # sums whose block partials meet in fp32 atomics.
+        self.wgrad_split_k = 1 if (self.full and self.deterministic) else 0
 
     # ------------------------------------------------------------------ buffers
-    def _alloc(self, B: int, T: int):
-        dev, h, f, r, L = self.device, self.h, self.f, self.r, self.L
-        M = B * T
+    def _alloc_layers(self, B: int, T: int):
+        dev, h, f, r, L, M = self.device, self.h, self.f, self.r, self.L, self.M_
         e = lambda *s: torch.empty(*s, dtype=BF, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-        self.B_, self.T_, self.M_ = B, T, M
-        self.ids = torch.zeros(B, T, dtype=torch.long, device=dev)
-        self.labels = torch.zeros(M, dtype=torch.long, device=dev)
         # saved for the backward, one slot per layer ([0] only in evaluation)
-        self.x_in = e(L + 1, M, h)
         self.mean1, self.rstd1 = f32(L, M), f32(L, M)
         self.xd1, self.xd2 = e(L, M, h), e(L, M, h)  # LoRA inputs of query_key_value / dense_h_to_4h (the norms' outputs when p = 0)
         self.qkv = e(L, M, 3 * h)                    # post-rotary, head-interleaved
@@ -275,10 +192,6 @@ class FusedPythiaStepper(FusedStepperBase):
         if not self.parallel:
             self.x1 = e(L, M, h)
             self.mean2, self.rstd2 = f32(L, M), f32(L, M)
-        if self.native_attn:
-            self.attn_o = e(L, M, h)
-            self.lse = f32(L, B, self.nh, T)
-            self.delta = f32(B, self.nh, T)
         # transients
         self.xn1, self.xn2, self.attn_t, self.x1_t = e(M, h), e(M, h), e(M, h), e(M, h)
         self.a = e(M, f)
@@ -292,17 +205,11 @@ class FusedPythiaStepper(FusedStepperBase):
         else:
             self.tmp_h, self.tmp_f = e(M, h), e(M, f)
             self.du_bufs = {"4": e(M, r), "h": e(M, r), "o": e(M, r), "qkv": e(M, r)}
-        ldv = (self.V + 7) // 8 * 8
-        self.logits = torch.zeros(min(self.ce_chunk, M), ldv, dtype=BF, device=dev)
-        self.loss_sum = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.count = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         # rotary tables of the module (linear / dynamic-NTK scaling, T beyond max_position_embeddings), fp32 [T, rot]
         if self.rot > 0:
             cos, sin = self.rotary(self.x_in, seq_len=T)
             self.cos = cos[0, 0, :T].float().contiguous()
             self.sin = sin[0, 0, :T].float().contiguous()
-        self._shape = (B, T)
 
     # ------------------------------------------------------------------ forward
     def _attention(self, qkv: torch.Tensor, train: bool, sl: int, out: torch.Tensor):
@@ -312,14 +219,7 @@ class FusedPythiaStepper(FusedStepperBase):
             return out
         v5 = qkv.view(B, T, nh, 3, hd)
         q, k, v = (v5[:, :, :, i].transpose(1, 2) for i in range(3))
-        if train:
-            q, k, v = (t.detach().requires_grad_() for t in (q, k, v))
-            with torch.enable_grad():
-                o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True)
-            self._attn_saved.append((o, q, k, v))
-        else:
-            o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True)
-        out.view(B, T, nh, hd).copy_(o.detach().transpose(1, 2))
+        out.view(B, T, nh, hd).copy_(self._sdpa(q, k, v, train).transpose(1, 2))
         return out
 
     def _norms(self, x, S, l, sl, train, p, both: bool, second_of=None):
@@ -356,10 +256,7 @@ class FusedPythiaStepper(FusedStepperBase):
         seed = self.seed
         C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
         self._attn_saved.clear()
-        for l, S in enumerate(self.layers):
-            sl = l if train else 0
-            x = self.x_in[l] if train else self.x_in[l % 2]
-            x_next = self.x_in[l + 1] if train else self.x_in[(l + 1) % 2]
+        for l, S, sl, x, x_next in self._layer_slots(train):
             qkv = self.qkv[sl]
             normed = self._norms(x, S, l, sl, train, p, both=self.parallel)
             xn1, xd1 = normed[0]
@@ -392,9 +289,8 @@ class FusedPythiaStepper(FusedStepperBase):
                 C.gelu_fwd(z, a, self.tanh)
                 xd_4 = a
             self._lora_group_fwd(a, xd_4, S.A_4, S.B_4, S.W_4, self.u_4[sl], x_next, G=1, K=f, Ng=h, residual=x1, bias=S.b_4)
-        x_last = self.x_in[self.L] if train else self.x_in[self.L % 2]
-        C.layernorm_fwd(x_last, self.w_norm, self.c_norm, self.xf, self.mean_f, self.rstd_f, self.eps_f)
-        return x_last
+        C.layernorm_fwd(x_next, self.w_norm, self.c_norm, self.xf, self.mean_f, self.rstd_f, self.eps_f)
+        return x_next
 
     # ------------------------------------------------------------------ backward
     def _backward(self):
@@ -427,8 +323,7 @@ class FusedPythiaStepper(FusedStepperBase):
                 C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
                                 1.0 / math.sqrt(hd), interleaved=True)
             else:
-                o, q, k, v = self._attn_saved[l]
-                dq, dk, dv = torch.autograd.grad(o, (q, k, v), self.dattn.view(B, T, nh, hd).transpose(1, 2))
+                dq, dk, dv = self._sdpa_bwd(l)
                 self._join("qkv")
                 d5 = self.dqkv.view(B, T, nh, 3, hd)
                 for i, d in enumerate((dq, dk, dv)):
@@ -447,29 +342,4 @@ class FusedPythiaStepper(FusedStepperBase):
                 C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[l], self.rstd1[l], dx_other, S.gw1, S.gc1, dres=dx,
                                 dres_sum=S.gb_o)
             dx, dx_other = dx_other, dx
-        if self.deterministic_embedding:
-            sorted_ids, perm = torch.sort(self.ids.view(-1), stable=True)
-            C.embedding_bwd_sorted(sorted_ids, perm, dx, self.gW_emb, -1)
-        else:
-            C.embedding_bwd(self.ids.view(-1), dx, self.gW_emb, -1)
-        for tag in ("4", "h", "o", "qkv"):
-            self._join(tag)
-        self._attn_saved.clear()
-
-    def _micro_body(self):
-        self._set_labels()
-        self._forward(True)
-        self._loss_and_head_backward(True)
-        self._backward()
-        self.C.seed_advance(self.seed)
-
-    def _eval_body(self):
-        self._forward(False)
-        self._loss_and_head_backward(False)
-
-    @torch.no_grad()
-    def merge_and_reinit(self):
-        """W += s·B@A per module (wgmma GEMM accumulating into W in fp32), then the hash re-init of the module path."""
-        if self.full:
-            raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
-        self._merge_modules([(m, (m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data)) for S in self.layers for m in S.mods])
+        self._embedding_bwd_and_join(dx, ("4", "h", "o", "qkv"))

@@ -11,7 +11,9 @@ gradient all-reduce hoisted out of the accumulation loop.  :class:`ModuleStepper
 ``nn.Module`` whose forward returns ``.loss`` (CPU/gloo and the generic GPU path);
 :class:`relora_b200.engine.fused_llama.FusedLlamaStepper` and
 :class:`relora_b200.engine.fused_pythia.FusedPythiaStepper` are the H100 executors (whole-layer fused
-kernels, CUDA graphs) with the same interface.
+kernels, CUDA graphs) with the same interface, built on :class:`relora_b200.engine.fused_common.FusedStepperBase`.
+:func:`make_stepper` picks the executor: the module's ``supports`` / ``supports_full_rank`` decide, then
+one constructor call builds it.
 """
 from __future__ import annotations
 
@@ -56,7 +58,6 @@ class ModuleStepper:
         zero: bool = False,
         transport: str = "nccl",
         native=None,
-        symm_factory=None,
     ):
         self.model, self.info = model, info
         self.ga = grad_accumulation
@@ -172,7 +173,7 @@ def peer_memory_update(st, *, grads_f32, skip, error_if_nonfinite: bool, local_l
     return UpdateInfo(total, False, mean_loss=mean_loss, skip_count=skip_count)
 
 
-def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None):
+def make_stepper(model, info: DistInfo, args, *, native=None):
     """Pick the executor for ``model`` on ``info.device`` according to ``--engine``."""
     engine = getattr(args, "engine", "auto")
     zero = str(args.optimizer).lower() == "adam_zero"
@@ -186,45 +187,34 @@ def make_stepper(model, info: DistInfo, args, *, native=None, symm_factory=None)
         zero=zero,
         transport=transport,
         native=native,
-        symm_factory=symm_factory,
     )
     if engine in ("auto", "fused") and info.device.type == "cuda":
-        from .fused_llama import FusedLlamaStepper, supports
+        from ..models.llama import LlamaForCausalLM
+        from ..models.pythia import GPTNeoXForCausalLM
+        from . import fused_llama, fused_pythia
 
-        ok, why = supports(model, args)
-        if ok:
-            return FusedLlamaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
-                                     attention=getattr(args, "attention", "auto"),
-                                     fp8=getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"),
-                                     fp8_backward=getattr(args, "frozen_dtype", None) == "fp8_full",
-                                     deterministic=bool(getattr(args, "deterministic", False)), **kw)
-        if engine == "fused":
+        frozen = getattr(args, "frozen_dtype", None)
+        ok, why = fused_llama.supports(model, args)
+        cls = fused_llama.FusedLlamaStepper if ok else None
+        if cls is None and engine == "fused":
             # Pythia (GPT-NeoX) and full-rank Llama run fused only on request; `auto` keeps both on the module path
-            from ..models.llama import LlamaForCausalLM
-            from ..models.pythia import GPTNeoXForCausalLM
-            from .fused_llama import supports_full_rank
-            from .fused_pythia import FusedPythiaStepper, supports as pythia_supports, supports_full_rank as pythia_supports_full_rank
-
-            if isinstance(model, LlamaForCausalLM):
-                ok, why = supports_full_rank(model, args)
-                if ok:
-                    return FusedLlamaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
-                                             attention=getattr(args, "attention", "auto"),
-                                             deterministic=bool(getattr(args, "deterministic", False)), **kw)
-                raise RuntimeError(f"--engine fused requested but not applicable: {why}")
-            if isinstance(model, GPTNeoXForCausalLM):
-                ok, why = pythia_supports_full_rank(model, args)
-                if ok:
-                    return FusedPythiaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
-                                              attention=getattr(args, "attention", "auto"),
-                                              deterministic=bool(getattr(args, "deterministic", False)), **kw)
-                raise RuntimeError(f"--engine fused requested but not applicable: {why}")
-            ok, why_p = pythia_supports(model, args)
-            if ok:
-                return FusedPythiaStepper(model, info, cuda_graphs=getattr(args, "cuda_graphs", True),
-                                          attention=getattr(args, "attention", "auto"), **kw)
             inner = getattr(model, "wrapped_model", model)
-            raise RuntimeError(f"--engine fused requested but not applicable: {why_p if isinstance(inner, GPTNeoXForCausalLM) else why}")
+            if isinstance(model, LlamaForCausalLM):
+                cls, check = fused_llama.FusedLlamaStepper, fused_llama.supports_full_rank
+            elif isinstance(model, GPTNeoXForCausalLM):
+                cls, check = fused_pythia.FusedPythiaStepper, fused_pythia.supports_full_rank
+            else:
+                cls, check = fused_pythia.FusedPythiaStepper, fused_pythia.supports
+            ok, why_fused = check(model, args)
+            if not ok:
+                # a wrapped model that is not GPT-NeoX keeps the Llama executor's reason
+                keep_llama_why = check is fused_pythia.supports and not isinstance(inner, GPTNeoXForCausalLM)
+                raise RuntimeError(f"--engine fused requested but not applicable: {why if keep_llama_why else why_fused}")
+        if cls is not None:
+            if cls is fused_llama.FusedLlamaStepper:
+                kw.update(fp8=frozen in ("fp8", "fp8_full"), fp8_backward=frozen == "fp8_full")
+            return cls(model, info, cuda_graphs=getattr(args, "cuda_graphs", True), attention=getattr(args, "attention", "auto"),
+                       deterministic=bool(getattr(args, "deterministic", False)), **kw)
     if info.device.type != "cuda":
         kw["transport"] = "nccl"  # CPU: the process group's own reduction (gloo)
     # the fp8 tensor-core path and the wgmma attention kernels belong to the fused executor: say so instead of silently
