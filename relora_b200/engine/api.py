@@ -19,8 +19,7 @@ import torch.distributed as dist
 from ..config import build_parser, check_args
 from ..models import LlamaForCausalLM, load_config
 from ..parallel.dist import DistInfo, init_distributed
-from ..relora import ReLoRaModel, get_scheduler, optimizer_reset
-from .stepper import make_stepper
+from .stepper import make_scheduler, make_stepper, reset_optimizer, wrap_relora
 
 __all__ = ["TrainingEngine"]
 
@@ -34,31 +33,13 @@ class TrainingEngine:
         cfg = load_config(args.model_config)
         model = LlamaForCausalLM(cfg)
         if args.use_peft:
-            model = ReLoRaModel(
-                model, r=args.lora_r, lora_alpha=args.lora_alpha, lora_dropout=args.lora_dropout,
-                target_modules=["attn", "attention", "mlp"], trainable_scaling=args.train_scaling,
-                keep_original_weights=True, lora_only=False, quantize=args.quantize,
-                use_double_quant=args.use_double_quant, init_lora_a=args.init_lora_a,
-            )
-            model.seed = args.seed
+            model = wrap_relora(model, args, lora_only=False)
         dtype = torch.bfloat16 if args.dtype in ("bf16", "bfloat16") else torch.float32
         self.model = model.to(device=device, dtype=dtype)
         self.model.train()
-        native = None
-        if device.type == "cuda":
-            from ..ops import fused
-
-            native = fused.NativeOptim()
-            from ..ops import reference as _ref
-
-            fused.seed_state.set(device, _ref.mix_seed(args.seed, 0x5eed))  # LoRA-dropout stream follows --seed
-        self.stepper = make_stepper(self.model, self.info, args, native=native)
+        self.stepper = make_stepper(self.model, self.info, args)
         self.optimizer = self.stepper.optimizer
-        self.scheduler = get_scheduler(
-            self.optimizer, scheduler_type=args.scheduler, num_training_steps=args.num_training_steps,
-            warmup_steps=args.warmup_steps, min_lr_ratio=args.min_lr_ratio, cycle_length=args.cycle_length,
-            restart_warmup_steps=args.restart_warmup_steps, adjust_step=args.adjust_step,
-        )
+        self.scheduler = make_scheduler(self.optimizer, args, args.num_training_steps)
         self.update_step = 0
         self.n_lora_restarts = 0
         self.n_optimizer_resets = 0
@@ -135,17 +116,10 @@ class TrainingEngine:
             return
         if self.update_step >= a.relora and self.update_step % a.relora == 1:
             self.n_lora_restarts += 1
-            if hasattr(self.stepper, "merge_and_reinit"):
-                self.stepper.merge_and_reinit()
-            else:
-                self.model.merge_and_reinit()
+            self.stepper.merge_and_reinit()
         if self.update_step >= a.cycle_length and self.update_step % a.cycle_length == 1:
             self.n_optimizer_resets += 1
-            optimizer_reset(
-                self.optimizer, reset_params=self.stepper.lora_params, optimizer_state_keys=["exp_avg", "exp_avg_sq"],
-                reset_optimizer_on_relora=a.reset_optimizer_on_relora, optimizer_random_pruning=a.optimizer_random_pruning,
-                optimizer_magnitude_pruning=a.optimizer_magnitude_pruning, seed=a.seed, reset_index=self.n_optimizer_resets,
-            )
+            reset_optimizer(self.optimizer, self.stepper.lora_params, a, self.n_optimizer_resets)
 
     @property
     def tokens_per_step(self) -> int:

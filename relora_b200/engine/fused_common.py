@@ -6,11 +6,11 @@ provides the rest:
 
 * the checks every ``supports`` / ``supports_full_rank`` shares: the ReLoRA wrapper, fp8 in full-rank training, the native
   attention head dim and, last, the device;
-* the constructor preamble (sizes, ReLoRA rank / dropout / scale, attention backend, side stream, environment knobs), the gradient
-  transport (NVLink peer-memory kernels when symmetric memory is available, NCCL otherwise), the flat parameter store with stacked
-  views, ``GradSync`` and ``FlatAdamW``;
+* the constructor preamble (sizes, ReLoRA rank / dropout / scale, attention backend, side stream, environment knobs) and the flat
+  fp32-gradient parameter store with stacked views; the gradient transport, ``update()`` and the optimizer are those of every
+  stepper (:class:`.stepper.Stepper`, ``parallel.grad_sync``);
 * the buffers both executors share, the per-layer slot selection, the SDPA fallback attention and the embedding backward;
-* ``update()`` (NCCL or the peer-memory kernel chain) and ``merge_and_reinit()``;
+* ``merge_and_reinit()``;
 * one CUDA graph per micro-batch shape, capture / replay and launch counting;
 * the LoRA group forward / backward on the wgmma GEMM and the fused input-gradient kernel, and the chunked LM head + CE.
 """
@@ -21,14 +21,13 @@ import os
 from typing import Dict, List, Optional, Tuple
 
 import torch
-import torch.distributed as dist
 import torch.nn.functional as F_
 
 from ..ops import fused
-from ..parallel.flat import FlatAdamW, FlatParamStore
-from ..parallel.grad_sync import GradSync, broadcast_params
+from ..parallel.flat import FlatParamStore
+from ..parallel.grad_sync import broadcast_params, peer_transport
 from ..relora import ReLoRaModel
-from .stepper import UpdateInfo
+from .stepper import Stepper
 
 BF = torch.bfloat16
 
@@ -79,7 +78,7 @@ class LayerViews:
             setattr(self, k, None)
 
 
-class FusedStepperBase:
+class FusedStepperBase(Stepper):
     # ------------------------------------------------------------------ construction helpers
     def __init__(self, model, info, supports, supports_full_rank, *, grad_accumulation: int, clip_grad_norm: float,
                  cuda_graphs: bool, ce_chunk: int, overlap_wgrad: bool, attention: str, deterministic: bool):
@@ -124,24 +123,6 @@ class FusedStepperBase:
         # embedding backward without atomics (default); RELORA_B200_ATOMIC_EMBEDDING=1 selects the atomicAdd scatter
         self.deterministic_embedding = os.environ.get("RELORA_B200_ATOMIC_EMBEDDING", "0") != "1"
 
-    def _init_transport(self, info, transport: str) -> None:
-        """NVLink peer-memory kernels when symmetric memory is available (``self.comm``), NCCL otherwise (``self.comm = None``)."""
-        self.comm = None
-        if info.world_size > 1 and transport in ("p2p", "auto"):
-            from ..parallel.symm import SymmComm, symmetric_memory_available
-
-            if symmetric_memory_available():
-                try:
-                    self.comm = SymmComm()
-                except Exception as e:  # no P2P access, allocation failure, ...
-                    if transport == "p2p":
-                        raise
-                    from ..obs import logger
-
-                    logger.warning(f"peer-memory collectives unavailable ({type(e).__name__}: {e}); using NCCL")
-            elif transport == "p2p":
-                raise RuntimeError("--comm p2p needs torch symmetric memory over an NCCL process group")
-
     def _build_store(self, params: List[torch.nn.Parameter], transport: str,
                      padded: Optional[Dict[int, Tuple[int, int]]] = None) -> None:
         """Gradient transport and flat fp32-gradient store over ``params``, which must be every trainable parameter of the model.
@@ -153,13 +134,10 @@ class FusedStepperBase:
         extra = [n for n, p in self.model.named_parameters() if p.requires_grad and id(p) not in seen]
         if extra:
             raise RuntimeError(f"unexpected trainable parameters for the fused executor: {extra}")
-        self._init_transport(self.info, transport)
+        self.comm = peer_transport(self.info, transport)
         self.store = FlatParamStore(named, world_size=self.info.world_size, grad_dtype=torch.float32, bind_grads=False,
                                     allocator=self.comm.allocator() if self.comm is not None else None,
                                     storage_shapes=padded or {})
-        self.trainable_params = [p for _, p in named]
-        self.trainable_names = [n for n, _ in named]
-        self.lora_params = [p for n, p in named if "lora_" in n]
 
     def _stacked_view(self, p, rows_mult: int = 1, rows: Optional[int] = None):
         """(params, grads) views over ``rows_mult`` adjacent parameters of the flat store, starting at ``p``; or, with ``rows``,
@@ -174,21 +152,10 @@ class FusedStepperBase:
         return self.store.params[o:o + tot].view(shape), self.store.grads[o:o + tot].view(shape)
 
     def _init_optimizer(self, *, lr, betas, eps, weight_decay, zero: bool, native) -> None:
-        info, dev = self.info, self.device
-        self.sync = GradSync(self.store, info, transport="nccl", zero=zero and self.comm is None)
-        shard = self.sync.shard if (zero and self.comm is None) else None
-        self._stage = None
-        if self.comm is not None:
-            # fused update: gradients travel as bf16 through a symmetric buffer, each rank owns 1/world of the
-            # optimizer state (ZeRO-1 dataflow) and writes its updated parameters into every replica
-            self.sync.transport = "p2p"
-            self.param_buf = self.comm.buffer_of(self.store.params)
-            self.grad_buf = self.comm.alloc(self.store.numel, BF)
-            self.gred = torch.empty(self.store.numel // info.world_size, dtype=torch.float32, device=dev)
-            shard = self.store.shard_bounds(info.rank, info.world_size)
-        self.optimizer = FlatAdamW(self.store, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, shard=shard,
-                                   native=native or fused.NativeOptim())
-        self.seed = fused.seed_state.get(dev)
+        # fp32 gradients: they cross the wire as a bf16 copy
+        self._init_update(zero=zero, stage_bf16=True, native=native or fused.NativeOptim(), lr=lr, betas=betas, eps=eps,
+                          weight_decay=weight_decay)
+        self.seed = fused.seed_state.get(self.device)
         self._shape = None
         self._graph = None
         self._replays = 0
@@ -489,45 +456,6 @@ class FusedStepperBase:
         self._eval_body()
         return self.loss_out.clone()
 
-    @property
-    def folds_loss_reduce(self) -> bool:
-        """True when ``update(local_loss=...)`` combines loss / skip over ranks inside the NVLink kernel chain (no NCCL call)."""
-        return self.comm is not None
-
-    @torch.no_grad()
-    def update(self, skip: Optional[torch.Tensor] = None, error_if_nonfinite: bool = False,
-               local_loss: Optional[torch.Tensor] = None) -> UpdateInfo:
-        opt = self.optimizer
-        world = self.info.world_size
-        if self.comm is not None:
-            from .stepper import peer_memory_update
-
-            return peer_memory_update(self, grads_f32=self.store.grads, skip=skip, error_if_nonfinite=error_if_nonfinite,
-                                      local_loss=local_loss)
-        grads = None
-        if world > 1 and not self.sync.zero:
-            # NCCL baseline: gradients cross the wire as bf16 (like the reference's bf16 DDP buckets), once per update
-            if self._stage is None:
-                self._stage = torch.empty(self.store.numel, dtype=BF, device=self.device)
-            self.C.cast_f32_to_bf16(self.store.grads, self._stage, 1.0)
-            dist.all_reduce(self._stage, op=dist.ReduceOp.SUM)
-            grads = self._stage
-            sq = torch.zeros(1, dtype=torch.float32, device=self.device)
-            self.C.sumsq(grads, sq)
-            total = sq[0].sqrt() / world
-            coef = torch.clamp(self.clip / (total + 1e-6), max=1.0) if self.clip and self.clip > 0 else torch.ones_like(total)
-            coef = torch.where(torch.isfinite(total), coef, torch.full_like(coef, float("nan")))  # non-finite norm: skip the update
-            scale = coef / world
-        else:
-            self.sync.reduce()
-            total, scale = self.sync.grad_norm_and_scale(self.clip)
-        if error_if_nonfinite and not bool(torch.isfinite(total)):
-            raise RuntimeError(f"The total norm of order 2.0 for gradients is non-finite ({float(total)}), so it cannot be clipped.")
-        opt.step(grad_scale=scale, skip=skip, grads=grads)
-        self.sync.gather_params()
-        opt.zero_grad()
-        return UpdateInfo(total, False)
-
     @torch.no_grad()
     def merge_and_reinit(self):
         """W += s·B@A for every module of every layer and its (B, A, W) block (``mods`` / ``merge`` of the layer views; wgmma GEMM
@@ -556,7 +484,3 @@ class FusedStepperBase:
     def mark_launch_window(self):
         self._replay_mark = self._replays
         self.C.reset_launch_count()
-
-    def set_lr(self, lr: float) -> None:
-        for grp in self.optimizer.param_groups:
-            grp["lr"] = lr

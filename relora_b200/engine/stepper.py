@@ -17,33 +17,52 @@ one constructor call builds it.
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 
 from ..parallel.dist import DistInfo
 from ..parallel.flat import FlatAdamW, FlatParamStore
-from ..parallel.grad_sync import GradSync, broadcast_params
+from ..parallel.grad_sync import GradSync, UpdateInfo, broadcast_params, peer_transport
+from ..relora import ReLoRaModel, get_scheduler, optimizer_reset
 
-__all__ = ["UpdateInfo", "ModuleStepper", "trainable_named_parameters", "make_stepper"]
-
-
-@dataclass
-class UpdateInfo:
-    grad_norm: torch.Tensor  # device scalar (norm of the averaged gradient, before clipping)
-    skipped: bool
-    # set by the peer-memory update when the caller handed it this rank's loss: mean loss over ranks and the number of ranks that
-    # asked to skip (device scalars; the reference's loss_info all-reduce folded into the kernel chain, torchrun_main.py:810)
-    mean_loss: Optional[torch.Tensor] = None
-    skip_count: Optional[torch.Tensor] = None
+__all__ = ["UpdateInfo", "Stepper", "ModuleStepper", "trainable_named_parameters", "make_stepper", "wrap_relora", "make_scheduler",
+           "reset_optimizer"]
 
 
 def trainable_named_parameters(model: torch.nn.Module) -> List[Tuple[str, torch.nn.Parameter]]:
     return [(n, p) for n, p in model.named_parameters() if p.requires_grad]
 
 
-class ModuleStepper:
+class Stepper:
+    """What every stepper has.  A subclass sets ``model``, ``info`` and ``clip``, picks ``comm`` (:func:`peer_transport`), carves
+    ``store`` out of that transport's allocator -- the symmetric allocation has to exist first -- and then calls ``_init_update``;
+    ``micro_step`` and ``eval_loss`` are its own."""
+
+    def _init_update(self, *, zero: bool, stage_bf16: bool, native, **adamw) -> None:
+        self.sync = GradSync(self.store, self.info, zero=zero, comm=self.comm, stage_bf16=stage_bf16)
+        self.optimizer = FlatAdamW(self.store, shard=self.sync.shard, native=native, **adamw)
+        self.trainable_params, self.trainable_names = list(self.store.param_list), list(self.store.names)
+        self.lora_params = [p for n, p in zip(self.trainable_names, self.trainable_params) if "lora_" in n]
+
+    @property
+    def folds_loss_reduce(self) -> bool:
+        """True when ``update(local_loss=...)`` combines loss / skip over ranks inside the NVLink kernel chain (no NCCL call)."""
+        return self.comm is not None
+
+    def update(self, skip: Optional[torch.Tensor] = None, error_if_nonfinite: bool = False,
+               local_loss: Optional[torch.Tensor] = None) -> UpdateInfo:
+        return self.sync.update(self.optimizer, self.clip, skip, error_if_nonfinite, local_loss)
+
+    def set_lr(self, lr: float) -> None:
+        for g in self.optimizer.param_groups:
+            g["lr"] = lr
+
+    def merge_and_reinit(self) -> None:
+        self.model.merge_and_reinit()
+
+
+class ModuleStepper(Stepper):
     def __init__(
         self,
         model: torch.nn.Module,
@@ -64,45 +83,13 @@ class ModuleStepper:
         self.clip = clip_grad_norm
         broadcast_params(model)
         named = trainable_named_parameters(model)
-        # ---- transport: the hand-written NVLink update (csrc/comm.cu) when symmetric memory is available -- bf16 parameters on
-        # CUDA, more than one rank -- and NCCL / gloo otherwise.  Same kernel chain as the fused executor, except that the bf16
-        # gradients autograd accumulated are already in the symmetric buffer (no cast pass).
-        self.comm = None
+        # the hand-written NVLink update needs bf16 parameters on CUDA.  Same kernel chain as the fused executor, except that the
+        # bf16 gradients autograd accumulated are already in the symmetric buffer (no cast pass).
         p0 = named[0][1]
-        if info.world_size > 1 and transport in ("p2p", "auto") and p0.is_cuda and p0.dtype == torch.bfloat16:
-            from ..parallel.symm import SymmComm, symmetric_memory_available
-
-            if symmetric_memory_available():
-                try:
-                    self.comm = SymmComm()
-                except Exception as e:  # no P2P access, allocation failure, ...
-                    if transport == "p2p":
-                        raise
-                    from ..obs import logger
-
-                    logger.warning(f"peer-memory collectives unavailable ({type(e).__name__}: {e}); using NCCL")
-            elif transport == "p2p":
-                raise RuntimeError("--comm p2p needs torch symmetric memory over an NCCL process group")
-        elif transport == "p2p" and info.world_size > 1:
-            raise RuntimeError("--comm p2p needs bf16 parameters on CUDA")
-        if self.comm is not None:
-            alloc = self.comm.allocator()
-            self.store = FlatParamStore(named, world_size=info.world_size, allocator=alloc, grad_allocator=alloc)
-            self.sync = GradSync(self.store, info, transport="nccl", zero=False)
-            self.sync.transport = "p2p"
-            self.param_buf = self.comm.buffer_of(self.store.params)
-            self.grad_buf = self.comm.buffer_of(self.store.grads)
-            self.gred = torch.empty(self.store.numel // info.world_size, dtype=torch.float32, device=p0.device)
-            shard = self.store.shard_bounds(info.rank, info.world_size)  # ZeRO-1 dataflow: each rank owns 1/world of the moments
-        else:
-            self.store = FlatParamStore(named, world_size=info.world_size)
-            self.sync = GradSync(self.store, info, transport="nccl", zero=zero)
-            shard = self.sync.shard if zero else None
-        self.optimizer = FlatAdamW(self.store, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
-                                   shard=shard, native=native)
-        self.trainable_params = [p for _, p in named]
-        self.trainable_names = [n for n, _ in named]
-        self.lora_params = [p for n, p in named if "lora_" in n]
+        self.comm = peer_transport(info, transport, eligible=p0.is_cuda and p0.dtype == torch.bfloat16)
+        alloc = self.comm.allocator() if self.comm is not None else None
+        self.store = FlatParamStore(named, world_size=info.world_size, allocator=alloc, grad_allocator=alloc)
+        self._init_update(zero=zero, stage_bf16=False, native=native, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
 
     # ------------------------------------------------------------------ one micro-batch
     def micro_step(self, input_ids: torch.Tensor) -> torch.Tensor:
@@ -119,62 +106,50 @@ class ModuleStepper:
     def eval_loss(self, input_ids: torch.Tensor) -> torch.Tensor:
         return self.model(input_ids=input_ids, labels=input_ids).loss.detach()
 
-    # ------------------------------------------------------------------ one optimizer update
-    @property
-    def folds_loss_reduce(self) -> bool:
-        """True when ``update(local_loss=...)`` combines loss / skip over ranks inside the NVLink kernel chain (no NCCL call)."""
-        return self.comm is not None
 
-    @torch.no_grad()
-    def update(self, skip: Optional[torch.Tensor] = None, error_if_nonfinite: bool = False,
-               local_loss: Optional[torch.Tensor] = None) -> UpdateInfo:
-        if self.comm is not None:
-            return peer_memory_update(self, grads_f32=None, skip=skip, error_if_nonfinite=error_if_nonfinite, local_loss=local_loss)
-        self.sync.reduce()
-        total, scale = self.sync.grad_norm_and_scale(self.clip)
-        if error_if_nonfinite and not bool(torch.isfinite(total)):
-            raise RuntimeError(
-                f"The total norm of order 2.0 for gradients is non-finite ({float(total)}), so it cannot be clipped."
-            )
-        skipped = bool(skip) if skip is not None and not self.store.params.is_cuda else False
-        self.optimizer.step(grad_scale=scale, skip=skip)
-        self.sync.gather_params()
-        self.optimizer.zero_grad()
-        return UpdateInfo(total, skipped)
-
-    def set_lr(self, lr: float) -> None:
-        for g in self.optimizer.param_groups:
-            g["lr"] = lr
+def wrap_relora(model: torch.nn.Module, args, *, lora_only: bool) -> ReLoRaModel:
+    """``model`` under ReLoRA as the command line describes it."""
+    model = ReLoRaModel(
+        model, r=args.lora_r, lora_alpha=args.lora_alpha, lora_dropout=args.lora_dropout,
+        target_modules=["attn", "attention", "mlp"], trainable_scaling=args.train_scaling,
+        keep_original_weights=True, lora_only=lora_only, quantize=args.quantize,
+        use_double_quant=args.use_double_quant, init_lora_a=args.init_lora_a,
+    )
+    model.seed = args.seed
+    return model
 
 
-def peer_memory_update(st, *, grads_f32, skip, error_if_nonfinite: bool, local_loss) -> UpdateInfo:
-    """The data-parallel update on the hand-written NVLink kernels (``SymmComm.fused_update``), shared by both steppers: reduce-
-    scatter + Σg² → norm / loss / skip exchange → AdamW on the owned shard → parameter broadcast.  ``skip`` and ``local_loss`` are
-    this rank's values; a skip requested by any rank, or a non-finite gradient norm, leaves parameters, moments and the Adam step
-    count untouched on every rank."""
-    opt = st.optimizer
-    grp = opt.param_groups[0]
-    dev = st.store.device
-    sk = None if skip is None else (skip if torch.is_tensor(skip) else torch.tensor(float(skip), device=dev))
-    opt.advance_step(None)  # optimistic: taken back below when the kernels skipped
-    norm = st.comm.fused_update(
-        grads_f32=grads_f32, grad_buf=st.grad_buf, gred=st.gred, param_buf=st.param_buf, exp_avg=opt.exp_avg, exp_avg_sq=opt.exp_avg_sq,
-        n=st.store.numel, lr=grp["lr"], betas=grp["betas"], eps=grp["eps"], weight_decay=grp["weight_decay"], step=opt.step_count,
-        max_norm=st.clip, skip=sk, step_dev=opt._step_t, local_loss=local_loss)
-    total = norm[0].clone()
-    skip_count = st.comm.skip_all.clone()
-    skipped_dev = (skip_count > 0).to(torch.float32)
-    opt._step_t.sub_(skipped_dev)
-    opt.undo_step_if_nonfinite(total, skipped_dev)
-    opt.zero_grad()
-    if error_if_nonfinite and not bool(torch.isfinite(total)):
-        raise RuntimeError(f"The total norm of order 2.0 for gradients is non-finite ({float(total)}), so it cannot be clipped.")
-    mean_loss = st.comm.loss_out[0].clone() if local_loss is not None else None
-    return UpdateInfo(total, False, mean_loss=mean_loss, skip_count=skip_count)
+def make_scheduler(optimizer, args, num_training_steps: int):
+    return get_scheduler(
+        optimizer, scheduler_type=args.scheduler, num_training_steps=num_training_steps,
+        warmup_steps=args.warmup_steps, min_lr_ratio=args.min_lr_ratio, cycle_length=args.cycle_length,
+        restart_warmup_steps=args.restart_warmup_steps, adjust_step=args.adjust_step,
+    )
 
 
-def make_stepper(model, info: DistInfo, args, *, native=None):
-    """Pick the executor for ``model`` on ``info.device`` according to ``--engine``."""
+def reset_optimizer(optimizer, lora_params, args, reset_index: int) -> float:
+    """Prune the Adam moments of the LoRA factors (the ``reset_index``-th reset of the run keys the random pruning)."""
+    return optimizer_reset(
+        optimizer, reset_params=lora_params, optimizer_state_keys=["exp_avg", "exp_avg_sq"],
+        reset_optimizer_on_relora=args.reset_optimizer_on_relora, optimizer_random_pruning=args.optimizer_random_pruning,
+        optimizer_magnitude_pruning=args.optimizer_magnitude_pruning, seed=args.seed, reset_index=reset_index,
+    )
+
+
+def make_stepper(model, info: DistInfo, args, *, native=None, dropout_seed: Optional[int] = None):
+    """Pick the executor for ``model`` on ``info.device`` according to ``--engine``.  On CUDA the optimizer runs on the extension's
+    AdamW (``native``, created here unless given) and the LoRA-dropout counter starts from ``dropout_seed`` (a resumed run's saved
+    counter) or, without one, from a value derived from ``--seed``, so runs with different seeds draw different masks."""
+    if info.device.type == "cuda":
+        from ..ops import fused, reference
+        from ..ops import native as extension
+
+        extension.require()  # a CUDA device without the sm_90a extension fails here, before any training step
+        native = native or fused.NativeOptim()
+        if dropout_seed is None and hasattr(args, "seed"):  # a hand-made namespace without --seed leaves the counter alone
+            dropout_seed = reference.mix_seed(args.seed, 0x5eed)
+        if dropout_seed is not None:
+            fused.seed_state.set(info.device, dropout_seed)
     engine = getattr(args, "engine", "auto")
     zero = str(args.optimizer).lower() == "adam_zero"
     transport = getattr(args, "comm", "auto")

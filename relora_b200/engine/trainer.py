@@ -31,8 +31,8 @@ from ..models import LlamaForCausalLM, config_to_dict, load_config
 from ..models.pythia import GPTNeoXForCausalLM
 from ..obs import JsonlSink, PhaseTimer, logger, make_sink, maybe_make_profiler, silence_non_zero_rank
 from ..parallel.dist import barrier, broadcast_object, init_distributed, shutdown
-from ..relora import ReLoRaLinear, ReLoRaModel, get_scheduler, optimizer_reset
-from .stepper import make_stepper
+from ..relora import ReLoRaLinear, ReLoRaModel
+from .stepper import make_scheduler, make_stepper, reset_optimizer, wrap_relora
 
 __all__ = ["run", "evaluate_model", "TrainState"]
 
@@ -285,20 +285,7 @@ def run(args) -> dict:
     if args.use_peft:
         need_linear_weight = args.relora is not None or args.force_keep_original or args.warmed_up_model is not None
         logger.info(f"Wrapping model with LoRA ({need_linear_weight=})")
-        model = ReLoRaModel(
-            model,
-            r=args.lora_r,
-            lora_alpha=args.lora_alpha,
-            lora_dropout=args.lora_dropout,
-            target_modules=["attn", "attention", "mlp"],
-            trainable_scaling=args.train_scaling,
-            keep_original_weights=True,
-            lora_only=not need_linear_weight,
-            quantize=args.quantize,
-            use_double_quant=args.use_double_quant,
-            init_lora_a=args.init_lora_a,
-        )
-        model.seed = args.seed
+        model = wrap_relora(model, args, lora_only=not need_linear_weight)
 
     _update_step_ckpt = None
     _resume_dropout_seed = None
@@ -341,21 +328,9 @@ def run(args) -> dict:
             raise ValueError(f"Model config vocab size ({model_config.vocab_size}) does not match tokenizer vocab size ({data_vocab})")
 
     # ---------------------------------------------------------------- executor / optimizer / scheduler
-    native = None
-    if device.type == "cuda":
-        from ..ops import native as _native
-
-        native = _native.require()
-        from ..ops import fused as _fused
-
-        native = _fused.NativeOptim()
-    if device.type == "cuda":
-        # LoRA-dropout stream: base counter derived from --seed (runs with different seeds draw different masks); a resumed run
-        # continues from the counter saved in training_state.json instead of replaying the masks of step 0
-        from ..ops import reference as _ref
-
-        _fused.seed_state.set(device, _resume_dropout_seed if _resume_dropout_seed is not None else _ref.mix_seed(args.seed, 0x5eed))
-    stepper = make_stepper(model, info, args, native=native)
+    # a resumed run continues the LoRA-dropout stream from the counter saved in training_state.json instead of replaying the masks
+    # of step 0
+    stepper = make_stepper(model, info, args, dropout_seed=_resume_dropout_seed)
     optimizer = stepper.optimizer
     lora_params = stepper.lora_params
     if args.use_peft and len(lora_params) == 0:
@@ -385,16 +360,7 @@ def run(args) -> dict:
     scheduler_start_step = st.update_step
     sched_steps = args.num_training_steps - scheduler_start_step
     logger.info(f"Scheduler will run for {sched_steps} update steps")
-    scheduler = get_scheduler(
-        optimizer,
-        scheduler_type=args.scheduler,
-        num_training_steps=sched_steps,
-        warmup_steps=args.warmup_steps,
-        min_lr_ratio=args.min_lr_ratio,
-        cycle_length=args.cycle_length,
-        restart_warmup_steps=args.restart_warmup_steps,
-        adjust_step=args.adjust_step,
-    )
+    scheduler = make_scheduler(optimizer, args, sched_steps)
 
     if args.resume_from:
         # upstream replays `update_step` scheduler steps here with update_step still at the warm-start
@@ -539,23 +505,14 @@ def run(args) -> dict:
             logger.info(f"Performing lora reset at update step {st.update_step}. Current lr is {optimizer.param_groups[0]['lr']}")
             st.n_lora_restarts += 1
             with phases.phase("merge"):
-                stepper.merge_and_reinit() if hasattr(stepper, "merge_and_reinit") else model.merge_and_reinit()
+                stepper.merge_and_reinit()
             logger.info(f"LoRA reset took {time.time() - t0:.2f}s")
 
         can_reset_optimizer = args.relora is not None and (args.resume_from is not None or local_step // ga >= args.cycle_length)
         if can_reset_optimizer and rel % args.cycle_length == 1:
             logger.info(f"Performing optimizer reset at update step {st.update_step}. Current lr is {optimizer.param_groups[0]['lr']}")
             st.n_optimizer_resets += 1
-            optimizer_reset(
-                optimizer,
-                reset_params=lora_params,
-                optimizer_state_keys=["exp_avg", "exp_avg_sq"],
-                reset_optimizer_on_relora=args.reset_optimizer_on_relora,
-                optimizer_random_pruning=args.optimizer_random_pruning,
-                optimizer_magnitude_pruning=args.optimizer_magnitude_pruning,
-                seed=args.seed,
-                reset_index=st.n_optimizer_resets,
-            )
+            reset_optimizer(optimizer, lora_params, args, st.n_optimizer_resets)
             from ..utils import check_lr_and_alert, optimizer_state_size
 
             # after a reset the schedule must be at (nearly) zero lr; a large value means reset and schedule are out of phase
