@@ -379,16 +379,30 @@ void mx_quantize_rows(const Tensor& x, Tensor& q, Tensor& sf) {
   chk_bf16(x, "x"); chk_2d_rowmajor(x, "x");
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1 && q.size(0) >= x.size(0), "q must be uint8 [M, Kpad]");
   TORCH_CHECK(sf.is_cuda() && sf.scalar_type() == at::kByte && sf.is_contiguous() && sf.numel() >= rb::mx_sf_bytes(x.size(0), x.size(1)), "sf too small");
+  TORCH_CHECK(q.size(1) >= (x.size(1) + 127) / 128 * 128, "mx_quantize_rows: q must be [M, >= K rounded up to 128]");
+  // the kernel loads 4 bf16 of x and stores 4 bytes of q per access
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(x.data_ptr()) & 7) == 0 && x.stride(0) % 4 == 0,
+              "mx_quantize_rows: x needs an 8-byte aligned base and a row pitch that is a multiple of 4 elements");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(q.data_ptr()) & 3) == 0 && q.stride(0) % 4 == 0,
+              "mx_quantize_rows: q needs a 4-byte aligned base and a row pitch that is a multiple of 4");
   c10::cuda::CUDAGuard guard(x.device());
   rb::mx_quantize_rows(x.data_ptr(), x.stride(0), q.data_ptr(), q.stride(0), sf.data_ptr(), (int)x.size(0), (int)x.size(1), cur_stream());
 }
 void mx_quantize_weight_2d(const OptTensor& w, const OptTensor& delta, Tensor& q, Tensor& sf_fwd, Tensor& sf_bwd, int64_t N, int64_t K) {
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1, "q must be uint8 [Npad, Kpad]");
   TORCH_CHECK(q.size(0) >= (N + 127) / 128 * 128 && q.size(1) >= (K + 127) / 128 * 128, "q must be padded to multiples of 128 in both dimensions");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(q.data_ptr()) & 3) == 0 && q.stride(0) % 4 == 0,
+              "mx_quantize_weight_2d: q needs a 4-byte aligned base and a row pitch that is a multiple of 4");
   TORCH_CHECK(sf_fwd.scalar_type() == at::kByte && sf_bwd.scalar_type() == at::kByte && sf_fwd.is_contiguous() && sf_bwd.is_contiguous());
   TORCH_CHECK(sf_fwd.numel() >= rb::mx_sf_bytes(N, K) && sf_bwd.numel() >= rb::mx_sf_bytes(K, N), "scale buffers too small");
   const void* wp = nullptr; long long ldw = 0;
-  if (w.has_value()) { chk_bf16(*w, "w"); chk_2d_rowmajor(*w, "w"); TORCH_CHECK(w->size(0) == N && w->size(1) == K); wp = w->data_ptr(); ldw = w->stride(0); }
+  if (w.has_value()) {
+    chk_bf16(*w, "w"); chk_2d_rowmajor(*w, "w"); TORCH_CHECK(w->size(0) == N && w->size(1) == K);
+    // the kernel loads 8 bf16 of w per access
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(w->data_ptr()) & 15) == 0 && w->stride(0) % 8 == 0,
+                "mx_quantize_weight_2d: w needs a 16-byte aligned base and a row pitch that is a multiple of 8 elements");
+    wp = w->data_ptr(); ldw = w->stride(0);
+  }
   const float* dp = nullptr; long long ldd = 0;
   if (delta.has_value()) {
     TORCH_CHECK(delta->scalar_type() == at::kFloat && delta->dim() == 2 && delta->stride(1) == 1 && delta->size(0) == N && delta->size(1) == K);
@@ -400,7 +414,16 @@ void mx_quantize_weight_2d(const OptTensor& w, const OptTensor& delta, Tensor& q
 }
 void mx_dequantize_weight(const Tensor& q, const Tensor& sf_fwd, Tensor& out) {
   chk_bf16(out, "out"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1 && sf_fwd.scalar_type() == at::kByte);
+  TORCH_CHECK(q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1 && sf_fwd.scalar_type() == at::kByte && sf_fwd.is_contiguous());
+  TORCH_CHECK(q.is_cuda() && sf_fwd.is_cuda() && q.device() == out.device() && sf_fwd.device() == out.device(),
+              "mx_dequantize_weight: operands must be on the device of out");
+  TORCH_CHECK(q.size(0) >= out.size(0) && q.size(1) >= out.size(1) && sf_fwd.numel() >= rb::mx_sf_bytes(out.size(0), out.size(1)),
+              "mx_dequantize_weight: q / sf_fwd are smaller than out");
+  // the kernel loads 4 bytes of q and stores 4 bf16 of out per access
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(q.data_ptr()) & 3) == 0 && q.stride(0) % 4 == 0,
+              "mx_dequantize_weight: q needs a 4-byte aligned base and a row pitch that is a multiple of 4");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(out.data_ptr()) & 7) == 0 && out.stride(0) % 4 == 0,
+              "mx_dequantize_weight: out needs an 8-byte aligned base and a row pitch that is a multiple of 4 elements");
   c10::cuda::CUDAGuard guard(q.device());
   rb::mx_dequantize_weight(q.data_ptr(), q.stride(0), sf_fwd.data_ptr(), out.data_ptr(), out.stride(0), (int)out.size(0), (int)out.size(1), cur_stream());
 }

@@ -228,14 +228,23 @@ __device__ __forceinline__ uint32_t sf_offset(long long row, int sfcol, int kg_p
   const int r = int(row & 127), kg = sfcol >> 2, j = sfcol & 3;
   return uint32_t(((rb * kg_per_block + kg) << 9) + ((r & 31) << 4) + ((r >> 5) << 2) + j);
 }
-// smallest power of two s = 2^e with amax / s <= 448 (E4M3 max); returns the biased UE8M0 byte and 1/s
+// Scale of a block whose largest magnitude is `amax` (NaN elements ignored): the smallest e with amax <= 448 * 2^e (E4M3 max),
+// clamped to [-127, 127] (an all-zero block gets -127); returns the biased UE8M0 byte e + 127 and 1/2^e.  Exact, from the bits:
+// amax = (1 + F/2^23) * 2^(E-127) <= 1.75 * 2^(E-126) = 448 * 2^(E-135) exactly when F <= 0x600000, else 448 * 2^(E-134) bounds
+// it.  A block holding +-Inf gets the OCP MX NaN scale 0xFF (ue8m0_value decodes it as Inf), so every product it feeds is
+// non-finite; its elements are encoded times 0 (zeros, NaN for the infinities).
 __device__ __forceinline__ uint8_t ue8m0_for(float amax, float& inv_scale) {
-  int e = -127;
-  if (amax > 0.f) {
-    e = (int)ceilf(log2f(amax * (1.f / 448.f)));
-    e = max(-127, min(127, e));
+  if (isinf(amax)) {
+    inv_scale = 0.f;
+    return 0xFF;
   }
-  inv_scale = exp2f((float)-e);
+  int e = -127;
+  if (amax > 0.f) {  // false for NaN: a block of NaN only counts as zero
+    const uint32_t bits = __float_as_uint(amax);
+    const int E = int(bits >> 23);
+    e = max(-127, E - 135 + ((bits & 0x7FFFFFu) > 0x600000u ? 1 : 0));  // <= 120 for finite amax
+  }
+  inv_scale = ue8m0_value(uint8_t(127 - e));
   return (uint8_t)(e + 127);
 }
 
@@ -299,7 +308,7 @@ __global__ void __launch_bounds__(256) mx_quantize_weight_2d_kernel(const bf16* 
           }
         }
       } else {  // requantisation: start from the packed weight and its (forward-layout) scale
-        const float s_old = exp2f((float)sf_old[sf_offset(n, tk, kg_fwd)] - 127.f);
+        const float s_old = ue8m0_value(sf_old[sf_offset(n, tk, kg_fwd)]);
 #pragma unroll
         for (int j = 0; j < 32; j += 4) {
           const int k = tk * 32 + j;
@@ -354,7 +363,7 @@ __global__ void __launch_bounds__(256) mx_dequantize_weight_kernel(const uint8_t
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long n = i / (K / 4);
     const int k = int(i % (K / 4)) * 4;
-    const float s = exp2f((float)sf[sf_offset(n, k >> 5, kg)] - 127.f);
+    const float s = ue8m0_value(sf[sf_offset(n, k >> 5, kg)]);
     const uint32_t raw = *reinterpret_cast<const uint32_t*>(q + n * ldq + k);
     float f[4];
 #pragma unroll

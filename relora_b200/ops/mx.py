@@ -9,7 +9,7 @@
 * :func:`merge_` — the ReLoRA merge on packed storage: dequantise → fp32 add → requantise with fresh tile scales, in place
   (reference ``relora.py:277-299``).
 
-The pure-PyTorch functions at the bottom are the numerics oracle (tests/test_kernels_gpu.py).
+The pure-PyTorch functions at the bottom decode the exact contracts of ops/reference.py (block-scaled MXFP8 section).
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ from typing import Optional, Tuple
 
 import torch
 
-from . import native
+from . import native, reference
 
 __all__ = ["MxWeight", "quantize_weight", "dequantize_weight", "quantize_rows", "linear", "merge_", "supported",
            "ref_quantize_rows", "ref_quantize_weight_2d"]
@@ -127,26 +127,16 @@ def linear(x: torch.Tensor, mw: MxWeight, bias: Optional[torch.Tensor] = None, a
 
 
 # ----------------------------------------------------------------------------- PyTorch oracle
-def _ue8m0(amax: torch.Tensor) -> torch.Tensor:
-    e = torch.ceil(torch.log2(torch.clamp(amax, min=2.0 ** -127) / 448.0)).clamp(-127, 127)
-    return torch.exp2(e)
-
-
 def ref_quantize_rows(x: torch.Tensor) -> torch.Tensor:
-    """Dequantised value of the row-wise (1 x 32) MXFP8 quantisation of ``x`` (fp32)."""
-    M, K = x.shape
-    Kp = (K + 31) // 32 * 32
-    xf = torch.nn.functional.pad(x.float(), (0, Kp - K)).view(M, Kp // 32, 32)
-    s = _ue8m0(xf.abs().amax(-1, keepdim=True))
-    q = (xf / s).clamp(-448, 448).to(torch.float8_e4m3fn).float()
-    return (q * s).view(M, Kp)[:, :K]
+    """Dequantised value of the row-wise (1 x 32) MXFP8 quantisation of ``x`` (fp32; the exact contract of
+    :func:`quantize_rows`, ops/reference.py)."""
+    q, sf = reference.mx_quantize_rows_exact(x.to(_BF16))
+    return reference.mx_decode_rows(q, sf, *x.shape).float()
 
 
 def ref_quantize_weight_2d(w: torch.Tensor) -> torch.Tensor:
-    """Dequantised value of the 32 x 32-tile MXFP8 quantisation of ``w`` (fp32)."""
+    """Dequantised value of the 32 x 32-tile MXFP8 quantisation of ``w`` (fp32; the exact contract of :func:`quantize_weight`,
+    ops/reference.py)."""
     N, K = w.shape
-    Np, Kp = (N + 31) // 32 * 32, (K + 31) // 32 * 32
-    wf = torch.nn.functional.pad(w.float(), (0, Kp - K, 0, Np - N)).view(Np // 32, 32, Kp // 32, 32)
-    s = _ue8m0(wf.abs().amax(dim=(1, 3), keepdim=True))
-    q = (wf / s).clamp(-448, 448).to(torch.float8_e4m3fn).float()
-    return (q * s).view(Np, Kp)[:N, :K]
+    q, sf_fwd, _ = reference.mx_quantize_weight_2d_exact(w.to(_BF16))
+    return reference.mx_decode_weight(q, sf_fwd, N, K).float()

@@ -18,6 +18,8 @@ from typing import Optional
 
 import torch
 
+from .reference import mx_encode_blocks
+
 __all__ = ["QuantizedWeight", "quantize", "dequantize", "canonical_format", "FORMATS"]
 
 FORMATS = ("mxfp8", "nvfp4")
@@ -74,14 +76,9 @@ def _quantize_mxfp8(w: torch.Tensor) -> QuantizedWeight:
     shape = w.shape
     wf = _pad_k(w.detach().to(torch.float32), 32)
     n, kp = wf.shape
-    blocks = wf.view(n, kp // 32, 32)
-    amax = blocks.abs().amax(dim=-1)
-    # smallest power of two s with amax / s <= 448
-    exp = torch.ceil(torch.log2(torch.clamp(amax, min=2.0**-127) / _E4M3_MAX)).clamp(-127, 127)
-    scale = torch.exp2(exp)
-    q = (blocks / scale.unsqueeze(-1)).clamp(-_E4M3_MAX, _E4M3_MAX).to(torch.float8_e4m3fn)
-    data = q.view(torch.uint8).reshape(n, kp)
-    return QuantizedWeight("mxfp8", shape, data, (exp + 127).to(torch.uint8))
+    # the exponent rule and encoding of the CUDA quantisers (ops/reference.py: smallest power of two s with amax / s <= 448)
+    q, scales = mx_encode_blocks(wf.view(n, kp // 32, 32))
+    return QuantizedWeight("mxfp8", shape, q.reshape(n, kp), scales)
 
 
 def _dequantize_mxfp8(qw: QuantizedWeight, dtype) -> torch.Tensor:

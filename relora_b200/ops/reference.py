@@ -1037,6 +1037,172 @@ def assert_bitwise_equal(name: str, got: torch.Tensor, ref: torch.Tensor) -> Non
         raise AssertionError(f"{name} differs at {n_bad} of {got.numel()} elements; first at {idx}: got={gv!r} expected={rv!r}")
 
 
+# ----------------------------------------------------------------------------- block-scaled MXFP8 (csrc/gemm_mx.cu)
+# Exact contracts of mx_quantize_rows, mx_quantize_weight_2d, mx_dequantize_weight and gemm_mx.  E4M3 elements, one UE8M0 scale
+# byte b (value 2^(b-127)) per 32 elements of the reduction dimension: per (row, 32 columns) for activations, per 32 x 32 tile for
+# weights (written once in the forward layout, rows N, and once in the backward layout, rows K).
+#
+#   exponent  e = the smallest integer with amax <= 448·2^e, clamped to [-127, 127]; amax = max |x| over the block, NaN elements
+#             ignored (an all-zero or all-NaN block gets -127)
+#   elements  RNE(x·2^-e) to E4M3, saturated to ±448; a NaN element gives an E4M3 NaN byte (sign unspecified)
+#   ±Inf      a block holding an infinity gets the OCP MX NaN scale 0xFF, decoded as Inf, so every product it feeds is
+#             non-finite; its elements are x·0 (zeros, NaN for the infinities).  Other blocks are unaffected.
+MX_SF_NAN = 0xFF
+
+
+def mx_sf_bytes(rows: int, k: int) -> int:
+    """Bytes of the scale array of a ``[rows, k]`` operand: 512 per block of 128 rows x 128 reduction elements."""
+    return (rows + 127) // 128 * ((k + 127) // 128) * 512
+
+
+def mx_sf_offset(row, sfcol, kg):
+    """Byte offset of the scale of (``row``, scale column ``sfcol``) with ``kg`` groups of 4 scale columns per 128-row block:
+    blocks ordered [row block][k group], inside a block byte (r % 32)·16 + (r // 32)·4 + j with r = row % 128, j = sfcol % 4.
+    Integers or integer tensors."""
+    r = row % 128
+    return ((row // 128) * kg + sfcol // 4) * 512 + (r % 32) * 16 + (r // 32) * 4 + sfcol % 4
+
+
+def _pad128(n: int) -> int:
+    return (n + 127) // 128 * 128
+
+
+def _sf_index(rows: int, k: int, device=None) -> torch.Tensor:
+    """``[pad128(rows), pad128(k)/32]`` byte offsets of every scale of a ``[rows, k]`` operand (the array is exactly covered)."""
+    r = torch.arange(_pad128(rows), device=device).unsqueeze(1)
+    j = torch.arange(_pad128(k) // 32, device=device).unsqueeze(0)
+    return mx_sf_offset(r, j, _pad128(k) // 128)
+
+
+def mx_scale_grid(sf: torch.Tensor, rows: int, k: int) -> torch.Tensor:
+    """The scale bytes of a ``[rows, k]`` operand as a ``[pad128(rows), pad128(k)/32]`` grid."""
+    return sf.reshape(-1)[_sf_index(rows, k, sf.device)]
+
+
+def mx_scale_pack(grid: torch.Tensor, rows: int, k: int) -> torch.Tensor:
+    """Inverse of :func:`mx_scale_grid`: the ``mx_sf_bytes(rows, k)`` array holding ``grid``."""
+    sf = torch.empty(mx_sf_bytes(rows, k), dtype=torch.uint8, device=grid.device)
+    sf[_sf_index(rows, k, grid.device)] = grid.to(torch.uint8)
+    return sf
+
+
+def mx_scale_exponent(amax: torch.Tensor) -> torch.Tensor:
+    """int64 e: the smallest integer with ``amax <= 448·2^e``, clamped to [-127, 127], for finite ``amax >= 0``.  Exact: with
+    amax = m·2^x (m in [0.5, 1), frexp), 448·2^(x-9) = 0.875·2^x and 448·2^(x-8) = 1.75·2^x bracket it, and the comparison with
+    448·2^e is exact in fp64."""
+    a = amax.to(_F64)
+    _, x = torch.frexp(a)
+    e0 = x.to(torch.int64) - 9
+    e = e0 + (a > torch.ldexp(torch.full_like(a, 448.0), e0)).to(torch.int64)
+    return torch.where(a > 0, e, torch.full_like(e, -127)).clamp(-127, 127)
+
+
+def mx_encode_blocks(v: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Blocks ``v [..., 32]`` (values as the kernel holds them in fp32) -> (E4M3 bytes ``[..., 32]``, scale bytes ``[...]``)."""
+    v = v.to(_F64)
+    amax = torch.where(torch.isnan(v), torch.zeros_like(v), v.abs()).amax(-1)
+    inf = torch.isinf(amax)
+    e = mx_scale_exponent(torch.where(inf, torch.zeros_like(amax), amax))
+    inv = torch.where(inf, torch.zeros_like(amax), torch.ldexp(torch.ones_like(amax), -e))
+    # x·2^-e is exact in fp64; where it is not exact in fp32 (below 2^-126) it rounds to ±0 in E4M3 either way
+    q = fp8_saturate((v * inv.unsqueeze(-1)).to(torch.float32))
+    return q, torch.where(inf, torch.full_like(e, MX_SF_NAN), e + 127).to(torch.uint8)
+
+
+def mx_quantize_rows_exact(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``mx_quantize_rows(x, q, sf)`` of a bf16 ``[M, K]``: ``(q [M, Kpad], sf)`` byte for byte, Kpad = K rounded up to 128.
+    Columns past K are quantised as zeros (padding bytes 0) and rows up to the next multiple of 128 get scales (of zero rows)."""
+    M, K = x.shape
+    Mp, Kp = _pad128(M), _pad128(K)
+    v = torch.zeros(Mp, Kp, dtype=_F64, device=x.device)
+    v[:M, :K] = x.to(_F64)
+    q, s = mx_encode_blocks(v.view(Mp, Kp // 32, 32))
+    return q.view(Mp, Kp)[:M].contiguous(), mx_scale_pack(s, M, K)
+
+
+def mx_decode(q: torch.Tensor, sf: torch.Tensor, rows: int, k: int) -> torch.Tensor:
+    """Exact fp64 values ``[rows, pad128(k)]`` of a K-major packed operand: E4M3(q[r, c]) · 2^(scale(r, c/32) - 127), scale byte
+    0xFF read as Inf."""
+    Kp = _pad128(k)
+    g = mx_scale_grid(sf, rows, k)[:rows].to(_F64)
+    s = torch.where(g == MX_SF_NAN, torch.full_like(g, math.inf), torch.exp2(g - 127.0))
+    e = q[:rows, :Kp].contiguous().view(torch.float8_e4m3fn).to(_F64)
+    return (e.view(rows, Kp // 32, 32) * s.unsqueeze(-1)).view(rows, Kp)
+
+
+def mx_decode_rows(q: torch.Tensor, sf: torch.Tensor, M: int, K: int) -> torch.Tensor:
+    """Exact fp64 ``[M, K]`` values of the output of ``mx_quantize_rows``."""
+    return mx_decode(q, sf, M, K)[:, :K]
+
+
+def mx_decode_weight(q: torch.Tensor, sf_fwd: torch.Tensor, N: int, K: int) -> torch.Tensor:
+    """Exact fp64 ``[N, K]`` values of a packed weight (the contract of ``mx_dequantize_weight`` before its bf16 rounding)."""
+    return mx_decode(q, sf_fwd, N, K)[:, :K]
+
+
+def mx_quantize_weight_2d_exact(w: Optional[torch.Tensor] = None, q_old: Optional[torch.Tensor] = None,
+                                sf_old: Optional[torch.Tensor] = None, delta: Optional[torch.Tensor] = None, *,
+                                N: Optional[int] = None, K: Optional[int] = None):
+    """``mx_quantize_weight_2d(w, delta, q, sf_fwd, sf_bwd, N, K)``: ``(q [Npad, Kpad], sf_fwd, sf_bwd)`` byte for byte.
+
+    The source is the bf16 ``w [N, K]``, or (``w`` None, the merge) the packed ``q_old [>= N, >= Kpad]`` / ``sf_old`` (forward
+    layout) decoded in fp32 over all Kpad columns; the fp32 ``delta [N, K]`` is then added in fp32.  Rows past N are zeros.
+    Each 32 x 32 tile is one block; its scale goes to (row n, column k/32) of ``sf_fwd`` and (row k, column n/32) of ``sf_bwd``."""
+    src = w if w is not None else delta
+    N = src.shape[0] if N is None else N
+    K = src.shape[1] if K is None else K
+    Np, Kp = _pad128(N), _pad128(K)
+    dev = (w if w is not None else q_old).device
+    v = torch.zeros(Np, Kp, dtype=torch.float32, device=dev)
+    if w is not None:
+        v[:N, :K] = w.to(torch.float32)
+    else:
+        v[:N] = mx_decode(q_old, sf_old, N, K).to(torch.float32)  # E4M3 value · power of two: exact in fp32
+    if delta is not None:
+        v[:N, :K] += delta.to(torch.float32)
+    tiles = v.view(Np // 32, 32, Kp // 32, 32).permute(0, 2, 1, 3)  # [tn, tk, n, k]
+    q, s = mx_encode_blocks(tiles.reshape(Np // 32, Kp // 32, 1024))
+    q = q.view(Np // 32, Kp // 32, 32, 32).permute(0, 2, 1, 3).reshape(Np, Kp)
+    s_fwd = s.repeat_interleave(32, 0)  # [Np, Kp/32]: row n, column tk
+    s_bwd = s.t().repeat_interleave(32, 0)  # [Kp, Np/32]: row k, column tn
+    return q, mx_scale_pack(s_fwd, N, K), mx_scale_pack(s_bwd, K, N)
+
+
+def gemm_mx_ref(a: torch.Tensor, sfa: torch.Tensor, b: torch.Tensor, sfb: torch.Tensor, M: int, N: int, K: int,
+                b_mn_major: bool = False, a2: Optional[torch.Tensor] = None, b2: Optional[torch.Tensor] = None,
+                residual: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp64 ``(ref, bound)`` of ``gemm_mx(a, sfa, b, sfb, out, M, N, K, b_mn_major, a2, b2, residual)``:
+
+        out[m, n] = Σ_{k < Kpad} A[m, k]·B[n, k]  +  Σ_j a2[m, j]·b2[n, j]  +  residual[m, n]
+
+    A the decoded ``a [M, Kpad]`` with scales ``sfa`` (rows M); B the decoded ``b [N, Kpad]`` (K-major) or ``b[:Kpad, :N]ᵀ``
+    (``b_mn_major``, the weight read for the input gradient), with scales ``sfb`` for rows N, reduction K.  The reduction runs
+    over the padded Kpad = K rounded up to 128 (the quantisers write zeros there).  ``bound`` is Σ|terms| for
+    :func:`assert_gemm_close` with ``fp8=True``.  An Inf scale or a NaN element makes the outputs it feeds non-finite."""
+    Kp = _pad128(K)
+    A = mx_decode(a, sfa, M, K)
+    bb = b[:Kp, :N].t() if b_mn_major else b[:N, :Kp]
+    B = mx_decode(bb, sfb, N, K)
+    ref, bound = A @ B.t(), A.abs() @ B.abs().t()
+    if a2 is not None:
+        x, y = a2[:M].to(_F64), b2[:N].to(_F64)
+        ref, bound = ref + x @ y.t(), bound + x.abs() @ y.abs().t()
+    if residual is not None:
+        r = residual[:M, :N].to(_F64)
+        ref, bound = ref + r, bound + r.abs()
+    return ref, bound
+
+
+def assert_e4m3_bytes_equal(name: str, got: torch.Tensor, expected: torch.Tensor) -> None:
+    """E4M3 bytes equal bit for bit, except that any NaN byte (0x7F / 0xFF) matches any other."""
+    nan_g, nan_e = (got & 0x7F) == 0x7F, (expected.to(got.device) & 0x7F) == 0x7F
+    same = torch.where(nan_e, nan_g, (got == expected.to(got.device)) & ~nan_g)
+    if not bool(same.all()):
+        idx = tuple(int(i) for i in (~same).nonzero()[0])
+        raise AssertionError(f"{name} differs at {int((~same).sum())} of {got.numel()} bytes; first at {idx}: "
+                             f"got 0x{int(got[idx]):02x} expected 0x{int(expected[idx]):02x}")
+
+
 # ----------------------------------------------------------------------------- merge
 def merge_delta(weight: torch.Tensor, lora_a: torch.Tensor, lora_b: torch.Tensor, scale: float) -> torch.Tensor:
     """W + s·B@A accumulated in fp32, rounded to ``weight.dtype`` (reference relora.py:275-276)."""

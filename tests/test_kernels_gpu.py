@@ -726,55 +726,56 @@ def test_module_path_attention_uses_the_wgmma_kernels(F):
 
 # ----------------------------------------------------------------------------------------- block-scaled MXFP8 (csrc/gemm_mx.cu)
 def test_mx_quantisers_match_the_oracle(C):
+    """The quantisers byte for byte against the exact contract (ops/reference.py); the full sweep is test_mx_modes_gpu.py."""
     from relora_b200.ops import mx
+    from relora_b200.ops import reference as ref
 
     torch.manual_seed(0)
     x = _rand(200, 328, scale=3.0)
     x[5] = 0                      # an all-zero row: scale 2^-127, zeros
     q, sf = mx.quantize_rows(x)
     assert q.shape == (200, 384)
-    # dequantise through the weight path to check values: quantise the same matrix as a "weight" with 1 x 32 semantics is not
-    # available, so compare through a GEMM with the identity instead (see test_mx_gemm); here: bytes of the padding are zero
-    assert int(q[:, 328:].max()) == 0
+    q_ref, sf_ref = ref.mx_quantize_rows_exact(x)
+    ref.assert_e4m3_bytes_equal("quantize_rows q", q, q_ref)
+    ref.assert_bitwise_equal("quantize_rows sf", sf, sf_ref)
     w = _rand(264, 328, scale=0.05)
     mw = mx.quantize_weight(w)
-    deq = mx.dequantize_weight(mw).float()
-    ref = mx.ref_quantize_weight_2d(w)
-    # the scale exponent may differ by one where amax / 448 sits on a power of two (log2f rounding): compare values, not bytes
-    assert _relerr(deq, ref) < 2e-2 and _relerr(deq, w) < 4e-2
+    for got, want, name in zip((mw.q, mw.sf_fwd, mw.sf_bwd), ref.mx_quantize_weight_2d_exact(w), ("q", "sf_fwd", "sf_bwd")):
+        ref.assert_bitwise_equal(f"quantize_weight {name}", got, want)
+    ref.assert_bitwise_equal("dequantize_weight", mx.dequantize_weight(mw), mx.ref_quantize_weight_2d(w).to(BF))
     # merge: W += delta, requantised in place
     delta = torch.randn(264, 328, device="cuda") * 0.01
+    want = ref.mx_quantize_weight_2d_exact(q_old=mw.q.clone(), sf_old=mw.sf_fwd.clone(), delta=delta)
     mx.merge_(mw, delta)
-    assert _relerr(mx.dequantize_weight(mw), mx.ref_quantize_weight_2d(deq + delta)) < 2e-2
+    for got, w_, name in zip((mw.q, mw.sf_fwd, mw.sf_bwd), want, ("q", "sf_fwd", "sf_bwd")):
+        ref.assert_bitwise_equal(f"merge {name}", got, w_)
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 128, 128), (384, 256, 512), (300, 264, 328), (1024, 768, 768)])
 def test_mx_gemm_forward_and_input_gradient(C, M, N, K):
-    """e4m3 wgmma per 32-element scale block vs the fp32 product of the dequantised operands."""
+    """e4m3 wgmma per 32-element scale block vs the exact product of the decoded operands (ops/reference.py: gemm_mx_ref)."""
     from relora_b200.ops import mx
+    from relora_b200.ops import reference as ref
 
     torch.manual_seed(1)
     x = _rand(M, K, scale=1.5)
     w = _rand(N, K, scale=0.03)
     mw = mx.quantize_weight(w)
-    wd = mx.dequantize_weight(mw).float()
     y = mx.linear(x, mw)
-    want = mx.ref_quantize_rows(x) @ wd.t()
-    assert _relerr(y, want) < 1e-2, ("forward", _relerr(y, want))
+    xq, sfx = mx.quantize_rows(x)
+    ref.assert_gemm_close(y, *ref.gemm_mx_ref(xq, sfx, mw.q, mw.sf_fwd, M, N, K), fp8=True)
     # input gradient: the same bytes read MN-major, reduction over N
     dy = _rand(M, N, scale=0.7)
     xr = x.clone().requires_grad_()
     mx.linear(xr, mw).backward(dy)
-    want_dx = mx.ref_quantize_rows(dy) @ wd
-    assert _relerr(xr.grad, want_dx) < 1e-2, ("dx", _relerr(xr.grad, want_dx))
+    dq, sfd = mx.quantize_rows(dy)
+    ref.assert_gemm_close(xr.grad, *ref.gemm_mx_ref(dq, sfd, mw.q, mw.sf_bwd, M, K, N, b_mn_major=True), fp8=True)
     # LoRA segment in the same accumulator + residual
     u, B = _rand(M, 128, scale=0.5), _rand(N, 128, scale=0.05)
     res = _rand(M, N)
     out = torch.empty(M, N, device="cuda", dtype=BF)
-    xq, sfx = mx.quantize_rows(x)
     C.gemm_mx(xq, sfx, mw.q, mw.sf_fwd, out, M, N, K, False, u, B, res)
-    want2 = want + u.float() @ B.float().t() + res.float()
-    assert _relerr(out, want2) < 1e-2
+    ref.assert_gemm_close(out, *ref.gemm_mx_ref(xq, sfx, mw.q, mw.sf_fwd, M, N, K, a2=u, b2=B, residual=res), fp8=True)
 
 
 def test_mx_relora_linear_packed_storage_trains():
