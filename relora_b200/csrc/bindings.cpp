@@ -1,5 +1,9 @@
 // Python bindings (pybind11 over torch::Tensor) for the sm_90a kernels.  Every function launches on the
 // current PyTorch CUDA stream, so the ops compose with torch streams and CUDA-graph capture.
+//
+// This is where Python tensors become raw pointers, so every tensor argument goes through arg() once, before anything
+// launches: a call that got past the host with a wrong operand would fault on the device instead of raising.  The launchers
+// keep only the limits of what their kernels support (row widths, head dims, tile multiples).
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -17,45 +21,97 @@ namespace {
 
 using torch::Tensor;
 using OptTensor = c10::optional<Tensor>;
+constexpr auto BF = at::kBFloat16;
+constexpr auto F32 = at::kFloat;
 
 cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
-void chk_bf16(const Tensor& t, const char* name) {
-  TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
-  TORCH_CHECK(t.scalar_type() == at::kBFloat16, name, " must be bfloat16");
-}
-void chk_2d_rowmajor(const Tensor& t, const char* name) {
-  TORCH_CHECK(t.dim() == 2 && t.stride(1) == 1, name, " must be 2-D with unit inner stride");
-}
-const uint32_t* u32ptr(const OptTensor& t) {
-  if (!t.has_value()) return nullptr;
-  TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kInt, "seed tensor must be a CUDA int32 tensor");
-  return reinterpret_cast<const uint32_t*>(t->data_ptr<int32_t>());
-}
-const float* f32ptr(const OptTensor& t) {
-  if (!t.has_value()) return nullptr;
-  TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat, "expected a CUDA float32 tensor");
-  return t->data_ptr<float>();
+// The binding being called and the device all of its tensors must be on.
+struct Call {
+  const char* fn;
+  c10::Device dev;
+};
+
+// Numbers are formatted with std::to_string: streaming an integer into a TORCH_CHECK message from this extension is not
+// safe against every libstdc++ the torch wheels are built with.
+std::string dims(c10::IntArrayRef v) {
+  std::string s = "[";
+  for (size_t i = 0; i < v.size(); ++i) s += (i ? ", " : "") + std::to_string(v[i]);
+  return s + "]";
 }
 
-rb::Operand operand(const Tensor& t, bool mn_major, const char* name) {
-  chk_bf16(t, name);
-  chk_2d_rowmajor(t, name);
-  rb::Operand o;
-  o.ptr = t.data_ptr();
-  o.ld = t.stride(0);
-  o.mn_major = mn_major;
-  return o;
+// Checks one tensor argument of binding c.fn and returns its data pointer.  The tensor must be a CUDA tensor on c.dev of
+// dtype `dt` (at::kByte: any one-byte type) that covers `shape`, the extent the kernel touches:
+//   - one entry: at least shape[0] elements of a contiguous tensor of any rank;
+//   - more: that rank, a unit inner stride and at least shape[d] entries in dimension d; `strides`, if given, pins the
+//     stride of every outer dimension (a kernel that derives the pitch itself).
+// `align` (bytes) is what the kernel's vector or TMA accesses need of the base and of every outer stride.  As for
+// is_contiguous(), the stride of a dimension of size 1 is never used and not checked.
+template <class T = void>
+T* arg(const Call& c, const Tensor& t, const char* name, at::ScalarType dt, c10::IntArrayRef shape, int64_t align = 1,
+       c10::IntArrayRef strides = {}) {
+  TORCH_CHECK(t.is_cuda() && t.device() == c.dev, c.fn, ": ", name, " must be a CUDA tensor on ", c.dev.str(), ", got ", t.device().str());
+  TORCH_CHECK(dt == at::kByte ? t.element_size() == 1 : t.scalar_type() == dt, c.fn, ": ", name, " must be ",
+              dt == at::kByte ? "a one-byte type" : c10::toString(dt), ", got ", c10::toString(t.scalar_type()));
+  const int64_t r = (int64_t)shape.size();
+  if (r == 1) {
+    TORCH_CHECK(t.is_contiguous(), c.fn, ": ", name, " must be contiguous");
+    TORCH_CHECK(t.numel() >= shape[0], c.fn, ": ", name, " has ", std::to_string(t.numel()), " elements, smaller than the ",
+                std::to_string(shape[0]), " expected");
+  } else {
+    TORCH_CHECK(t.dim() == r && t.stride(r - 1) == 1, c.fn, ": ", name, " must be ", std::to_string(r), "-D with unit inner stride, got sizes ",
+                dims(t.sizes()), " and strides ", dims(t.strides()));
+    for (int64_t d = 0; d < r; ++d)
+      TORCH_CHECK(t.size(d) >= shape[d], c.fn, ": ", name, " ", dims(t.sizes()), " is smaller than the ", dims(shape), " expected");
+    for (int64_t d = 0; d + 1 < r && !strides.empty(); ++d)
+      TORCH_CHECK(t.size(d) <= 1 || t.stride(d) == strides[d], c.fn, ": ", name, " must have strides ", dims(strides), " in its outer dimensions, got ",
+                  dims(t.strides()));
+  }
+  bool aligned = reinterpret_cast<uintptr_t>(t.data_ptr()) % align == 0;
+  for (int64_t d = 0; d + 1 < r; ++d) aligned = aligned && (t.size(d) <= 1 || t.stride(d) * t.element_size() % align == 0);
+  TORCH_CHECK(aligned, c.fn, ": ", name, " needs a ", std::to_string(align), "-byte-aligned base and row pitch, got strides ",
+              dims(t.strides()));
+  return static_cast<T*>(t.data_ptr());
+}
+// optional tensors: nullptr when absent
+template <class T = void>
+T* arg(const Call& c, const OptTensor& t, const char* name, at::ScalarType dt, c10::IntArrayRef shape, int64_t align = 1,
+       c10::IntArrayRef strides = {}) {
+  return t.has_value() ? arg<T>(c, *t, name, dt, shape, align, strides) : nullptr;
 }
 
-rb::Fp8Out fp8_out(const OptTensor& q8, const OptTensor& inv_scale, const OptTensor& amax, int64_t rows, int64_t cols) {
+// The LoRA-dropout arguments of one call: the device seed (absent: seed 0), min_keys .. max_keys mask keys (one per group)
+// and p in [0, 1).
+struct Dropout {
+  const uint32_t* seed = nullptr;
+  uint32_t keys[4] = {0, 0, 0, 0};
+  int groups = 0;
+  uint32_t thr16 = 0;  // round(p * 65536)
+  float inv_keep = 1.f;
+  rb::LnDrop ln() const { return {seed, thr16, inv_keep}; }
+};
+Dropout dropout(const Call& c, const OptTensor& seed, const std::vector<int64_t>& keys, double p, int min_keys, int max_keys) {
+  const int n = (int)keys.size();
+  TORCH_CHECK(n >= min_keys && n <= max_keys, c.fn, ": ", std::to_string(n), " dropout keys, expected ", std::to_string(min_keys), " to ",
+              std::to_string(max_keys));
+  TORCH_CHECK(p >= 0.0 && p < 1.0, c.fn, ": dropout p must be in [0, 1), got ", std::to_string(p));
+  Dropout d;
+  d.seed = arg<const uint32_t>(c, seed, "seed", at::kInt, {1});
+  d.groups = n;
+  for (int i = 0; i < n; ++i) d.keys[i] = (uint32_t)keys[i];
+  d.thr16 = (uint32_t)llround(p * 65536.0);
+  d.inv_keep = (float)(1.0 / (1.0 - p));
+  return d;
+}
+
+rb::Fp8Out fp8_out(const Call& c, const OptTensor& q8, const OptTensor& inv_scale, const OptTensor& amax, int64_t rows, int64_t cols) {
   rb::Fp8Out f;
   if (!q8.has_value()) return f;
-  TORCH_CHECK(q8->is_cuda() && q8->element_size() == 1 && q8->dim() == 2 && q8->stride(1) == 1 && q8->size(0) == rows && q8->size(1) == cols,
-              "fp8 output: one-byte [rows, cols] tensor");
-  TORCH_CHECK(inv_scale.has_value() && amax.has_value(), "fp8 output needs inv_scale and amax");
-  f.q = reinterpret_cast<uint8_t*>(q8->data_ptr()); f.ld = q8->stride(0);
-  f.inv_scale = f32ptr(inv_scale); f.amax = const_cast<float*>(f32ptr(amax));
+  TORCH_CHECK(inv_scale.has_value() && amax.has_value(), c.fn, ": the fp8 output q8 needs q_inv_scale and q_amax");
+  f.q = arg<uint8_t>(c, q8, "q8", at::kByte, {rows, cols}, 8);  // 8-byte stores
+  f.ld = q8->stride(0);
+  f.inv_scale = arg<const float>(c, inv_scale, "q_inv_scale", F32, {1});
+  f.amax = arg<float>(c, amax, "q_amax", F32, {1});
   return f;
 }
 
@@ -65,449 +121,329 @@ void gemm(const Tensor& a1, const Tensor& b1, Tensor& out, int64_t M, int64_t N,
           const OptTensor& residual, double alpha, bool accumulate, int64_t block_n, int64_t split_k, int64_t b1_group_kofs,
           bool b1_local_n, int64_t m_per_group, int64_t b1_mn_ofs_per_mgroup, const OptTensor& bias, int64_t pair, int64_t fp8,
           const OptTensor& alpha_dev) {
-  c10::cuda::CUDAGuard guard(out.device());
+  const Call c{"gemm", out.device()};
   rb::GemmDesc d;
-  if (fp8) {
-    // E4M3 bytes (torch.uint8 / float8_e4m3fn storage), K-major; leading dimensions in bytes
-    TORCH_CHECK(!a1_mn && !b1_mn, "fp8 operands must be K-major");
-    for (const Tensor* t : {&a1, &b1}) {
-      TORCH_CHECK(t->is_cuda() && t->element_size() == 1 && t->dim() == 2 && t->stride(1) == 1, "fp8 operands: 2-D one-byte CUDA tensors");
-    }
-    d.a1.ptr = a1.data_ptr(); d.a1.ld = a1.stride(0); d.a1.mn_major = false;
-    d.b1.ptr = b1.data_ptr(); d.b1.ld = b1.stride(0); d.b1.mn_major = false;
-    d.fp8 = true; d.fp8_a_e5m2 = fp8 == 2;
-  } else {
-    d.a1 = operand(a1, a1_mn, "a1");
-    d.b1 = operand(b1, b1_mn, "b1");
-  }
-  if (alpha_dev.has_value()) d.alpha_dev = f32ptr(alpha_dev);
   d.M = (int)M; d.N = (int)N; d.K1 = (int)K1; d.K2 = (int)K2;
-  if (K2 > 0) {
-    TORCH_CHECK(a2.has_value() && b2.has_value(), "a2/b2 required when K2 > 0");
-    d.a2 = operand(*a2, false, "a2");
-    d.b2 = operand(*b2, false, "b2");
-  }
+  d.a1.mn_major = a1_mn; d.b1.mn_major = b1_mn;
+  d.fp8 = fp8 != 0; d.fp8_a_e5m2 = fp8 == 2;  // E4M3 / E5M2 bytes (torch.uint8 / float8 storage), leading dimensions in bytes
   d.n_per_group = (int)n_per_group; d.a1_group_kofs = (int)a1_group_kofs; d.a2_group_kofs = (int)a2_group_kofs;
-  TORCH_CHECK(out.is_cuda() && out.dim() == 2 && out.stride(1) == 1, "out must be 2-D row-major CUDA");
-  TORCH_CHECK(out.scalar_type() == at::kBFloat16 || out.scalar_type() == at::kFloat, "out must be bf16 or fp32");
-  TORCH_CHECK(out.size(0) >= M && out.size(1) >= N, "out too small");
-  d.out = out.data_ptr(); d.ldc = out.stride(0); d.out_f32 = out.scalar_type() == at::kFloat;
-  d.accumulate = accumulate; d.alpha = (float)alpha; d.block_n = (int)block_n; d.split_k = (int)split_k; d.pair = (int)pair;
   d.b1_group_kofs = (int)b1_group_kofs; d.b1_local_n = b1_local_n; d.m_per_group = (int)m_per_group;
   d.b1_mn_ofs_per_mgroup = (int)b1_mn_ofs_per_mgroup;
-  if (residual.has_value()) {
-    chk_bf16(*residual, "residual");
-    chk_2d_rowmajor(*residual, "residual");
-    d.residual = residual->data_ptr(); d.ldr = residual->stride(0);
+  d.accumulate = accumulate; d.alpha = (float)alpha; d.block_n = (int)block_n; d.split_k = (int)split_k; d.pair = (int)pair;
+  TORCH_CHECK(K2 <= 0 || (a2.has_value() && b2.has_value()), "gemm: a2 and b2 are required when K2 > 0");
+  // the tensor maps span these extents, so each operand must cover them
+  const rb::GemmExtents e = rb::gemm_operand_extents(d);
+  const auto in = d.fp8 ? at::kByte : BF;
+  d.a1.ptr = arg(c, a1, "a1", in, {e.a1.rows, e.a1.cols}, 16); d.a1.ld = a1.stride(0);
+  d.b1.ptr = arg(c, b1, "b1", in, {e.b1.rows, e.b1.cols}, 16); d.b1.ld = b1.stride(0);
+  if (K2 > 0) {
+    d.a2.ptr = arg(c, a2, "a2", BF, {e.a2.rows, e.a2.cols}, 16); d.a2.ld = a2->stride(0);
+    d.b2.ptr = arg(c, b2, "b2", BF, {e.b2.rows, e.b2.cols}, 16); d.b2.ld = b2->stride(0);
   }
-  if (bias.has_value()) {
-    chk_bf16(*bias, "bias");
-    TORCH_CHECK(bias->is_contiguous() && bias->numel() >= N, "bias must be contiguous [N]");
-    d.bias = bias->data_ptr();
-  }
+  d.out_f32 = out.scalar_type() == F32;
+  d.out = arg(c, out, "out", d.out_f32 ? F32 : BF, {M, N}); d.ldc = out.stride(0);
+  d.residual = arg(c, residual, "residual", BF, {M, N}); d.ldr = residual.has_value() ? residual->stride(0) : 0;
+  d.bias = arg(c, bias, "bias", BF, {N});
+  d.alpha_dev = arg<const float>(c, alpha_dev, "alpha_dev", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
   rb::gemm_bf16(d, cur_stream());
 }
 
 void rmsnorm_fwd(const Tensor& x, const Tensor& w, Tensor& y, Tensor& rstd, double eps, const OptTensor& xd, const OptTensor& seed,
                  std::vector<int64_t> keys, double p, const OptTensor& q8, const OptTensor& q_inv_scale, const OptTensor& q_amax) {
-  chk_bf16(x, "x"); chk_bf16(w, "w"); chk_bf16(y, "y");
-  TORCH_CHECK(x.is_contiguous() && y.is_contiguous() && w.is_contiguous(), "rmsnorm: contiguous tensors required");
-  const int H = (int)x.size(-1);
-  const int M = (int)(x.numel() / H);
-  c10::cuda::CUDAGuard guard(x.device());
-  uint32_t k[4] = {0, 0, 0, 0};
-  int G = 0;
-  void* xdp = nullptr;
-  if (xd.has_value()) {
-    chk_bf16(*xd, "xd");
-    TORCH_CHECK(xd->is_contiguous(), "xd must be contiguous");
-    G = (int)keys.size();
-    TORCH_CHECK(G >= 1 && G <= 4 && xd->numel() == (int64_t)M * G * H, "xd must be [M, G*H]");
-    for (int i = 0; i < G; ++i) k[i] = (uint32_t)keys[i];
-    xdp = xd->data_ptr();
-  }
-  const uint32_t thr = (uint32_t)llround(p * 65536.0);
-  rb::rmsnorm_fwd(x.data_ptr(), w.data_ptr(), y.data_ptr(), rstd.data_ptr<float>(), M, H, (float)eps, xdp, G, u32ptr(seed), k, thr,
-                  (float)(1.0 / (1.0 - p)), fp8_out(q8, q_inv_scale, q_amax, M, H), cur_stream());
+  const Call c{"rmsnorm_fwd", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0}, 16);
+  const int64_t H = x.size(-1), M = x.numel() / H;
+  const Dropout dr = dropout(c, seed, keys, p, xd.has_value() ? 1 : 0, 4);
+  const int G = xd.has_value() ? dr.groups : 0;
+  void* xdp = arg(c, xd, "xd", BF, {M * G * H}, 16);
+  const void* wp = arg(c, w, "w", BF, {H}, 16);
+  void* yp = arg(c, y, "y", BF, {M * H}, 16);
+  float* rp = arg<float>(c, rstd, "rstd", F32, {M});
+  const rb::Fp8Out f8 = fp8_out(c, q8, q_inv_scale, q_amax, M, H);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::rmsnorm_fwd(xp, wp, yp, rp, (int)M, (int)H, (float)eps, xdp, G, dr.seed, dr.keys, dr.thr16, dr.inv_keep, f8, cur_stream());
 }
 
 void rmsnorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& w, const Tensor& rstd, const OptTensor& dx_add, Tensor& dx, Tensor& dw,
                  const OptTensor& ws, const OptTensor& ticket) {
-  chk_bf16(dy, "dy"); chk_bf16(x, "x"); chk_bf16(w, "w"); chk_bf16(dx, "dx");
-  TORCH_CHECK(dw.scalar_type() == at::kFloat && dw.is_contiguous(), "dw must be fp32");
-  TORCH_CHECK(dy.is_contiguous() && x.is_contiguous() && dx.is_contiguous(), "rmsnorm_bwd: contiguous tensors required");
-  const int H = (int)x.size(-1);
-  const int M = (int)(x.numel() / H);
-  c10::cuda::CUDAGuard guard(x.device());
-  const void* add = nullptr;
-  if (dx_add.has_value()) { chk_bf16(*dx_add, "dx_add"); TORCH_CHECK(dx_add->is_contiguous()); add = dx_add->data_ptr(); }
-  float* wsp = nullptr;
-  unsigned int* tk = nullptr;
-  if (ws.has_value() && ticket.has_value()) {
-    TORCH_CHECK(ws->scalar_type() == at::kFloat && ws->numel() >= (int64_t)rb::rmsnorm_bwd_ws_blocks() * H, "rmsnorm workspace too small");
-    TORCH_CHECK(ticket->scalar_type() == at::kInt && ticket->numel() >= 1, "ticket must be int32");
-    wsp = ws->data_ptr<float>();
-    tk = reinterpret_cast<unsigned int*>(ticket->data_ptr<int32_t>());
-  }
-  rb::rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), rstd.data_ptr<float>(), add, dx.data_ptr(), dw.data_ptr<float>(), M, H,
-                  wsp, tk, cur_stream());
+  const Call c{"rmsnorm_bwd", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0}, 16);
+  const int64_t H = x.size(-1), M = x.numel() / H;
+  const void* dyp = arg(c, dy, "dy", BF, {M * H}, 16);
+  const void* wp = arg(c, w, "w", BF, {H}, 16);
+  const float* rp = arg<const float>(c, rstd, "rstd", F32, {M});
+  const void* add = arg(c, dx_add, "dx_add", BF, {M * H}, 16);
+  void* dxp = arg(c, dx, "dx", BF, {M * H}, 16);
+  float* dwp = arg<float>(c, dw, "dw", F32, {H});
+  // the warp-per-row kernel runs only with both its workspace and ticket
+  const bool warp = ws.has_value() && ticket.has_value();
+  float* wsp = warp ? arg<float>(c, ws, "ws", F32, {rb::rmsnorm_bwd_ws_blocks() * H}) : nullptr;
+  auto* tk = warp ? arg<unsigned int>(c, ticket, "ticket", at::kInt, {1}) : nullptr;
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::rmsnorm_bwd(dyp, xp, wp, rp, add, dxp, dwp, (int)M, (int)H, wsp, tk, cur_stream());
 }
 
 void dropout_expand(const Tensor& x, Tensor& xd, const OptTensor& seed, std::vector<int64_t> keys, double p, const OptTensor& q8,
                     const OptTensor& q_inv_scale, const OptTensor& q_amax) {
-  chk_bf16(x, "x"); chk_bf16(xd, "xd");
-  TORCH_CHECK(x.is_contiguous() && xd.is_contiguous());
-  const int H = (int)x.size(-1);
-  const int M = (int)(x.numel() / H);
-  const int G = (int)keys.size();
-  TORCH_CHECK(xd.numel() == (int64_t)M * G * H, "xd must be [M, G*H]");
-  uint32_t k[4] = {0, 0, 0, 0};
-  for (int i = 0; i < G && i < 4; ++i) k[i] = (uint32_t)keys[i];
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::dropout_expand(x.data_ptr(), xd.data_ptr(), M, H, G, u32ptr(seed), k, (uint32_t)llround(p * 65536.0), (float)(1.0 / (1.0 - p)),
-                     fp8_out(q8, q_inv_scale, q_amax, M, H), cur_stream());
+  const Call c{"dropout_expand", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0}, 16);
+  const int64_t H = x.size(-1), M = x.numel() / H;
+  const Dropout dr = dropout(c, seed, keys, p, 1, 4);
+  void* xdp = arg(c, xd, "xd", BF, {M * dr.groups * H}, 16);
+  const rb::Fp8Out f8 = fp8_out(c, q8, q_inv_scale, q_amax, M, H);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::dropout_expand(xp, xdp, (int)M, (int)H, dr.groups, dr.seed, dr.keys, dr.thr16, dr.inv_keep, f8, cur_stream());
 }
 
 void dropout_combine(const OptTensor& base, const Tensor& parts, Tensor& out, const OptTensor& seed, std::vector<int64_t> keys, double p) {
-  // parts: either [G, M, H] contiguous, or [M, G*H] row-major (group g at column offset g*H)
-  chk_bf16(parts, "parts"); chk_bf16(out, "out");
-  TORCH_CHECK(out.dim() == 2 && out.is_contiguous(), "out must be contiguous [M, H]");
-  const int M = (int)out.size(0), H = (int)out.size(1);
-  const int G = (int)keys.size();
-  long long part_stride, ld_parts;
-  if (parts.dim() == 3) {
-    TORCH_CHECK(parts.is_contiguous() && parts.size(0) == G && parts.size(1) == M && parts.size(2) == H, "parts must be [G, M, H]");
-    part_stride = (long long)M * H; ld_parts = H;
-  } else {
-    TORCH_CHECK(parts.dim() == 2 && parts.stride(1) == 1 && parts.size(0) == M && parts.size(1) == (int64_t)G * H, "parts must be [M, G*H]");
-    part_stride = H; ld_parts = parts.stride(0);
-  }
-  uint32_t k[4] = {0, 0, 0, 0};
-  for (int i = 0; i < G && i < 4; ++i) k[i] = (uint32_t)keys[i];
-  const void* bp = nullptr;
-  if (base.has_value()) { chk_bf16(*base, "base"); TORCH_CHECK(base->is_contiguous() && base->numel() == out.numel()); bp = base->data_ptr(); }
-  c10::cuda::CUDAGuard guard(out.device());
-  rb::dropout_combine(bp, parts.data_ptr(), part_stride, ld_parts, out.data_ptr(), M, H, G, u32ptr(seed), k,
-                      (uint32_t)llround(p * 65536.0), (float)(1.0 / (1.0 - p)), cur_stream());
+  const Call c{"dropout_combine", out.device()};
+  void* op = arg(c, out, "out", BF, {0, 0}, 16, {out.size(-1)});
+  const int64_t M = out.size(0), H = out.size(1);
+  const Dropout dr = dropout(c, seed, keys, p, 1, 4);
+  const int64_t G = dr.groups;
+  // parts: [G, M, H] contiguous, or [M, G*H] row-major with group g at column offset g*H
+  const bool stacked = parts.dim() == 3;
+  const void* pp = stacked ? arg(c, parts, "parts", BF, {G, M, H}, 16, {M * H, H}) : arg(c, parts, "parts", BF, {M, G * H}, 16);
+  const void* bp = arg(c, base, "base", BF, {M * H}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::dropout_combine(bp, pp, stacked ? M * H : H, stacked ? H : parts.stride(0), op, (int)M, (int)H, (int)G, dr.seed, dr.keys,
+                      dr.thr16, dr.inv_keep, cur_stream());
 }
 
 void fp8_quantize_weight(const Tensor& w, Tensor& w8, Tensor& scratch, Tensor& scale, Tensor& inv_scale, const OptTensor& w8t) {
-  chk_bf16(w, "w"); chk_2d_rowmajor(w, "w");
-  TORCH_CHECK(w8.is_cuda() && w8.element_size() == 1 && w8.dim() == 2 && w8.stride(1) == 1 && w8.sizes() == w.sizes(), "w8: one-byte tensor shaped like w");
-  void* tp = nullptr;
-  long long tld = 0;
-  if (w8t.has_value()) {
-    TORCH_CHECK(w8t->is_cuda() && w8t->element_size() == 1 && w8t->dim() == 2 && w8t->stride(1) == 1 && w8t->size(0) == w.size(1) && w8t->size(1) == w.size(0),
-                "w8t: one-byte tensor shaped like w transposed");
-    tp = w8t->data_ptr(); tld = w8t->stride(0);
-  }
-  c10::cuda::CUDAGuard guard(w.device());
-  rb::fp8_quantize_weight(w.data_ptr(), w.stride(0), w8.data_ptr(), w8.stride(0), tp, tld, (int)w.size(0), (int)w.size(1),
-                          const_cast<float*>(f32ptr(scratch)), const_cast<float*>(f32ptr(scale)), const_cast<float*>(f32ptr(inv_scale)),
+  const Call c{"fp8_quantize_weight", w.device()};
+  const void* wp = arg(c, w, "w", BF, {0, 0}, 16);
+  const int64_t R = w.size(0), C = w.size(1);
+  void* w8p = arg(c, w8, "w8", at::kByte, {R, C}, 16);
+  void* tp = arg(c, w8t, "w8t", at::kByte, {C, R});
+  float* sp = arg<float>(c, scratch, "scratch", F32, {1});
+  float* scp = arg<float>(c, scale, "scale", F32, {1});
+  float* isp = arg<float>(c, inv_scale, "inv_scale", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::fp8_quantize_weight(wp, w.stride(0), w8p, w8.stride(0), tp, w8t.has_value() ? w8t->stride(0) : 0, (int)R, (int)C, sp, scp, isp,
                           cur_stream());
 }
 void fp8_quantize_act(const Tensor& x, Tensor& x8, const Tensor& inv_scale, const OptTensor& amax_cur, bool e5m2) {
-  chk_bf16(x, "x"); chk_2d_rowmajor(x, "x");
-  TORCH_CHECK(x8.is_cuda() && x8.element_size() == 1 && x8.dim() == 2 && x8.stride(1) == 1 && x8.sizes() == x.sizes(), "x8: one-byte tensor shaped like x");
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::fp8_quantize_act(x.data_ptr(), x.stride(0), x8.data_ptr(), x8.stride(0), (int)x.size(0), (int)x.size(1), f32ptr(inv_scale),
-                       const_cast<float*>(f32ptr(amax_cur)), e5m2, cur_stream());
+  const Call c{"fp8_quantize_act", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0, 0}, 16);
+  const int64_t R = x.size(0), C = x.size(1);
+  void* x8p = arg(c, x8, "x8", at::kByte, {R, C}, 16);
+  const float* isp = arg<const float>(c, inv_scale, "inv_scale", F32, {1});
+  float* ap = arg<float>(c, amax_cur, "amax_cur", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::fp8_quantize_act(xp, x.stride(0), x8p, x8.stride(0), (int)R, (int)C, isp, ap, e5m2, cur_stream());
 }
 void fp8_prep(Tensor& state, const Tensor& w_scale, Tensor& inv_sx, Tensor& alpha_main, Tensor& alpha_inv, double margin, int64_t n_e4m3) {
-  const int n = (int)w_scale.numel();
-  TORCH_CHECK(state.numel() == 2 * n && inv_sx.numel() == n && alpha_main.numel() == n && alpha_inv.numel() == n, "fp8_prep: size mismatch");
-  TORCH_CHECK(state.is_contiguous() && w_scale.is_contiguous() && inv_sx.is_contiguous() && alpha_main.is_contiguous() && alpha_inv.is_contiguous());
-  c10::cuda::CUDAGuard guard(state.device());
-  rb::fp8_prep(const_cast<float*>(f32ptr(state)), f32ptr(w_scale), const_cast<float*>(f32ptr(inv_sx)), const_cast<float*>(f32ptr(alpha_main)),
-               const_cast<float*>(f32ptr(alpha_inv)), n, (float)margin, n_e4m3 < 0 ? n : (int)n_e4m3, cur_stream());
+  const Call c{"fp8_prep", w_scale.device()};
+  const float* wsp = arg<const float>(c, w_scale, "w_scale", F32, {0});
+  const int64_t n = w_scale.numel();
+  float* sp = arg<float>(c, state, "state", F32, {2 * n});
+  float* ip = arg<float>(c, inv_sx, "inv_sx", F32, {n});
+  float* mp = arg<float>(c, alpha_main, "alpha_main", F32, {n});
+  float* ap = arg<float>(c, alpha_inv, "alpha_inv", F32, {n});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::fp8_prep(sp, wsp, ip, mp, ap, (int)n, (float)margin, n_e4m3 < 0 ? (int)n : (int)n_e4m3, cur_stream());
 }
 
 // out[M,N] = dy[M,Kb]·W[Kb,N] + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)     (fused input gradient of a stacked LoRA group)
 void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Tensor& a, Tensor& out, const OptTensor& seed,
              std::vector<int64_t> keys, double p, const OptTensor& base, int64_t pair) {
-  chk_bf16(du, "du"); chk_bf16(a, "a"); chk_bf16(out, "out");
-  chk_2d_rowmajor(du, "du"); chk_2d_rowmajor(a, "a"); chk_2d_rowmajor(out, "out");
-  const int G = (int)keys.size();
-  TORCH_CHECK(G >= 1 && G <= 3, "lora_dx: 1..3 groups");
+  const Call c{"lora_dx", out.device()};
+  const Dropout dr = dropout(c, seed, keys, p, 1, 3);
   rb::LoraDxDesc d;
-  d.M = (int)du.size(0); d.N = (int)a.size(1); d.groups = G;
-  TORCH_CHECK(du.size(1) % G == 0, "du must be [M, G*r]");
-  d.r = (int)(du.size(1) / G);
-  TORCH_CHECK(a.size(0) == du.size(1), "a must be [G*r, N]");
-  TORCH_CHECK(out.size(0) == d.M && out.size(1) == d.N, "out must be [M, N]");
+  d.groups = dr.groups;
+  d.du = arg(c, du, "du", BF, {0, 0}, 16); d.ld_du = du.stride(0);
+  const int64_t du_cols = du.size(1);  // du = [du_0 | du_1 | ...], [M, G*r]
+  TORCH_CHECK(du_cols % d.groups == 0, "lora_dx: du must be [M, G*r] for the G = ", std::to_string(d.groups), " dropout keys");
+  d.M = (int)du.size(0); d.r = (int)(du_cols / d.groups);
+  d.a = arg(c, a, "a", BF, {(int64_t)d.groups * d.r, 0}, 16); d.ld_a = a.stride(0);
+  d.N = (int)a.size(1);
+  d.out = arg(c, out, "out", BF, {d.M, d.N}, 16); d.ldc = out.stride(0);
   if (base.has_value()) {
     // two-kernel form: base = dy·W from the plain GEMM, this launch adds the masked low-rank terms
-    chk_bf16(*base, "base"); chk_2d_rowmajor(*base, "base");
-    TORCH_CHECK(base->size(0) == d.M && base->size(1) == d.N, "base must be [M, N]");
-    d.base = base->data_ptr(); d.ld_base = base->stride(0); d.Kb = 0;
+    d.base = arg(c, base, "base", BF, {d.M, d.N}, 16); d.ld_base = base->stride(0); d.Kb = 0;
   } else {
     TORCH_CHECK(dy.has_value() && w.has_value(), "lora_dx: pass (dy, w) or base");
-    chk_bf16(*dy, "dy"); chk_bf16(*w, "w"); chk_2d_rowmajor(*dy, "dy"); chk_2d_rowmajor(*w, "w");
+    d.dy = arg(c, dy, "dy", BF, {d.M, 0}, 16); d.ld_dy = dy->stride(0);
     d.Kb = (int)dy->size(1);
-    TORCH_CHECK(dy->size(0) == d.M && w->size(0) == d.Kb && w->size(1) == d.N, "dy must be [M, Kb], w [Kb, N]");
-    d.dy = dy->data_ptr(); d.ld_dy = dy->stride(0);
-    d.w = w->data_ptr(); d.ld_w = w->stride(0);
+    d.w = arg(c, w, "w", BF, {d.Kb, d.N}, 16); d.ld_w = w->stride(0);
   }
-  d.du = du.data_ptr(); d.ld_du = du.stride(0);
-  d.a = a.data_ptr(); d.ld_a = a.stride(0);
-  d.out = out.data_ptr(); d.ldc = out.stride(0);
-  d.drop_threshold16 = (uint32_t)llround(p * 65536.0);
-  d.inv_keep = (float)(1.0 / (1.0 - p));
-  d.seed_ptr = u32ptr(seed);
-  for (int i = 0; i < G; ++i) d.seed_key[i] = (uint32_t)keys[i];
+  d.drop_threshold16 = dr.thr16; d.inv_keep = dr.inv_keep; d.seed_ptr = dr.seed;
+  for (int i = 0; i < 3; ++i) d.seed_key[i] = dr.keys[i];
   d.pair = (int)pair;
-  c10::cuda::CUDAGuard guard(out.device());
+  c10::cuda::CUDAGuard guard(c.dev);
   rb::lora_dx(d, cur_stream());
 }
 
-// The attention kernels read out rows with 16-byte loads and store 4-byte pairs into out / dqkv, so those tensors obey the
-// rule the TMA maps enforce for qkv / dout: a 16-byte-aligned base and a row pitch that is a multiple of 8 elements.
-void chk_attn_rows(const Tensor& t, const char* name) {
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0 && t.stride(0) % 8 == 0, "attention: ", name,
-              " needs a 16-byte-aligned base and a row pitch that is a multiple of 8 elements");
-}
-
-// causal flash attention over the packed (post-RoPE) qkv buffer [B*T, (nh + 2*nkv)*hd]; nkv < 0 means nkv = nh
+// causal flash attention over the packed (post-RoPE) qkv buffer [B*T, (nh + 2*nkv)*hd]; nkv < 0 means nkv = nh.  The kernels
+// read out rows with 16-byte loads and store 4-byte pairs into out / dqkv, so those tensors obey the rule the TMA maps enforce
+// for qkv / dout: a 16-byte-aligned base and row pitch.
 void attention_fwd(const Tensor& qkv, Tensor& out, Tensor& lse, int64_t B, int64_t T, int64_t nh, int64_t hd, double scale, bool interleaved,
                    int64_t nkv) {
   if (nkv < 0) nkv = nh;
-  chk_bf16(qkv, "qkv"); chk_bf16(out, "out"); chk_2d_rowmajor(qkv, "qkv"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == (nh + 2 * nkv) * hd, "qkv must be [B*T, (nh+2*nkv)*hd]");
-  TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd, "out must be [B*T, nh*hd]");
-  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
-  chk_attn_rows(out, "out");
+  const Call c{"attention_fwd", qkv.device()};
   rb::AttnDesc d;
-  d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0); d.lse = lse.data_ptr<float>();
+  d.qkv = arg(c, qkv, "qkv", BF, {B * T, (nh + 2 * nkv) * hd}, 16); d.ld_qkv = qkv.stride(0);
+  d.out = arg(c, out, "out", BF, {B * T, nh * hd}, 16); d.ld_out = out.stride(0);
+  d.lse = arg<float>(c, lse, "lse", F32, {B * nh * T});
   d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.nkv = (int)nkv; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
-  c10::cuda::CUDAGuard guard(qkv.device());
+  c10::cuda::CUDAGuard guard(c.dev);
   rb::attention_fwd(d, cur_stream());
 }
 void attention_bwd(const Tensor& qkv, const Tensor& out, const Tensor& dout, const Tensor& lse, Tensor& delta, Tensor& dqkv, int64_t B,
                    int64_t T, int64_t nh, int64_t hd, double scale, const OptTensor& ds_workspace, bool interleaved, int64_t nkv) {
   if (nkv < 0) nkv = nh;
-  chk_bf16(qkv, "qkv"); chk_bf16(out, "out"); chk_bf16(dout, "dout"); chk_bf16(dqkv, "dqkv");
-  chk_2d_rowmajor(qkv, "qkv"); chk_2d_rowmajor(out, "out"); chk_2d_rowmajor(dout, "dout"); chk_2d_rowmajor(dqkv, "dqkv");
-  TORCH_CHECK(qkv.size(0) == B * T && qkv.size(1) == (nh + 2 * nkv) * hd && dqkv.size(0) == B * T && dqkv.size(1) == (nh + 2 * nkv) * hd,
-              "qkv / dqkv must be [B*T, (nh+2*nkv)*hd]");
-  TORCH_CHECK(out.size(0) == B * T && out.size(1) == nh * hd && dout.size(0) == B * T && dout.size(1) == nh * hd, "out / dout must be [B*T, nh*hd]");
-  TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * nh * T, "lse must be fp32 [B, nh, T]");
-  TORCH_CHECK(delta.is_cuda() && delta.scalar_type() == at::kFloat && delta.is_contiguous() && delta.numel() == B * nh * T, "delta must be fp32 [B, nh, T]");
-  chk_attn_rows(out, "out");
-  chk_attn_rows(dqkv, "dqkv");
+  const Call c{"attention_bwd", qkv.device()};
   rb::AttnBwdDesc d;
-  d.qkv = qkv.data_ptr(); d.ld_qkv = qkv.stride(0); d.out = out.data_ptr(); d.ld_out = out.stride(0);
-  d.dout = dout.data_ptr(); d.ld_dout = dout.stride(0); d.lse = lse.data_ptr<float>(); d.delta = delta.data_ptr<float>();
-  d.dqkv = dqkv.data_ptr(); d.ld_dqkv = dqkv.stride(0);
+  d.qkv = arg(c, qkv, "qkv", BF, {B * T, (nh + 2 * nkv) * hd}, 16); d.ld_qkv = qkv.stride(0);
+  d.out = arg(c, out, "out", BF, {B * T, nh * hd}, 16); d.ld_out = out.stride(0);
+  d.dout = arg(c, dout, "dout", BF, {B * T, nh * hd}, 16); d.ld_dout = dout.stride(0);
+  d.lse = arg<float>(c, lse, "lse", F32, {B * nh * T});
+  d.delta = arg<float>(c, delta, "delta", F32, {B * nh * T});
+  d.dqkv = arg(c, dqkv, "dqkv", BF, {B * T, (nh + 2 * nkv) * hd}, 16); d.ld_dqkv = dqkv.stride(0);
+  d.ds_workspace = arg(c, ds_workspace, "ds_workspace", BF, {rb::attention_ds_workspace_elems((int)B, (int)T, (int)nh)});
   d.B = (int)B; d.T = (int)T; d.nh = (int)nh; d.nkv = (int)nkv; d.hd = (int)hd; d.scale = (float)scale; d.interleaved = interleaved;
-  if (ds_workspace.has_value()) {
-    chk_bf16(*ds_workspace, "ds_workspace");
-    TORCH_CHECK(ds_workspace->is_contiguous() && ds_workspace->numel() >= rb::attention_ds_workspace_elems((int)B, (int)T, (int)nh),
-                "ds_workspace too small (attention_ds_workspace_elems)");
-    d.ds_workspace = ds_workspace->data_ptr();
-  }
-  c10::cuda::CUDAGuard guard(qkv.device());
+  c10::cuda::CUDAGuard guard(c.dev);
   rb::attention_bwd(d, cur_stream());
 }
 
+// operand name of the bf16 rotary tables: rows are positions, pitch rotary_dim
+constexpr const char* kCos = "cos (rotary table [pos, rotary_dim])";
+constexpr const char* kSin = "sin (rotary table [pos, rotary_dim])";
+
 void rope_inplace(Tensor& buf, int64_t T, int64_t n_rot_heads, int64_t hd, int64_t rotary_dim, const Tensor& cos, const Tensor& sin,
                   bool backward, int64_t pos0) {
-  chk_bf16(buf, "buf"); chk_bf16(cos, "cos"); chk_bf16(sin, "sin");
-  chk_2d_rowmajor(buf, "buf");
-  TORCH_CHECK(cos.is_contiguous() && sin.is_contiguous() && cos.size(-1) == rotary_dim, "cos/sin must be [n_pos, rotary_dim]");
-  TORCH_CHECK(sin.sizes() == cos.sizes() && T + pos0 <= cos.size(0), "rotary table too short");
-  TORCH_CHECK(rotary_dim > 0 && rotary_dim <= hd && n_rot_heads * hd <= buf.size(1), "rope: rotary_dim <= hd and n_rot_heads * hd <= width");
+  TORCH_CHECK(rotary_dim > 0 && rotary_dim <= hd, "rope_inplace: rotary_dim must be in (0, hd]");
+  const Call c{"rope_inplace", buf.device()};
   // the scalar kernel (taken when the 16-byte one cannot run) moves element pairs with 4-byte accesses
-  for (const Tensor* t : std::initializer_list<const Tensor*>{&buf, &cos, &sin})
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 3) == 0, "rope: buf, cos and sin must be 4-byte aligned");
-  c10::cuda::CUDAGuard guard(buf.device());
-  rb::rope_inplace(buf.data_ptr(), buf.stride(0), (int)buf.size(0), (int)T, (int)n_rot_heads, (int)hd, (int)rotary_dim, cos.data_ptr(),
-                   sin.data_ptr(), backward, (int)pos0, cur_stream());
+  void* bp = arg(c, buf, "buf", BF, {0, n_rot_heads * hd}, 4);
+  const void* cp = arg(c, cos, kCos, BF, {T + pos0, rotary_dim}, 4, {rotary_dim});
+  const void* sp = arg(c, sin, kSin, BF, {T + pos0, rotary_dim}, 4, {rotary_dim});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::rope_inplace(bp, buf.stride(0), (int)buf.size(0), (int)T, (int)n_rot_heads, (int)hd, (int)rotary_dim, cp, sp, backward, (int)pos0,
+                   cur_stream());
 }
 
 // dq [B, nh, T, hd]; dk, dv [B, nkv, T, hd] (nkv < 0 means nh), nh % nkv == 0 -> out [B*T, (nh + 2*nkv)*hd]
 void rope_pack_bwd(const Tensor& dq, const Tensor& dk, const Tensor& dv, Tensor& out, int64_t rotary_dim, const Tensor& cos,
                    const Tensor& sin, int64_t pos0, int64_t nkv) {
-  chk_bf16(dq, "dq"); chk_bf16(dk, "dk"); chk_bf16(dv, "dv"); chk_bf16(out, "out"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(dq.dim() == 4 && dq.stride(3) == 1 && dk.dim() == 4 && dk.sizes() == dv.sizes(), "dq must be [B, nh, T, hd], dk/dv [B, nkv, T, hd]");
-  const int B = (int)dq.size(0), nh = (int)dq.size(1), T = (int)dq.size(2), hd = (int)dq.size(3);
+  const Call c{"rope_pack_bwd", out.device()};
+  const void* dqp = arg(c, dq, "dq", BF, {0, 0, 0, 0}, 16);
+  const int64_t B = dq.size(0), nh = dq.size(1), T = dq.size(2), hd = dq.size(3);
   if (nkv < 0) nkv = nh;
-  TORCH_CHECK(nkv > 0 && nh % nkv == 0 && dk.size(0) == B && dk.size(1) == nkv && dk.size(2) == T && dk.size(3) == hd,
-              "dk/dv must be [B, nkv, T, hd] with nh % nkv == 0");
-  TORCH_CHECK(dk.strides() == dv.strides() && dk.stride(3) == 1, "dk/dv must share strides");
-  TORCH_CHECK(nkv != nh || dq.strides() == dk.strides(), "dq/dk/dv must share strides");
-  TORCH_CHECK(out.size(0) == (int64_t)B * T && out.size(1) == (nh + 2 * nkv) * hd, "out must be [B*T, (nh+2*nkv)*hd]");
-  chk_bf16(cos, "cos"); chk_bf16(sin, "sin");
-  TORCH_CHECK(cos.is_contiguous() && sin.is_contiguous() && cos.dim() == 2 && cos.size(1) == rotary_dim && sin.sizes() == cos.sizes(),
-              "rope_pack_bwd: cos/sin must be [n_pos, rotary_dim]");
   TORCH_CHECK(rotary_dim > 0 && rotary_dim <= hd, "rope_pack_bwd: rotary_dim must be in (0, hd]");
-  TORCH_CHECK(T + pos0 <= cos.size(0), "rope_pack_bwd: rotary table too short for T + pos0");
-  for (const Tensor* t : std::initializer_list<const Tensor*>{&dq, &dk, &dv, &out, &cos, &sin})
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, "rope_pack_bwd: 16-byte aligned operands required");
-  c10::cuda::CUDAGuard guard(out.device());
-  rb::rope_pack_bwd(dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), dq.stride(0), dq.stride(1), dq.stride(2), dk.stride(0), dk.stride(1), dk.stride(2),
-                    out.data_ptr(), out.stride(0), B, T, nh, (int)nkv, hd, (int)rotary_dim, cos.data_ptr(), sin.data_ptr(), (int)pos0, cur_stream());
+  const void* dkp = arg(c, dk, "dk", BF, {B, nkv, T, hd}, 16);
+  const void* dvp = arg(c, dv, "dv", BF, {B, nkv, T, hd}, 16, dk.strides());  // dk and dv share the strides kB, kH, kT
+  void* op = arg(c, out, "out", BF, {B * T, (nh + 2 * nkv) * hd}, 16);
+  const void* cp = arg(c, cos, kCos, BF, {T + pos0, rotary_dim}, 16, {rotary_dim});
+  const void* sp = arg(c, sin, kSin, BF, {T + pos0, rotary_dim}, 16, {rotary_dim});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::rope_pack_bwd(dqp, dkp, dvp, dq.stride(0), dq.stride(1), dq.stride(2), dk.stride(0), dk.stride(1), dk.stride(2), op, out.stride(0),
+                    (int)B, (int)T, (int)nh, (int)nkv, (int)hd, (int)rotary_dim, cp, sp, (int)pos0, cur_stream());
 }
 
 void swiglu_fwd(const Tensor& gu, Tensor& h, const OptTensor& hd, const OptTensor& seed, int64_t key, double p, const OptTensor& q8,
                 const OptTensor& q_inv_scale, const OptTensor& q_amax) {
-  chk_bf16(gu, "gu"); chk_bf16(h, "h"); chk_2d_rowmajor(gu, "gu"); chk_2d_rowmajor(h, "h");
-  const int F = (int)h.size(1);
-  TORCH_CHECK(gu.size(1) == 2 * F && gu.size(0) == h.size(0));
-  void* hdp = nullptr;
-  long long ldhd = 0;
-  if (hd.has_value()) {
-    chk_bf16(*hd, "hd"); chk_2d_rowmajor(*hd, "hd");
-    TORCH_CHECK(hd->size(0) == h.size(0) && hd->size(1) == F, "hd must be [M, F]");
-    hdp = hd->data_ptr(); ldhd = hd->stride(0);
-  }
-  c10::cuda::CUDAGuard guard(gu.device());
-  rb::swiglu_fwd(gu.data_ptr(), gu.stride(0), h.data_ptr(), h.stride(0), (int)h.size(0), F, hdp, ldhd, u32ptr(seed), (uint32_t)key,
-                 (uint32_t)llround(p * 65536.0), (float)(1.0 / (1.0 - p)), fp8_out(q8, q_inv_scale, q_amax, h.size(0), F), cur_stream());
+  const Call c{"swiglu_fwd", h.device()};
+  void* hp = arg(c, h, "h", BF, {0, 0}, 16);
+  const int64_t M = h.size(0), F = h.size(1);
+  const void* gp = arg(c, gu, "gu", BF, {M, 2 * F}, 16);
+  void* hdp = arg(c, hd, "hd", BF, {M, F}, 16);
+  const Dropout dr = dropout(c, seed, {key}, p, 1, 1);
+  const rb::Fp8Out f8 = fp8_out(c, q8, q_inv_scale, q_amax, M, F);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::swiglu_fwd(gp, gu.stride(0), hp, h.stride(0), (int)M, (int)F, hdp, hd.has_value() ? hd->stride(0) : 0, dr.seed, dr.keys[0],
+                 dr.thr16, dr.inv_keep, f8, cur_stream());
 }
 void swiglu_bwd(const Tensor& dh, const Tensor& gu, Tensor& dgu) {
-  chk_bf16(dh, "dh"); chk_bf16(gu, "gu"); chk_bf16(dgu, "dgu");
-  chk_2d_rowmajor(dh, "dh"); chk_2d_rowmajor(gu, "gu"); chk_2d_rowmajor(dgu, "dgu");
-  const int F = (int)dh.size(1);
-  TORCH_CHECK(gu.size(1) == 2 * F && dgu.size(1) == 2 * F);
-  c10::cuda::CUDAGuard guard(gu.device());
-  rb::swiglu_bwd(dh.data_ptr(), dh.stride(0), gu.data_ptr(), gu.stride(0), dgu.data_ptr(), dgu.stride(0), (int)dh.size(0), F, cur_stream());
+  const Call c{"swiglu_bwd", dh.device()};
+  const void* dhp = arg(c, dh, "dh", BF, {0, 0}, 16);
+  const int64_t M = dh.size(0), F = dh.size(1);
+  const void* gp = arg(c, gu, "gu", BF, {M, 2 * F}, 16);
+  void* dgp = arg(c, dgu, "dgu", BF, {M, 2 * F}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::swiglu_bwd(dhp, dh.stride(0), gp, gu.stride(0), dgp, dgu.stride(0), (int)M, (int)F, cur_stream());
 }
 
 // ---------------------------------------------------------------------------------------------- block-scaled MXFP8
 int64_t mx_sf_bytes(int64_t rows, int64_t k) { return rb::mx_sf_bytes(rows, k); }
+int64_t pad128(int64_t n) { return (n + 127) / 128 * 128; }
+// the quantisers load 4 bf16 (8 bytes) or, for the weight, 8 bf16 (16 bytes) and store 4 bytes of q per access
 void mx_quantize_rows(const Tensor& x, Tensor& q, Tensor& sf) {
-  chk_bf16(x, "x"); chk_2d_rowmajor(x, "x");
-  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1 && q.size(0) >= x.size(0), "q must be uint8 [M, Kpad]");
-  TORCH_CHECK(sf.is_cuda() && sf.scalar_type() == at::kByte && sf.is_contiguous() && sf.numel() >= rb::mx_sf_bytes(x.size(0), x.size(1)), "sf too small");
-  TORCH_CHECK(q.size(1) >= (x.size(1) + 127) / 128 * 128, "mx_quantize_rows: q must be [M, >= K rounded up to 128]");
-  // the kernel loads 4 bf16 of x and stores 4 bytes of q per access
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(x.data_ptr()) & 7) == 0 && x.stride(0) % 4 == 0,
-              "mx_quantize_rows: x needs an 8-byte aligned base and a row pitch that is a multiple of 4 elements");
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(q.data_ptr()) & 3) == 0 && q.stride(0) % 4 == 0,
-              "mx_quantize_rows: q needs a 4-byte aligned base and a row pitch that is a multiple of 4");
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::mx_quantize_rows(x.data_ptr(), x.stride(0), q.data_ptr(), q.stride(0), sf.data_ptr(), (int)x.size(0), (int)x.size(1), cur_stream());
+  const Call c{"mx_quantize_rows", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0, 0}, 8);
+  const int64_t M = x.size(0), K = x.size(1);
+  void* qp = arg(c, q, "q", at::kByte, {M, pad128(K)}, 4);
+  void* sp = arg(c, sf, "sf", at::kByte, {rb::mx_sf_bytes(M, K)});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::mx_quantize_rows(xp, x.stride(0), qp, q.stride(0), sp, (int)M, (int)K, cur_stream());
 }
 void mx_quantize_weight_2d(const OptTensor& w, const OptTensor& delta, Tensor& q, Tensor& sf_fwd, Tensor& sf_bwd, int64_t N, int64_t K) {
-  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1, "q must be uint8 [Npad, Kpad]");
-  TORCH_CHECK(q.size(0) >= (N + 127) / 128 * 128 && q.size(1) >= (K + 127) / 128 * 128, "q must be padded to multiples of 128 in both dimensions");
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(q.data_ptr()) & 3) == 0 && q.stride(0) % 4 == 0,
-              "mx_quantize_weight_2d: q needs a 4-byte aligned base and a row pitch that is a multiple of 4");
-  TORCH_CHECK(sf_fwd.scalar_type() == at::kByte && sf_bwd.scalar_type() == at::kByte && sf_fwd.is_contiguous() && sf_bwd.is_contiguous());
-  TORCH_CHECK(sf_fwd.numel() >= rb::mx_sf_bytes(N, K) && sf_bwd.numel() >= rb::mx_sf_bytes(K, N), "scale buffers too small");
-  const void* wp = nullptr; long long ldw = 0;
-  if (w.has_value()) {
-    chk_bf16(*w, "w"); chk_2d_rowmajor(*w, "w"); TORCH_CHECK(w->size(0) == N && w->size(1) == K);
-    // the kernel loads 8 bf16 of w per access
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(w->data_ptr()) & 15) == 0 && w->stride(0) % 8 == 0,
-                "mx_quantize_weight_2d: w needs a 16-byte aligned base and a row pitch that is a multiple of 8 elements");
-    wp = w->data_ptr(); ldw = w->stride(0);
-  }
-  const float* dp = nullptr; long long ldd = 0;
-  if (delta.has_value()) {
-    TORCH_CHECK(delta->scalar_type() == at::kFloat && delta->dim() == 2 && delta->stride(1) == 1 && delta->size(0) == N && delta->size(1) == K);
-    dp = delta->data_ptr<float>(); ldd = delta->stride(0);
-  }
-  c10::cuda::CUDAGuard guard(q.device());
-  rb::mx_quantize_weight_2d(wp, ldw, q.data_ptr(), sf_fwd.data_ptr(), dp, ldd, q.data_ptr(), q.stride(0), sf_fwd.data_ptr(), sf_bwd.data_ptr(),
-                            (int)N, (int)K, cur_stream());
+  const Call c{"mx_quantize_weight_2d", q.device()};
+  void* qp = arg(c, q, "q", at::kByte, {pad128(N), pad128(K)}, 4);
+  void* fp = arg(c, sf_fwd, "sf_fwd", at::kByte, {rb::mx_sf_bytes(N, K)});
+  void* bp = arg(c, sf_bwd, "sf_bwd", at::kByte, {rb::mx_sf_bytes(K, N)});
+  const void* wp = arg(c, w, "w", BF, {N, K}, 16);
+  const float* dp = arg<const float>(c, delta, "delta", F32, {N, K});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::mx_quantize_weight_2d(wp, w.has_value() ? w->stride(0) : 0, qp, fp, dp, delta.has_value() ? delta->stride(0) : 0, qp, q.stride(0), fp,
+                            bp, (int)N, (int)K, cur_stream());
 }
 void mx_dequantize_weight(const Tensor& q, const Tensor& sf_fwd, Tensor& out) {
-  chk_bf16(out, "out"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(q.scalar_type() == at::kByte && q.dim() == 2 && q.stride(1) == 1 && sf_fwd.scalar_type() == at::kByte && sf_fwd.is_contiguous());
-  TORCH_CHECK(q.is_cuda() && sf_fwd.is_cuda() && q.device() == out.device() && sf_fwd.device() == out.device(),
-              "mx_dequantize_weight: operands must be on the device of out");
-  TORCH_CHECK(q.size(0) >= out.size(0) && q.size(1) >= out.size(1) && sf_fwd.numel() >= rb::mx_sf_bytes(out.size(0), out.size(1)),
-              "mx_dequantize_weight: q / sf_fwd are smaller than out");
-  // the kernel loads 4 bytes of q and stores 4 bf16 of out per access
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(q.data_ptr()) & 3) == 0 && q.stride(0) % 4 == 0,
-              "mx_dequantize_weight: q needs a 4-byte aligned base and a row pitch that is a multiple of 4");
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(out.data_ptr()) & 7) == 0 && out.stride(0) % 4 == 0,
-              "mx_dequantize_weight: out needs an 8-byte aligned base and a row pitch that is a multiple of 4 elements");
-  c10::cuda::CUDAGuard guard(q.device());
-  rb::mx_dequantize_weight(q.data_ptr(), q.stride(0), sf_fwd.data_ptr(), out.data_ptr(), out.stride(0), (int)out.size(0), (int)out.size(1), cur_stream());
+  const Call c{"mx_dequantize_weight", out.device()};
+  void* op = arg(c, out, "out", BF, {0, 0}, 8);
+  const int64_t N = out.size(0), K = out.size(1);
+  const void* qp = arg(c, q, "q", at::kByte, {N, K}, 4);
+  const void* fp = arg(c, sf_fwd, "sf_fwd", at::kByte, {rb::mx_sf_bytes(N, K)});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::mx_dequantize_weight(qp, q.stride(0), fp, op, out.stride(0), (int)N, (int)K, cur_stream());
 }
 void gemm_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tensor& sfb, Tensor& out, int64_t M, int64_t N, int64_t K, bool b_mn_major,
              const OptTensor& a2, const OptTensor& b2, const OptTensor& residual) {
-  TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kByte && b.scalar_type() == at::kByte && a.dim() == 2 && b.dim() == 2 && a.stride(1) == 1 && b.stride(1) == 1);
-  TORCH_CHECK(sfa.scalar_type() == at::kByte && sfb.scalar_type() == at::kByte && sfa.is_contiguous() && sfb.is_contiguous());
-  chk_bf16(out, "out"); chk_2d_rowmajor(out, "out");
-  const int64_t Kpad = (K + 127) / 128 * 128;
-  TORCH_CHECK(a.size(0) >= M && a.size(1) >= Kpad, "a must be [>= M, >= Kpad] fp8 bytes");
-  if (b_mn_major) {
-    TORCH_CHECK(b.size(0) >= Kpad && b.size(1) >= N, "MN-major b must be [>= Kpad rows, >= N]");
-  } else {
-    TORCH_CHECK(b.size(0) >= N && b.size(1) >= Kpad, "K-major b must be [>= N, >= Kpad]");
-  }
-  TORCH_CHECK(sfa.numel() >= rb::mx_sf_bytes(M, K) && sfb.numel() >= rb::mx_sf_bytes(N, K), "scale buffers too small");
-  TORCH_CHECK(out.size(0) == M && out.size(1) == N);
+  TORCH_CHECK(!a2.has_value() || b2.has_value(), "gemm_mx: a2 needs b2");
+  const Call c{"gemm_mx", out.device()};
   rb::MxGemmDesc d;
-  d.a = a.data_ptr(); d.lda = a.stride(0); d.b = b.data_ptr(); d.ldb = b.stride(0); d.sfa = sfa.data_ptr(); d.sfb = sfb.data_ptr();
-  d.b_mn_major = b_mn_major; d.M = (int)M; d.N = (int)N; d.K = (int)K; d.out = out.data_ptr(); d.ldc = out.stride(0);
+  const int64_t Kpad = pad128(K);
+  d.a = arg(c, a, "a", at::kByte, {M, Kpad}, 16); d.lda = a.stride(0);
+  d.b = b_mn_major ? arg(c, b, "b", at::kByte, {Kpad, N}, 16) : arg(c, b, "b", at::kByte, {N, Kpad}, 16); d.ldb = b.stride(0);
+  d.sfa = arg(c, sfa, "sfa", at::kByte, {rb::mx_sf_bytes(M, K)});
+  d.sfb = arg(c, sfb, "sfb", at::kByte, {rb::mx_sf_bytes(N, K)});
+  d.out = arg(c, out, "out", BF, {M, N}, 16); d.ldc = out.stride(0);
+  d.b_mn_major = b_mn_major; d.M = (int)M; d.N = (int)N; d.K = (int)K;
   if (a2.has_value()) {
-    TORCH_CHECK(b2.has_value(), "a2 needs b2");
-    chk_bf16(*a2, "a2"); chk_bf16(*b2, "b2"); chk_2d_rowmajor(*a2, "a2"); chk_2d_rowmajor(*b2, "b2");
-    TORCH_CHECK(a2->size(0) == M && b2->size(0) == N && a2->size(1) == b2->size(1));
-    d.a2 = a2->data_ptr(); d.lda2 = a2->stride(0); d.b2 = b2->data_ptr(); d.ldb2 = b2->stride(0); d.K2 = (int)a2->size(1);
+    d.a2 = arg(c, a2, "a2", BF, {M, 0}, 16); d.lda2 = a2->stride(0); d.K2 = (int)a2->size(1);
+    d.b2 = arg(c, b2, "b2", BF, {N, d.K2}, 16); d.ldb2 = b2->stride(0);
   }
-  if (residual.has_value()) {
-    chk_bf16(*residual, "residual"); chk_2d_rowmajor(*residual, "residual");
-    TORCH_CHECK(residual->size(0) == M && residual->size(1) == N);
-    d.residual = residual->data_ptr(); d.ldr = residual->stride(0);
-  }
-  c10::cuda::CUDAGuard guard(a.device());
+  d.residual = arg(c, residual, "residual", BF, {M, N}, 16); d.ldr = residual.has_value() ? residual->stride(0) : 0;
+  c10::cuda::CUDAGuard guard(c.dev);
   rb::gemm_mx(d, cur_stream());
 }
 
 // ---------------------------------------------------------------------------------------------- GPT-NeoX / Pythia block
-void chk_ln_vec(const OptTensor& t, int64_t H, const char* name) {
-  if (!t.has_value()) return;
-  chk_bf16(*t, name);
-  TORCH_CHECK(t->is_contiguous() && t->numel() == H, name, " must be contiguous [H]");
-}
-void chk_f32_vec(const OptTensor& t, int64_t n, const char* name) {
-  if (!t.has_value()) return;
-  TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == n, name, " must be fp32 contiguous [", n, "]");
-}
-void chk_rows(const OptTensor& t, const Tensor& like, const char* name) {
-  if (!t.has_value()) return;
-  chk_bf16(*t, name);
-  TORCH_CHECK(t->is_contiguous() && t->sizes() == like.sizes(), name, " must be contiguous and shaped like x");
-}
-void* ptr_or_null(const OptTensor& t) { return t.has_value() ? t->data_ptr() : nullptr; }
-float* f32_or_null(const OptTensor& t) { return t.has_value() ? t->data_ptr<float>() : nullptr; }
-
-rb::LnDrop ln_drop(const OptTensor& seed, double p) {
-  rb::LnDrop d;
-  d.seed_ptr = u32ptr(seed);
-  d.thr16 = (uint32_t)llround(p * 65536.0);
-  d.inv_keep = (float)(1.0 / (1.0 - p));
-  return d;
-}
-
 // y = LN(x; w, b).  Executor options: y2 = LN(x; w2, b2) from the same statistics, and dropout copies xd (of y, mask key `keys[0]`) /
 // xd2 (of y2, `keys[1]`) with probability p from the device seed.
 void layernorm_fwd(const Tensor& x, const Tensor& w, const OptTensor& b, Tensor& y, Tensor& mean, Tensor& rstd, double eps, const OptTensor& w2,
                    const OptTensor& b2, const OptTensor& y2, const OptTensor& xd, const OptTensor& xd2, const OptTensor& seed,
                    std::vector<int64_t> keys, double p) {
-  chk_bf16(x, "x"); chk_bf16(w, "weight"); chk_bf16(y, "y");
-  TORCH_CHECK(x.is_contiguous() && y.is_contiguous() && w.is_contiguous() && x.dim() == 2 && w.numel() == x.size(1));
-  TORCH_CHECK(mean.scalar_type() == at::kFloat && rstd.scalar_type() == at::kFloat && mean.numel() == x.size(0) && rstd.numel() == x.size(0));
-  const int64_t H = x.size(1);
-  if (b.has_value()) { chk_bf16(*b, "bias"); TORCH_CHECK(b->is_contiguous() && b->numel() == H); }
-  chk_ln_vec(w2, H, "w2"); chk_ln_vec(b2, H, "b2");
-  chk_rows(y2, x, "y2"); chk_rows(xd, x, "xd"); chk_rows(xd2, x, "xd2");
-  TORCH_CHECK(y2.has_value() == w2.has_value(), "y2 and w2 go together");
-  TORCH_CHECK(!xd2.has_value() || y2.has_value(), "xd2 needs y2");
-  const size_t nkeys = (xd.has_value() || xd2.has_value()) ? 2 : 0;
-  TORCH_CHECK(nkeys == 0 || (keys.size() == 2 && seed.has_value() && p >= 0.0 && p < 1.0), "dropout copies need the seed, two keys and p");
+  TORCH_CHECK(y2.has_value() == w2.has_value(), "layernorm_fwd: y2 and w2 go together");
+  TORCH_CHECK(!xd2.has_value() || y2.has_value(), "layernorm_fwd: xd2 needs y2");
+  const bool copies = xd.has_value() || xd2.has_value();
+  TORCH_CHECK(!copies || seed.has_value(), "layernorm_fwd: dropout copies need the seed");
+  const Call c{"layernorm_fwd", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0, 0}, 16, {x.size(-1)});
+  const int64_t M = x.size(0), H = x.size(1);
+  const Dropout dr = dropout(c, seed, keys, p, copies ? 2 : 0, 2);
   rb::LnFwdOut n1, n2;
-  n1.w = w.data_ptr(); n1.b = ptr_or_null(b); n1.y = y.data_ptr(); n1.xd = ptr_or_null(xd);
-  n2.w = ptr_or_null(w2); n2.b = ptr_or_null(b2); n2.y = ptr_or_null(y2); n2.xd = ptr_or_null(xd2);
-  if (nkeys) { n1.key = (uint32_t)keys[0]; n2.key = (uint32_t)keys[1]; }
-  c10::cuda::CUDAGuard guard(x.device());
-  const bool ok = rb::layernorm_fwd_dual(x.data_ptr(), n1, n2, mean.data_ptr<float>(), rstd.data_ptr<float>(), (int)x.size(0), (int)H, (float)eps,
-                                         nkeys ? ln_drop(seed, p) : rb::LnDrop{}, cur_stream());
+  n1.w = arg(c, w, "w", BF, {H}, 16); n1.b = arg(c, b, "b", BF, {H}, 16); n1.y = arg(c, y, "y", BF, {M * H}, 16);
+  n1.xd = arg(c, xd, "xd", BF, {M * H}, 16);
+  n2.w = arg(c, w2, "w2", BF, {H}, 16); n2.b = arg(c, b2, "b2", BF, {H}, 16); n2.y = arg(c, y2, "y2", BF, {M * H}, 16);
+  n2.xd = arg(c, xd2, "xd2", BF, {M * H}, 16);
+  n1.key = dr.keys[0]; n2.key = dr.keys[1];
+  float* mp = arg<float>(c, mean, "mean", F32, {M});
+  float* rp = arg<float>(c, rstd, "rstd", F32, {M});
+  c10::cuda::CUDAGuard guard(c.dev);
+  const bool ok = rb::layernorm_fwd_dual(xp, n1, n2, mp, rp, (int)M, (int)H, (float)eps, copies ? dr.ln() : rb::LnDrop{}, cur_stream());
   TORCH_CHECK(ok, "layernorm_fwd: hidden size must be a multiple of 8 and <= 4096");
 }
 
@@ -516,220 +452,257 @@ void layernorm_fwd(const Tensor& x, const Tensor& w, const OptTensor& b, Tensor&
 void layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& w, const Tensor& mean, const Tensor& rstd, Tensor& dx, Tensor& dw,
                    const OptTensor& db, const OptTensor& dres, const OptTensor& dy2, const OptTensor& w2, const OptTensor& dw2,
                    const OptTensor& db2, const OptTensor& dres_sum, const OptTensor& dres_sum2) {
-  chk_bf16(dy, "dy"); chk_bf16(x, "x"); chk_bf16(w, "weight"); chk_bf16(dx, "dx");
-  TORCH_CHECK(dy.is_contiguous() && x.is_contiguous() && dx.is_contiguous() && w.is_contiguous() && x.dim() == 2);
-  TORCH_CHECK(dw.scalar_type() == at::kFloat && dw.is_contiguous() && dw.numel() == x.size(1));
-  if (db.has_value()) TORCH_CHECK(db->scalar_type() == at::kFloat && db->is_contiguous() && db->numel() == x.size(1));
-  c10::cuda::CUDAGuard guard(x.device());
-  const int64_t H = x.size(1);
+  TORCH_CHECK(dy2.has_value() == w2.has_value() && dy2.has_value() == dw2.has_value(), "layernorm_bwd: dy2, w2 and dw2 go together");
+  TORCH_CHECK(!dres_sum.has_value() || dres.has_value(), "layernorm_bwd: dres_sum needs dres");
+  TORCH_CHECK(!dres_sum2.has_value() || dres_sum.has_value(), "layernorm_bwd: dres_sum2 needs dres_sum");
+  const Call c{"layernorm_bwd", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0, 0}, 16, {x.size(-1)});
+  const int64_t M = x.size(0), H = x.size(1);
+  const bool dual = dres.has_value() || dy2.has_value() || dres_sum.has_value();
+  // the module form adds dw / db with 16-byte reductions, the executor form with scalar atomics
+  const int64_t wgrad_align = dual ? 4 : 16;
+  rb::LnBwdNorm n1, n2;
+  n1.dy = arg(c, dy, "dy", BF, {M * H}, 16); n1.w = arg(c, w, "w", BF, {H}, 16);
+  n1.dw = arg<float>(c, dw, "dw", F32, {H}, wgrad_align); n1.db = arg<float>(c, db, "db", F32, {H}, wgrad_align);
+  n2.dy = arg(c, dy2, "dy2", BF, {M * H}, 16); n2.w = arg(c, w2, "w2", BF, {H}, 16);
+  n2.dw = arg<float>(c, dw2, "dw2", F32, {H}); n2.db = arg<float>(c, db2, "db2", F32, {H});
+  const float* mp = arg<const float>(c, mean, "mean", F32, {M});
+  const float* rp = arg<const float>(c, rstd, "rstd", F32, {M});
+  void* dxp = arg(c, dx, "dx", BF, {M * H}, 16);
+  const void* drp = arg(c, dres, "dres", BF, {M * H}, 16);
+  float* s1 = arg<float>(c, dres_sum, "dres_sum", F32, {H});
+  float* s2 = arg<float>(c, dres_sum2, "dres_sum2", F32, {H});
+  c10::cuda::CUDAGuard guard(c.dev);
   bool ok;
-  if (!dres.has_value() && !dy2.has_value() && !dres_sum.has_value()) {
-    ok = rb::layernorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), dx.data_ptr(),
-                           dw.data_ptr<float>(), db.has_value() ? db->data_ptr<float>() : nullptr, (int)x.size(0), (int)H, cur_stream());
+  if (!dual) {
+    ok = rb::layernorm_bwd(n1.dy, xp, n1.w, mp, rp, dxp, n1.dw, n1.db, (int)M, (int)H, cur_stream());
   } else {
-    chk_rows(dres, x, "dres"); chk_rows(dy2, x, "dy2"); chk_ln_vec(w2, H, "w2");
-    chk_f32_vec(dw2, H, "dw2"); chk_f32_vec(db2, H, "db2"); chk_f32_vec(dres_sum, H, "dres_sum"); chk_f32_vec(dres_sum2, H, "dres_sum2");
-    TORCH_CHECK(dy2.has_value() == w2.has_value() && dy2.has_value() == dw2.has_value(), "dy2, w2 and dw2 go together");
-    TORCH_CHECK(!dres_sum.has_value() || dres.has_value(), "dres_sum needs dres");
-    TORCH_CHECK(!dres_sum2.has_value() || dres_sum.has_value(), "dres_sum2 needs dres_sum");
-    rb::LnBwdNorm n1, n2;
-    n1.dy = dy.data_ptr(); n1.w = w.data_ptr(); n1.dw = dw.data_ptr<float>(); n1.db = f32_or_null(db);
-    n2.dy = ptr_or_null(dy2); n2.w = ptr_or_null(w2); n2.dw = f32_or_null(dw2); n2.db = f32_or_null(db2);
     Tensor total;  // Σ rows of dres, formed once when it goes to two outputs
-    if (dres_sum2.has_value()) total = at::empty({H}, x.options().dtype(at::kFloat));
-    ok = rb::layernorm_bwd_dual(x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), n1, n2, ptr_or_null(dres), dx.data_ptr(),
-                                f32_or_null(dres_sum), f32_or_null(dres_sum2), dres_sum2.has_value() ? total.data_ptr<float>() : nullptr,
-                                (int)x.size(0), (int)H, cur_stream());
+    if (s2 != nullptr) total = at::empty({H}, x.options().dtype(F32));
+    ok = rb::layernorm_bwd_dual(xp, mp, rp, n1, n2, drp, dxp, s1, s2, s2 != nullptr ? total.data_ptr<float>() : nullptr, (int)M, (int)H,
+                                cur_stream());
   }
   TORCH_CHECK(ok, "layernorm_bwd: hidden size must be a multiple of 8 and <= 2048");
 }
 // a = GELU(z); xd (optional): dropout copy of a with mask key `key` (rows of z.size(-1) elements)
 void gelu_fwd(const Tensor& z, Tensor& a, bool tanh_approx, const OptTensor& xd, const OptTensor& seed, int64_t key, double p) {
-  chk_bf16(z, "z"); chk_bf16(a, "a");
-  TORCH_CHECK(z.is_contiguous() && a.is_contiguous() && z.numel() == a.numel());
-  chk_rows(xd, z, "xd");
-  TORCH_CHECK(!xd.has_value() || (seed.has_value() && p >= 0.0 && p < 1.0), "the dropout copy needs the seed and p");
-  c10::cuda::CUDAGuard guard(z.device());
-  rb::gelu_fwd(z.data_ptr(), a.data_ptr(), z.numel(), tanh_approx, cur_stream(), ptr_or_null(xd), (int)z.size(-1), (uint32_t)key,
-               xd.has_value() ? ln_drop(seed, p) : rb::LnDrop{});
+  TORCH_CHECK(!xd.has_value() || seed.has_value(), "gelu_fwd: the dropout copy needs the seed");
+  const Call c{"gelu_fwd", z.device()};
+  const void* zp = arg(c, z, "z", BF, {0}, 16);
+  const int64_t n = z.numel();
+  void* ap = arg(c, a, "a", BF, {n}, 16);
+  void* xdp = arg(c, xd, "xd", BF, {n}, 16);
+  const Dropout dr = dropout(c, seed, {key}, p, 1, 1);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::gelu_fwd(zp, ap, n, tanh_approx, cur_stream(), xdp, (int)z.size(-1), dr.keys[0], xdp != nullptr ? dr.ln() : rb::LnDrop{});
 }
 // dz = da · GELU'(z); dbias (optional, fp32 [N]) += Σ rows of dz
 void gelu_bwd(const Tensor& da, const Tensor& z, Tensor& dz, bool tanh_approx, const OptTensor& dbias) {
-  chk_bf16(da, "da"); chk_bf16(z, "z"); chk_bf16(dz, "dz");
-  TORCH_CHECK(da.is_contiguous() && z.is_contiguous() && dz.is_contiguous() && z.numel() == da.numel() && z.numel() == dz.numel());
-  c10::cuda::CUDAGuard guard(z.device());
-  if (dbias.has_value()) {
-    const int64_t N = z.size(-1);
-    chk_f32_vec(dbias, N, "dbias");
-    rb::gelu_bwd_colsum(da.data_ptr(), z.data_ptr(), dz.data_ptr(), dbias->data_ptr<float>(), (int)(z.numel() / N), (int)N, tanh_approx, cur_stream());
-    return;
-  }
-  rb::gelu_bwd(da.data_ptr(), z.data_ptr(), dz.data_ptr(), z.numel(), tanh_approx, cur_stream());
+  const Call c{"gelu_bwd", z.device()};
+  const void* zp = arg(c, z, "z", BF, {0}, 16);
+  const int64_t n = z.numel(), N = z.size(-1);
+  const void* dap = arg(c, da, "da", BF, {n}, 16);
+  void* dzp = arg(c, dz, "dz", BF, {n}, 16);
+  float* bp = arg<float>(c, dbias, "dbias", F32, {N}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  if (bp != nullptr) rb::gelu_bwd_colsum(dap, zp, dzp, bp, (int)(n / N), (int)N, tanh_approx, cur_stream());
+  else rb::gelu_bwd(dap, zp, dzp, n, tanh_approx, cur_stream());
 }
 // out (fp32 [N]) += Σ rows of x [M, N]
 void colsum(const Tensor& x, Tensor& out) {
-  chk_bf16(x, "x"); chk_2d_rowmajor(x, "x");
-  TORCH_CHECK(x.is_contiguous(), "x must be contiguous");
-  chk_f32_vec(out, x.size(1), "out");
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::colsum(x.data_ptr(), out.data_ptr<float>(), (int)x.size(0), (int)x.size(1), cur_stream());
+  const Call c{"colsum", x.device()};
+  const void* xp = arg(c, x, "x", BF, {0, 0}, 16, {x.size(-1)});
+  float* op = arg<float>(c, out, "out", F32, {x.size(1)}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::colsum(xp, op, (int)x.size(0), (int)x.size(1), cur_stream());
 }
 void neox_rope(Tensor& qkv, int64_t T, int64_t nh, int64_t hd, int64_t rot, const Tensor& cos, const Tensor& sin, int64_t pos0, bool inverse) {
-  chk_bf16(qkv, "qkv"); chk_2d_rowmajor(qkv, "qkv");
-  TORCH_CHECK(qkv.size(1) == nh * 3 * hd, "qkv must be [rows, nh * 3 * hd]");
-  TORCH_CHECK(cos.scalar_type() == at::kFloat && sin.scalar_type() == at::kFloat && cos.is_contiguous() && sin.is_contiguous() &&
-              cos.dim() == 2 && cos.size(1) == rot && sin.sizes() == cos.sizes() && T + pos0 <= cos.size(0), "cos / sin must be fp32 [n_pos, rot]");
-  c10::cuda::CUDAGuard guard(qkv.device());
-  rb::neox_rope(qkv.data_ptr(), qkv.stride(0), qkv.size(0), (int)T, (int)nh, (int)hd, (int)rot, cos.data_ptr<float>(), sin.data_ptr<float>(),
-                (int)pos0, inverse, cur_stream());
+  const Call c{"neox_rope", qkv.device()};
+  void* qp = arg(c, qkv, "qkv", BF, {0, nh * 3 * hd});
+  const float* cp = arg<const float>(c, cos, "cos (rotary table [pos, rot])", F32, {T + pos0, rot}, 1, {rot});
+  const float* sp = arg<const float>(c, sin, "sin (rotary table [pos, rot])", F32, {T + pos0, rot}, 1, {rot});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::neox_rope(qp, qkv.stride(0), qkv.size(0), (int)T, (int)nh, (int)hd, (int)rot, cp, sp, (int)pos0, inverse, cur_stream());
 }
 
 void embedding_fwd(const Tensor& ids, const Tensor& table, Tensor& out) {
-  chk_bf16(table, "table"); chk_bf16(out, "out");
-  TORCH_CHECK(ids.is_cuda() && ids.scalar_type() == at::kLong && ids.is_contiguous() && table.is_contiguous() && out.is_contiguous());
-  c10::cuda::CUDAGuard guard(out.device());
-  rb::embedding_fwd(ids.data_ptr<int64_t>(), table.data_ptr(), out.data_ptr(), (int)ids.numel(), (int)table.size(1), cur_stream());
+  const Call c{"embedding_fwd", out.device()};
+  const int64_t* ip = arg<const int64_t>(c, ids, "ids", at::kLong, {0});
+  const void* tp = arg(c, table, "table", BF, {0, 0}, 16, {table.size(-1)});
+  const int64_t M = ids.numel(), H = table.size(1);
+  void* op = arg(c, out, "out", BF, {M * H}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::embedding_fwd(ip, tp, op, (int)M, (int)H, cur_stream());
 }
 void embedding_bwd(const Tensor& ids, const Tensor& dout, Tensor& dtable, int64_t padding_idx) {
-  chk_bf16(dout, "dout");
-  TORCH_CHECK(dtable.scalar_type() == at::kFloat && dtable.is_contiguous() && dout.is_contiguous() && ids.is_contiguous());
-  c10::cuda::CUDAGuard guard(dout.device());
-  rb::embedding_bwd(ids.data_ptr<int64_t>(), dout.data_ptr(), dtable.data_ptr<float>(), (int)ids.numel(), (int)dtable.size(1), padding_idx,
-                    cur_stream());
+  const Call c{"embedding_bwd", dout.device()};
+  const int64_t* ip = arg<const int64_t>(c, ids, "ids", at::kLong, {0});
+  float* tp = arg<float>(c, dtable, "dtable", F32, {0, 0}, 1, {dtable.size(-1)});
+  const int64_t M = ids.numel(), H = dtable.size(1);
+  const void* dp = arg(c, dout, "dout", BF, {M * H}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::embedding_bwd(ip, dp, tp, (int)M, (int)H, padding_idx, cur_stream());
 }
-
 void embedding_bwd_sorted(const Tensor& sorted_ids, const Tensor& perm, const Tensor& dout, Tensor& dtable, int64_t padding_idx) {
-  chk_bf16(dout, "dout");
-  TORCH_CHECK(dtable.scalar_type() == at::kFloat && dtable.is_contiguous() && dout.is_contiguous());
-  TORCH_CHECK(sorted_ids.scalar_type() == at::kLong && perm.scalar_type() == at::kLong && sorted_ids.is_contiguous() && perm.is_contiguous() &&
-              sorted_ids.numel() == perm.numel());
-  c10::cuda::CUDAGuard guard(dout.device());
-  rb::embedding_bwd_sorted(sorted_ids.data_ptr<int64_t>(), perm.data_ptr<int64_t>(), dout.data_ptr(), dtable.data_ptr<float>(),
-                           (int)sorted_ids.numel(), (int)dtable.size(1), padding_idx, cur_stream());
+  const Call c{"embedding_bwd_sorted", dout.device()};
+  const int64_t* ip = arg<const int64_t>(c, sorted_ids, "sorted_ids", at::kLong, {0});
+  const int64_t M = sorted_ids.numel();
+  const int64_t* pp = arg<const int64_t>(c, perm, "perm", at::kLong, {M});
+  float* tp = arg<float>(c, dtable, "dtable", F32, {0, 0}, 16, {dtable.size(-1)});  // 16-byte read-modify-writes
+  const int64_t H = dtable.size(1);
+  const void* dp = arg(c, dout, "dout", BF, {M * H}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::embedding_bwd_sorted(ip, pp, dp, tp, (int)M, (int)H, padding_idx, cur_stream());
 }
 
 void cross_entropy_fwd_bwd(Tensor& logits, const Tensor& labels, int64_t V, double grad_scale, int64_t ignore_index, Tensor& loss_sum,
                            Tensor& count) {
-  chk_bf16(logits, "logits"); chk_2d_rowmajor(logits, "logits");
-  TORCH_CHECK(labels.is_cuda() && labels.scalar_type() == at::kLong && labels.is_contiguous() && labels.numel() == logits.size(0));
-  TORCH_CHECK(loss_sum.scalar_type() == at::kFloat && count.scalar_type() == at::kFloat);
-  c10::cuda::CUDAGuard guard(logits.device());
-  rb::cross_entropy_fwd_bwd(logits.data_ptr(), logits.stride(0), labels.data_ptr<int64_t>(), (int)logits.size(0), (int)V, (float)grad_scale,
-                            ignore_index, loss_sum.data_ptr<float>(), count.data_ptr<float>(), cur_stream());
+  const Call c{"cross_entropy_fwd_bwd", logits.device()};
+  void* lp = arg(c, logits, "logits", BF, {0, V}, 16);
+  const int64_t M = logits.size(0);
+  const int64_t* yp = arg<const int64_t>(c, labels, "labels", at::kLong, {M});
+  float* sp = arg<float>(c, loss_sum, "loss_sum", F32, {1});
+  float* np = arg<float>(c, count, "count", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::cross_entropy_fwd_bwd(lp, logits.stride(0), yp, (int)M, (int)V, (float)grad_scale, ignore_index, sp, np, cur_stream());
 }
 
 void transpose(const Tensor& in, Tensor& out) {
-  chk_bf16(in, "in"); chk_bf16(out, "out"); chk_2d_rowmajor(in, "in"); chk_2d_rowmajor(out, "out");
-  TORCH_CHECK(out.size(0) == in.size(1) && out.size(1) == in.size(0));
-  c10::cuda::CUDAGuard guard(in.device());
-  rb::transpose_bf16(in.data_ptr(), in.stride(0), out.data_ptr(), out.stride(0), (int)in.size(0), (int)in.size(1), cur_stream());
+  const Call c{"transpose", in.device()};
+  const void* ip = arg(c, in, "in", BF, {0, 0});
+  const int64_t R = in.size(0), C = in.size(1);
+  void* op = arg(c, out, "out", BF, {C, R});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::transpose_bf16(ip, in.stride(0), op, out.stride(0), (int)R, (int)C, cur_stream());
 }
 void add(const Tensor& a, const Tensor& b, Tensor& out) {
-  chk_bf16(a, "a"); chk_bf16(b, "b"); chk_bf16(out, "out");
-  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && out.is_contiguous() && a.numel() == b.numel() && a.numel() == out.numel());
-  c10::cuda::CUDAGuard guard(a.device());
-  rb::add_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), cur_stream());
+  const Call c{"add", a.device()};
+  const void* ap = arg(c, a, "a", BF, {0}, 16);
+  const int64_t n = a.numel();
+  const void* bp = arg(c, b, "b", BF, {n}, 16);
+  void* op = arg(c, out, "out", BF, {n}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::add_bf16(ap, bp, op, n, cur_stream());
 }
 void cast_f32_to_bf16(const Tensor& in, Tensor& out, double scale) {
-  TORCH_CHECK(in.scalar_type() == at::kFloat && in.is_contiguous() && out.is_contiguous() && in.numel() == out.numel());
-  chk_bf16(out, "out");
-  c10::cuda::CUDAGuard guard(in.device());
-  rb::cast_f32_to_bf16(in.data_ptr<float>(), out.data_ptr(), in.numel(), (float)scale, cur_stream());
+  const Call c{"cast_f32_to_bf16", in.device()};
+  const float* ip = arg<const float>(c, in, "in", F32, {0}, 16);
+  void* op = arg(c, out, "out", BF, {in.numel()}, 16);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::cast_f32_to_bf16(ip, op, in.numel(), (float)scale, cur_stream());
 }
 void fill_uniform_hash(Tensor& out, int64_t seed, double bound) {
-  chk_bf16(out, "out"); chk_2d_rowmajor(out, "out");
-  c10::cuda::CUDAGuard guard(out.device());
-  rb::fill_uniform_hash(out.data_ptr(), (int)out.size(0), (int)out.size(1), out.stride(0), (uint32_t)seed, (float)bound, cur_stream());
+  const Call c{"fill_uniform_hash", out.device()};
+  void* op = arg(c, out, "out", BF, {0, 0});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::fill_uniform_hash(op, (int)out.size(0), (int)out.size(1), out.stride(0), (uint32_t)seed, (float)bound, cur_stream());
 }
 void seed_advance(Tensor& seed) {
-  TORCH_CHECK(seed.is_cuda() && seed.scalar_type() == at::kInt && seed.numel() == 1);
-  c10::cuda::CUDAGuard guard(seed.device());
-  rb::seed_advance(reinterpret_cast<uint32_t*>(seed.data_ptr<int32_t>()), cur_stream());
+  const Call c{"seed_advance", seed.device()};
+  uint32_t* sp = arg<uint32_t>(c, seed, "seed", at::kInt, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::seed_advance(sp, cur_stream());
 }
+
+// bf16 or fp32 flat buffers: the dtype is the tensor's own, and must be one of the two
+at::ScalarType bf16_or_f32(const Tensor& t) { return t.scalar_type() == F32 ? F32 : BF; }
 
 void adamw_flat(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, double lr, double b1, double b2, double eps, double wd, int64_t step,
                 const OptTensor& grad_scale, double grad_scale_host, const OptTensor& skip, const OptTensor& step_dev) {
-  chk_bf16(p, "param");
-  TORCH_CHECK(p.is_contiguous() && g.is_contiguous() && m.is_contiguous() && v.is_contiguous());
-  TORCH_CHECK(g.numel() == p.numel() && m.numel() == p.numel() && v.numel() == p.numel());
-  const bool gf = g.scalar_type() == at::kFloat, sf = m.scalar_type() == at::kFloat;
-  TORCH_CHECK(gf || g.scalar_type() == at::kBFloat16, "grad must be bf16 or fp32");
-  TORCH_CHECK((sf || m.scalar_type() == at::kBFloat16) && m.scalar_type() == v.scalar_type(), "moments must be bf16 or fp32");
-  c10::cuda::CUDAGuard guard(p.device());
-  rb::adamw_flat(p.data_ptr(), g.data_ptr(), gf, m.data_ptr(), v.data_ptr(), sf, p.numel(), (float)lr, (float)b1, (float)b2, (float)eps,
-                 (float)wd, (int)step, f32ptr(grad_scale), (float)grad_scale_host, f32ptr(skip), f32ptr(step_dev), cur_stream());
+  const Call c{"adamw_flat", p.device()};
+  void* pp = arg(c, p, "param", BF, {0}, 16);
+  const int64_t n = p.numel();
+  const auto gt = bf16_or_f32(g), st = bf16_or_f32(m);
+  const void* gp = arg(c, g, "grad", gt, {n});
+  void* mp = arg(c, m, "exp_avg", st, {n});
+  void* vp = arg(c, v, "exp_avg_sq", st, {n});
+  const float* gsp = arg<const float>(c, grad_scale, "grad_scale", F32, {1});
+  const float* skp = arg<const float>(c, skip, "skip", F32, {1});
+  const float* sdp = arg<const float>(c, step_dev, "step_dev", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::adamw_flat(pp, gp, gt == F32, mp, vp, st == F32, n, (float)lr, (float)b1, (float)b2, (float)eps, (float)wd, (int)step, gsp,
+                 (float)grad_scale_host, skp, sdp, cur_stream());
 }
 void sumsq(const Tensor& x, Tensor& out) {
-  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && out.scalar_type() == at::kFloat);
-  const bool f = x.scalar_type() == at::kFloat;
-  TORCH_CHECK(f || x.scalar_type() == at::kBFloat16);
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::sumsq(x.data_ptr(), f, x.numel(), out.data_ptr<float>(), cur_stream());
+  const Call c{"sumsq", x.device()};
+  const auto xt = bf16_or_f32(x);
+  const void* xp = arg(c, x, "x", xt, {0});
+  float* op = arg<float>(c, out, "out", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::sumsq(xp, xt == F32, x.numel(), op, cur_stream());
 }
 void random_prune(Tensor& x, double ratio, int64_t seed, int64_t col_offset) {
-  TORCH_CHECK(x.is_cuda() && x.is_contiguous());
-  const bool f = x.scalar_type() == at::kFloat;
-  TORCH_CHECK(f || x.scalar_type() == at::kBFloat16);
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::random_prune(x.data_ptr(), f, x.numel(), (float)ratio, (uint32_t)seed, col_offset, cur_stream());
+  const Call c{"random_prune", x.device()};
+  const auto xt = bf16_or_f32(x);
+  void* xp = arg(c, x, "x", xt, {0});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::random_prune(xp, xt == F32, x.numel(), (float)ratio, (uint32_t)seed, col_offset, cur_stream());
 }
 void magnitude_prune(Tensor& x, double ratio, Tensor& workspace, Tensor& thr) {
-  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && thr.scalar_type() == at::kFloat);
-  TORCH_CHECK((size_t)workspace.numel() * workspace.element_size() >= rb::magnitude_quantile_workspace_bytes(), "workspace too small");
-  const bool f = x.scalar_type() == at::kFloat;
-  TORCH_CHECK(f || x.scalar_type() == at::kBFloat16);
-  c10::cuda::CUDAGuard guard(x.device());
-  rb::magnitude_quantile(x.data_ptr(), f, x.numel(), (float)ratio, thr.data_ptr<float>(), workspace.data_ptr(), cur_stream());
-  rb::threshold_prune(x.data_ptr(), f, x.numel(), thr.data_ptr<float>(), cur_stream());
+  const Call c{"magnitude_prune", x.device()};
+  const auto xt = bf16_or_f32(x);
+  void* xp = arg(c, x, "x", xt, {0});
+  void* wp = arg(c, workspace, "workspace", at::kByte, {(int64_t)rb::magnitude_quantile_workspace_bytes()});
+  float* tp = arg<float>(c, thr, "thr", F32, {1});
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::magnitude_quantile(xp, xt == F32, x.numel(), (float)ratio, tp, wp, cur_stream());
+  rb::threshold_prune(xp, xt == F32, x.numel(), tp, cur_stream());
 }
 
 // ---------------------------------------------------------------------------------------------- NVLink collectives
+// The peer and multicast addresses are raw integers from the symmetric-memory allocator and cannot be checked here; the
+// tensor arguments are.
 rb::PeerPtrs peer_ptrs(const std::vector<int64_t>& v) {
   TORCH_CHECK((int)v.size() <= rb::kMaxPeers, "at most 8 peers");
   rb::PeerPtrs p;
   for (int i = 0; i < rb::kMaxPeers; ++i) p.ptr[i] = i < (int)v.size() ? reinterpret_cast<void*>(v[i]) : nullptr;
   return p;
 }
-rb::CommCtx comm_ctx(const std::vector<int64_t>& flag_ptrs, int64_t rank, int64_t world, Tensor& local_go) {
-  TORCH_CHECK(local_go.is_cuda() && local_go.scalar_type() == at::kInt && local_go.numel() >= 2, "local_go must be int32[2] on the device");
-  rb::CommCtx c;
-  c.rank = (int)rank; c.world = (int)world; c.flags = peer_ptrs(flag_ptrs);
-  c.local_go = reinterpret_cast<uint32_t*>(local_go.data_ptr<int32_t>());
-  return c;
+rb::CommCtx comm_ctx(const Call& c, const std::vector<int64_t>& flag_ptrs, int64_t rank, int64_t world, Tensor& local_go) {
+  rb::CommCtx x;
+  x.rank = (int)rank; x.world = (int)world; x.flags = peer_ptrs(flag_ptrs);
+  x.local_go = arg<uint32_t>(c, local_go, "local_go", at::kInt, {2});
+  return x;
 }
 void comm_barrier(std::vector<int64_t> flag_ptrs, int64_t rank, int64_t world, Tensor& local_go, int64_t set, int64_t epoch) {
-  c10::cuda::CUDAGuard guard(local_go.device());
-  rb::xgpu_barrier(comm_ctx(flag_ptrs, rank, world, local_go), (int)set, (uint32_t)epoch, cur_stream());
+  const Call c{"comm_barrier", local_go.device()};
+  const rb::CommCtx x = comm_ctx(c, flag_ptrs, rank, world, local_go);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::xgpu_barrier(x, (int)set, (uint32_t)epoch, cur_stream());
 }
 void comm_allreduce_bf16(std::vector<int64_t> flag_ptrs, int64_t rank, int64_t world, Tensor& local_go, std::vector<int64_t> buf_ptrs,
                          int64_t mc_ptr, int64_t off_elems, int64_t n, int64_t epoch, int64_t max_blocks) {
-  c10::cuda::CUDAGuard guard(local_go.device());
-  rb::allreduce_bf16(comm_ctx(flag_ptrs, rank, world, local_go), peer_ptrs(buf_ptrs), reinterpret_cast<void*>(mc_ptr), off_elems, n,
-                     (uint32_t)epoch, (int)max_blocks, cur_stream());
+  const Call c{"comm_allreduce_bf16", local_go.device()};
+  const rb::CommCtx x = comm_ctx(c, flag_ptrs, rank, world, local_go);
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::allreduce_bf16(x, peer_ptrs(buf_ptrs), reinterpret_cast<void*>(mc_ptr), off_elems, n, (uint32_t)epoch, (int)max_blocks, cur_stream());
 }
 void comm_fused_update(std::vector<int64_t> flag_ptrs, int64_t rank, int64_t world, Tensor& local_go, const OptTensor& grads_f32,
                        std::vector<int64_t> grad_ptrs, int64_t grad_mc, Tensor& gred, std::vector<int64_t> param_ptrs, int64_t param_mc,
                        Tensor& exp_avg, Tensor& exp_avg_sq, int64_t n, double lr, double b1, double b2, double eps, double wd, int64_t step,
                        double max_norm, const OptTensor& skip, Tensor& norm_out, Tensor& scratch, int64_t epoch, int64_t max_blocks,
                        const OptTensor& step_dev, const OptTensor& loss_in, const OptTensor& loss_out) {
-  if (grads_f32.has_value())
-    TORCH_CHECK(grads_f32->scalar_type() == at::kFloat && grads_f32->is_contiguous() && grads_f32->numel() >= n, "grads must be fp32 [n]");
-  TORCH_CHECK(gred.scalar_type() == at::kFloat && gred.numel() * world >= n, "gred must be fp32 [n / world]");
-  chk_bf16(exp_avg, "exp_avg"); chk_bf16(exp_avg_sq, "exp_avg_sq");
-  TORCH_CHECK(exp_avg.numel() * world >= n && exp_avg_sq.numel() * world >= n, "moments must be [n / world]");
-  TORCH_CHECK(norm_out.scalar_type() == at::kFloat && scratch.scalar_type() == at::kFloat && scratch.numel() >= 3);
-  c10::cuda::CUDAGuard guard(local_go.device());
+  TORCH_CHECK(world >= 1, "comm_fused_update: world must be positive");
+  const Call c{"comm_fused_update", local_go.device()};
+  const rb::CommCtx x = comm_ctx(c, flag_ptrs, rank, world, local_go);
+  const int64_t shard = (n + world - 1) / world;  // this rank's slice of the reduced gradient and of the moments
   rb::FusedUpdateArgs a;
-  a.grads_f32 = grads_f32.has_value() ? grads_f32->data_ptr<float>() : nullptr;
+  a.grads_f32 = arg<float>(c, grads_f32, "grads_f32", F32, {n});
   a.grad_bufs = peer_ptrs(grad_ptrs); a.grad_mc = reinterpret_cast<void*>(grad_mc);
-  a.gred = gred.data_ptr<float>();
+  a.gred = arg<float>(c, gred, "gred", F32, {shard});
   a.param_bufs = peer_ptrs(param_ptrs); a.param_mc = reinterpret_cast<void*>(param_mc);
-  a.exp_avg = exp_avg.data_ptr(); a.exp_avg_sq = exp_avg_sq.data_ptr();
+  a.exp_avg = arg(c, exp_avg, "exp_avg", BF, {shard});
+  a.exp_avg_sq = arg(c, exp_avg_sq, "exp_avg_sq", BF, {shard});
   a.n = n; a.lr = (float)lr; a.beta1 = (float)b1; a.beta2 = (float)b2; a.eps = (float)eps; a.weight_decay = (float)wd;
-  a.step = (int)step; a.step_dev = f32ptr(step_dev); a.max_norm = (float)max_norm; a.inv_world = 1.0f / (float)world;
-  a.loss_in = f32ptr(loss_in); a.loss_out = const_cast<float*>(f32ptr(loss_out));
-  a.skip = f32ptr(skip); a.norm_out = norm_out.data_ptr<float>(); a.sq_accum = scratch.data_ptr<float>(); a.max_blocks = (int)max_blocks;
-  rb::fused_update(comm_ctx(flag_ptrs, rank, world, local_go), a, (uint32_t)epoch, cur_stream());
+  a.step = (int)step; a.step_dev = arg<const float>(c, step_dev, "step_dev", F32, {1}); a.max_norm = (float)max_norm;
+  a.inv_world = 1.0f / (float)world;
+  a.loss_in = arg<const float>(c, loss_in, "loss_in", F32, {1}); a.loss_out = arg<float>(c, loss_out, "loss_out", F32, {1});
+  a.skip = arg<const float>(c, skip, "skip", F32, {1});
+  a.norm_out = arg<float>(c, norm_out, "norm_out", F32, {1});
+  a.sq_accum = arg<float>(c, scratch, "scratch", F32, {3});
+  a.max_blocks = (int)max_blocks;
+  c10::cuda::CUDAGuard guard(c.dev);
+  rb::fused_update(x, a, (uint32_t)epoch, cur_stream());
 }
 
 long long launch_count() { return rb::g_launch_count; }

@@ -62,7 +62,6 @@ __global__ void __launch_bounds__(256) rmsnorm_fwd_kernel(const bf16* __restrict
 void rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int M, int H, float eps, void* xd, int G,
                  const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s) {
   if (H % 8 != 0 || H > 8 * 256 * 4) throw std::runtime_error("rmsnorm: H must be a multiple of 8 and <= 8192");
-  if (G > 4) throw std::runtime_error("rmsnorm: at most 4 dropout groups");
   uint4 k = make_uint4(0, 0, 0, 0);
   if (G > 0) k = make_uint4(keys[0], G > 1 ? keys[1] : 0, G > 2 ? keys[2] : 0, G > 3 ? keys[3] : 0);
   if (rmsnorm_fwd_warp(x, w, y, rstd, M, H, eps, xd, G, seed_ptr, k, thr16, inv_keep, f8, s)) return;
@@ -200,7 +199,7 @@ __global__ void __launch_bounds__(256) dropout_expand_kernel(const bf16* __restr
 
 void dropout_expand(const void* x, void* xd, int M, int H, int G, const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16,
                     float inv_keep, Fp8Out f8, cudaStream_t s) {
-  if (H % 8 != 0 || G < 1 || G > 4) throw std::runtime_error("dropout_expand: bad shape");
+  if (H % 8 != 0) throw std::runtime_error("dropout_expand: H must be a multiple of 8");
   uint4 k = make_uint4(keys[0], G > 1 ? keys[1] : 0, G > 2 ? keys[2] : 0, G > 3 ? keys[3] : 0);
   const long long n_vec = (long long)M * H / 8;
   const int grid = (int)std::min<long long>((n_vec + 255) / 256, (long long)num_sms() * 8);
@@ -238,7 +237,7 @@ __global__ void __launch_bounds__(256) dropout_combine_kernel(const bf16* __rest
 
 void dropout_combine(const void* base, const void* parts, long long part_stride, long long ld_parts, void* out, int M, int H, int G,
                      const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16, float inv_keep, cudaStream_t s) {
-  if (H % 8 != 0 || G < 1 || G > 4) throw std::runtime_error("dropout_combine: bad shape");
+  if (H % 8 != 0) throw std::runtime_error("dropout_combine: H must be a multiple of 8");
   uint4 k = make_uint4(keys[0], G > 1 ? keys[1] : 0, G > 2 ? keys[2] : 0, G > 3 ? keys[3] : 0);
   const long long n_vec = (long long)M * H / 8;
   const int grid = (int)std::min<long long>((n_vec + 255) / 256, (long long)num_sms() * 8);
@@ -276,7 +275,7 @@ void rope_inplace(void* buf, long long ld, int M, int T, int n_rot_heads, int hd
                   bool backward, int pos0, cudaStream_t s) {
   if (rope_inplace_vec(buf, ld, M, T, n_rot_heads, hd, rotary_dim, cos, sin, backward, pos0, s)) return;
   const int half = rotary_dim / 2;
-  if (rotary_dim % 4 != 0 || hd % 2 != 0 || ld % 2 != 0) throw std::runtime_error("rope: rotary_dim must be a multiple of 4");
+  if (rotary_dim % 4 != 0 || hd % 2 != 0) throw std::runtime_error("rope: rotary_dim must be a multiple of 4");
   const long long total = (long long)M * n_rot_heads * (half / 2);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 16);
   rope_kernel<<<grid, 256, 0, s>>>((bf16*)buf, ld, total, T, n_rot_heads, hd, half, (const bf16*)cos, (const bf16*)sin,
@@ -363,7 +362,7 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const bf16* __restrict_
 }
 void swiglu_fwd(const void* gu, long long ldgu, void* h, long long ldh, int M, int F, void* hd, long long ldhd,
                 const uint32_t* seed_ptr, uint32_t key, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s) {
-  if (F % 8 || ldgu % 8 || ldh % 8 || (hd != nullptr && ldhd % 8)) throw std::runtime_error("swiglu: F and leading dims must be multiples of 8");
+  if (F % 8) throw std::runtime_error("swiglu: F must be a multiple of 8");
   const long long total = (long long)M * (F / 8);
   const int grid = (int)std::min<long long>((total + 511) / 512, (long long)num_sms() * 8);
   launch_k(swiglu_fwd_kernel, grid > 0 ? grid : 1, 256, 0, s, (const bf16*)gu, ldgu, (bf16*)h, ldh, M, F, (bf16*)hd, ldhd, seed_ptr, key, thr16, inv_keep, f8);
@@ -371,7 +370,7 @@ void swiglu_fwd(const void* gu, long long ldgu, void* h, long long ldh, int M, i
 }
 void swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, void* dgu, long long lddgu, int M, int F,
                 cudaStream_t s) {
-  if (F % 8 || ldgu % 8 || lddh % 8 || lddgu % 8) throw std::runtime_error("swiglu_bwd: dims must be multiples of 8");
+  if (F % 8) throw std::runtime_error("swiglu_bwd: F must be a multiple of 8");
   const long long total = (long long)M * (F / 8);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 8);
   launch_k(swiglu_bwd_kernel, grid, 256, 0, s, (const bf16*)dh, lddh, (const bf16*)gu, ldgu, (bf16*)dgu, lddgu, M, F);

@@ -125,7 +125,7 @@ int grid_for(long long total) { return (int)std::max<long long>(1, std::min<long
 
 void fp8_quantize_weight(const void* w, long long ld, void* w8, long long ld8, void* w8t, long long ld8t, int R, int C,
                          float* amax_scratch, float* scale, float* inv_scale, cudaStream_t s) {
-  if (C % 16 != 0 || ld % 8 != 0 || ld8 % 16 != 0) throw std::runtime_error("fp8_quantize_weight: columns must be a multiple of 16");
+  if (C % 16 != 0) throw std::runtime_error("fp8_quantize_weight: columns must be a multiple of 16");
   check(cudaMemsetAsync(amax_scratch, 0, sizeof(float), s), "cudaMemsetAsync(amax)");
   amax_kernel<<<grid_for((long long)R * C / 8), 256, 0, s>>>((const bf16*)w, ld, R, C, amax_scratch);
   RB_CHECK_LAUNCH("fp8_amax");
@@ -142,7 +142,7 @@ void fp8_quantize_weight(const void* w, long long ld, void* w8, long long ld8, v
 
 void fp8_quantize_act(const void* x, long long ld, void* x8, long long ld8, int R, int C, const float* inv_scale, float* amax_cur,
                       bool e5m2, cudaStream_t s) {
-  if (C % 16 != 0 || ld % 8 != 0 || ld8 % 16 != 0) throw std::runtime_error("fp8_quantize_act: columns must be a multiple of 16");
+  if (C % 16 != 0) throw std::runtime_error("fp8_quantize_act: columns must be a multiple of 16");
   if (e5m2) launch_k(quantize_kernel<true>, grid_for((long long)R * C / 16), 256, 0, s, (const bf16*)x, ld, (uint8_t*)x8, ld8, R, C, inv_scale, amax_cur);
   else launch_k(quantize_kernel<false>, grid_for((long long)R * C / 16), 256, 0, s, (const bf16*)x, ld, (uint8_t*)x8, ld8, R, C, inv_scale, amax_cur);
   RB_CHECK_LAUNCH("fp8_quantize_act");

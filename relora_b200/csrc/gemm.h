@@ -59,6 +59,15 @@ struct GemmDesc {
 };
 
 void gemm_bf16(const GemmDesc& d, cudaStream_t stream);
+// The stored [rows, cols] (cols contiguous) of each operand that gemm_bf16's tensor maps span: [mn, k] K-major, [k, mn]
+// MN-major, with the per-group K windows and M-group offsets included; fp8 extents are in bytes.  A2 / B2 are empty when K2 = 0.
+struct GemmExtent {
+  long long rows = 0, cols = 0;
+};
+struct GemmExtents {
+  GemmExtent a1, b1, a2, b2;
+};
+GemmExtents gemm_operand_extents(const GemmDesc& d);
 // Schedule choices of gemm_bf16 (host side): the tile width, whether the epilogue stores through shared memory with TMA,
 // and the dynamic shared memory of a tile width.
 int gemm_block_n(const GemmDesc& d);

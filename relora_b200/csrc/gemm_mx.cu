@@ -420,7 +420,6 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   if (d.M <= 0 || d.N <= 0) return;
   const int K8 = (d.K + 127) / 128 * 128;
   if (d.K2 % KB16) throw std::runtime_error("gemm_mx: the bf16 segment must be a multiple of 64");
-  if (d.ldc % 8 || (reinterpret_cast<uintptr_t>(d.out) & 15)) throw std::runtime_error("gemm_mx: output must be 16-byte aligned");
   if (d.N % 8) throw std::runtime_error("gemm_mx: N must be a multiple of 8");
   MxArgs p;
   p.M = d.M; p.N = d.N; p.K8 = K8; p.K2 = d.K2;
@@ -436,9 +435,6 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   if (d.K2 > 0) {
     ma2 = make_map_2d_sw128(d.a2, d.K2, d.M, d.lda2, KB16, BM, 2);
     mb2 = make_map_2d_sw128(d.b2, d.K2, d.N, d.ldb2, KB16, BN, 2);
-  }
-  if (d.residual != nullptr) {
-    if (d.ldr % 8 || (reinterpret_cast<uintptr_t>(d.residual) & 15)) throw std::runtime_error("gemm_mx: residual must be 16-byte aligned");
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();

@@ -751,11 +751,29 @@ CUtensorMap make_map_2d_sw128(const void* ptr, long long inner, long long outer,
 }
 
 
-// Operand covering `mn` rows/cols of the output dimension and `k` of the reduction dimension.
-static CUtensorMap operand_map(const Operand& o, long long mn, long long k, int block_mn, bool fp8 = false) {
-  if (fp8) return make_map_2d(o.ptr, k, mn, o.ld, 2 * BLOCK_K, block_mn, 1);  // E4M3 bytes, K-major only
-  if (!o.mn_major) return make_map_2d(o.ptr, k, mn, o.ld, BLOCK_K, block_mn);
-  return make_map_2d(o.ptr, mn, k, o.ld, 64, BLOCK_K);
+// Map of an operand over its stored extent e (gemm_operand_extents); boxes of block_mn rows/cols of the output dimension.
+static CUtensorMap operand_map(const Operand& o, const GemmExtent& e, int block_mn, bool fp8 = false) {
+  if (fp8) return make_map_2d(o.ptr, e.cols, e.rows, o.ld, 2 * BLOCK_K, block_mn, 1);  // E4M3 bytes, K-major only
+  if (!o.mn_major) return make_map_2d(o.ptr, e.cols, e.rows, o.ld, BLOCK_K, block_mn);
+  return make_map_2d(o.ptr, e.cols, e.rows, o.ld, 64, BLOCK_K);
+}
+
+static int gemm_n_per_group(const GemmDesc& d) { return d.n_per_group > 0 ? d.n_per_group : (d.N > 0 ? d.N : 1); }
+
+GemmExtents gemm_operand_extents(const GemmDesc& d) {
+  // K extents include the per-group windows, B1's MN extent the per-M-group offsets
+  const int groups = ceil_div(d.N, gemm_n_per_group(d));
+  const int mgroups = d.m_per_group > 0 ? ceil_div(d.M, d.m_per_group) : 1;
+  const auto stored = [](const Operand& o, long long mn, long long k) { return o.mn_major ? GemmExtent{k, mn} : GemmExtent{mn, k}; };
+  GemmExtents e;
+  e.a1 = stored(d.a1, d.M, (long long)d.K1 + (long long)(groups - 1) * d.a1_group_kofs);
+  e.b1 = stored(d.b1, (d.b1_local_n ? (long long)gemm_n_per_group(d) : (long long)d.N) + (long long)(mgroups - 1) * d.b1_mn_ofs_per_mgroup,
+                (long long)d.K1 + (long long)(groups - 1) * d.b1_group_kofs);
+  if (d.K2 > 0) {
+    e.a2 = stored(d.a2, d.M, (long long)d.K2 + (long long)(groups - 1) * d.a2_group_kofs);
+    e.b2 = stored(d.b2, d.N, d.K2);
+  }
+  return e;
 }
 
 // The TMA store needs a 16-byte aligned base and row pitch, and a row length of whole 16-byte chunks: past a ragged last
@@ -771,7 +789,7 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   using L = SmemLayout<BLOCK_N>;
   KernelArgs p;
   p.M = d.M; p.N = d.N; p.K1 = d.K1; p.K2 = d.K2;
-  p.n_per_group = d.n_per_group > 0 ? d.n_per_group : (d.N > 0 ? d.N : 1);
+  p.n_per_group = gemm_n_per_group(d);
   p.a1_group_kofs = d.a1_group_kofs; p.a2_group_kofs = d.a2_group_kofs;
   p.b1_group_kofs = d.b1_group_kofs; p.b1_local_n = d.b1_local_n ? 1 : 0;
   p.m_per_group = d.m_per_group > 0 ? d.m_per_group : (1 << 30); p.b1_mn_ofs_per_mgroup = d.b1_mn_ofs_per_mgroup;
@@ -792,24 +810,19 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   if (groups > 1 && d.a1_group_kofs != 0 && d.b1_group_kofs != 0 && d.K1 % (d.fp8 ? 2 * BLOCK_K : BLOCK_K) != 0)
     throw std::runtime_error("gemm: with per-group K windows on both A1 and B1, K1 must be a multiple of the k-block (64, fp8: 128)");
 
-  // K extents of the global tensors include the per-group windows
-  const long long a1_k_total = (long long)d.K1 + (long long)(groups - 1) * d.a1_group_kofs;
+  const GemmExtents e = gemm_operand_extents(d);
   if (d.fp8 && (A_MN || B_MN)) throw std::runtime_error("gemm: fp8 operands must be K-major");
-  CUtensorMap ma1 = operand_map(d.a1, d.M, a1_k_total, BLOCK_M, d.fp8);
-  const int mgroups = d.m_per_group > 0 ? ceil_div(d.M, d.m_per_group) : 1;
-  const long long b1_mn_total = (d.b1_local_n ? (long long)p.n_per_group : (long long)d.N) + (long long)(mgroups - 1) * d.b1_mn_ofs_per_mgroup;
-  const long long b1_k_total = (long long)d.K1 + (long long)(groups - 1) * d.b1_group_kofs;
+  CUtensorMap ma1 = operand_map(d.a1, e.a1, BLOCK_M, d.fp8);
   if (d.m_per_group > 0 && (d.m_per_group % BLOCK_M) != 0) throw std::runtime_error("gemm: m_per_group must be a multiple of the M tile");
   const bool paired = gemm_pairs(d, BLOCK_N);
   p.paired = paired ? 1 : 0;
   const int b_box = paired ? BLOCK_N / 2 : BLOCK_N;  // each CTA of a pair loads half of the B tile
-  CUtensorMap mb1 = operand_map(d.b1, b1_mn_total, b1_k_total, b_box, d.fp8);
+  CUtensorMap mb1 = operand_map(d.b1, e.b1, b_box, d.fp8);
   CUtensorMap ma2 = ma1, mb2 = mb1;
   if (d.K2 > 0) {
     if (d.a2.mn_major || d.b2.mn_major) throw std::runtime_error("gemm: the LoRA (A2/B2) operands must be K-major");
-    const long long a2_k_total = (long long)d.K2 + (long long)(groups - 1) * d.a2_group_kofs;
-    ma2 = operand_map(d.a2, d.M, a2_k_total, BLOCK_M);
-    mb2 = operand_map(d.b2, d.N, d.K2, b_box);
+    ma2 = operand_map(d.a2, e.a2, BLOCK_M);
+    mb2 = operand_map(d.b2, e.b2, b_box);
   }
   auto kern = gemm_kernel<BLOCK_N, A_MN, B_MN>;
   static int max_pairs = 0;  // clusters of 2 resident at once
@@ -893,11 +906,8 @@ bool lora_dx_uses_tma_store(const LoraDxDesc& d) { return d.N % 8 == 0; }
 
 void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
   if (d.M <= 0 || d.N <= 0) return;
-  if (d.groups < 1 || d.groups > 3) throw std::runtime_error("lora_dx: 1..3 stacked LoRA groups");
   if (d.r <= 0 || d.r % BLOCK_K != 0) throw std::runtime_error("lora_dx: the LoRA rank must be a multiple of 64");
-  if (d.Kb == 0 && (d.base == nullptr || d.ld_base % 8 != 0 || (reinterpret_cast<uintptr_t>(d.base) & 15) != 0))
-    throw std::runtime_error("lora_dx: Kb == 0 needs a 16-byte aligned base product");
-  if (d.ldc % 8 != 0 || (reinterpret_cast<uintptr_t>(d.out) & 15) != 0) throw std::runtime_error("lora_dx: output must be 16-byte aligned");
+  if (d.Kb == 0 && d.base == nullptr) throw std::runtime_error("lora_dx: Kb == 0 needs the base product");
   if (d.N % 2 != 0) throw std::runtime_error("lora_dx: N must be even");
   using L = SmemLayout<128>;
   LoraDxArgs p;

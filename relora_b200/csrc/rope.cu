@@ -106,8 +106,7 @@ void rope_pack_bwd(const void* dq, const void* dk, const void* dv, long long sB,
                    long long kT, void* out, long long ldo, int B, int T, int nh, int nkv, int hd, int rotary_dim, const void* cos,
                    const void* sin, int pos0, cudaStream_t s) {
   const int half = rotary_dim / 2;
-  if (half % 8 != 0 || hd % 8 != 0 || ldo % 8 != 0 || sB % 8 != 0 || sH % 8 != 0 || sT % 8 != 0 || kB % 8 != 0 || kH % 8 != 0 || kT % 8 != 0)
-    throw std::runtime_error("rope_pack_bwd: head_dim / rotary_dim / strides must allow 128-bit accesses");
+  if (half % 8 != 0 || hd % 8 != 0) throw std::runtime_error("rope_pack_bwd: head_dim and rotary_dim must allow 128-bit accesses");
   if (nkv <= 0 || nkv > nh || nh % nkv != 0) throw std::runtime_error("rope_pack_bwd: nh must be a multiple of nkv");
   const long long total = (long long)B * T * nh * (hd / 8);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 16);
