@@ -69,7 +69,7 @@ def main():
         flops = 2.0 * Mx * N * K
         t_cublas = timeit(lambda: torch.matmul(x, W.t(), out=out), flush)
         rec = {"shape": name, "M": Mx, "N": N, "K": K, "cublas_us": t_cublas * 1e6, "cublas_tflops": flops / t_cublas / 1e12}
-        for bn in (128, 256):
+        for bn in (128, 192, 256):
             try:
                 t = timeit(lambda: F.gemm(x, W, out, block_n=bn, pair=0), flush)
                 rec[f"ours_bn{bn}_us"] = t * 1e6
@@ -108,6 +108,9 @@ def main():
             t = timeit(lambda: F.gemm(dy, W, dx, M=Mx, N=K, K1=N, b1_mn=True, pair=0), flush)
             rec["ours_dx_mnB_us"] = t * 1e6
             rec["ours_dx_mnB_tflops"] = flops / t / 1e12
+            for bn in (128, 192):
+                t = timeit(lambda: F.gemm(dy, W, dx, M=Mx, N=K, K1=N, b1_mn=True, block_n=bn, pair=0), flush)
+                rec[f"ours_dx_mnB_bn{bn}_us"] = t * 1e6
             t = timeit(lambda: F.gemm(dy, W, dx, M=Mx, N=K, K1=N, b1_mn=True, block_n=128, pair=1), flush)
             rec["ours_dx_mnB_pair_us"] = t * 1e6
             rec["ours_dx_mnB_pair_tflops"] = flops / t / 1e12

@@ -1,5 +1,5 @@
 """T(K) sweep at fixed M, N: separates the per-tile fixed cost (epilogue, tile hand-off) from the per-k-block cost
-(tensor pipe / L2 feed) for the 128- and 256-wide tiles of the wgmma GEMM, the 128-wide one also as CTA pairs.
+(tensor pipe / L2 feed) for the 128-, 192- and 256-wide tiles of the wgmma GEMM, the 128-wide one also as CTA pairs.
 
     python bench/gemm_ksweep.py [--M 12288] [--N 2304] [--out gemm_ksweep.json]
 """
@@ -35,6 +35,7 @@ for K in (128, 256, 512, 768, 1536, 3072, 6144):
     rec = {"M": a.M, "N": a.N, "K": K}
     rec["cublas_us"] = timeit(lambda: torch.matmul(x, W.t(), out=out), flush) * 1e6
     rec["bn128_us"] = timeit(lambda: F.gemm(x, W, out, block_n=128, pair=0), flush) * 1e6
+    rec["bn192_us"] = timeit(lambda: F.gemm(x, W, out, block_n=192, pair=0), flush) * 1e6
     rec["bn128_pair_us"] = timeit(lambda: F.gemm(x, W, out, block_n=128, pair=1), flush) * 1e6
     rec["bn256_us"] = timeit(lambda: F.gemm(x, W, out, block_n=256, pair=0), flush) * 1e6
     rec["pair_us"] = timeit(lambda: F.gemm(x, W, out, block_n=256, pair=1), flush) * 1e6

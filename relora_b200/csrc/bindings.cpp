@@ -248,7 +248,7 @@ void fp8_prep(Tensor& state, const Tensor& w_scale, Tensor& inv_sx, Tensor& alph
 
 // out[M,N] = dy[M,Kb]·W[Kb,N] + Σ_g keep_g ⊙ (du_g·A_g)/(1-p)     (fused input gradient of a stacked LoRA group)
 void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Tensor& a, Tensor& out, const OptTensor& seed,
-             std::vector<int64_t> keys, double p, const OptTensor& base, int64_t pair) {
+             std::vector<int64_t> keys, double p, const OptTensor& base, int64_t pair, int64_t block_n) {
   const Call c{"lora_dx", out.device()};
   const Dropout dr = dropout(c, seed, keys, p, 1, 3);
   rb::LoraDxDesc d;
@@ -272,6 +272,8 @@ void lora_dx(const OptTensor& dy, const OptTensor& w, const Tensor& du, const Te
   d.drop_threshold16 = dr.thr16; d.inv_keep = dr.inv_keep; d.seed_ptr = dr.seed;
   for (int i = 0; i < 3; ++i) d.seed_key[i] = dr.keys[i];
   d.pair = (int)pair;
+  TORCH_CHECK(block_n == 0 || block_n == 128 || block_n == 192, "lora_dx: block_n must be 0 (auto), 128 or 192");
+  d.block_n = (int)block_n;
   c10::cuda::CUDAGuard guard(c.dev);
   rb::lora_dx(d, cur_stream());
 }
@@ -714,16 +716,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "relora_b200 sm_90a kernels";
   m.def("gemm", &gemm, "wgmma GEMM with fused LoRA K-extension");
   m.def("gemm_clear_descriptor_cache", &rb::gemm_clear_descriptor_cache);
-  // host-side schedule of one gemm call (no launch): (block_n, tma_store, dynamic shared memory bytes, CTA pairs)
+  // host-side schedule of one gemm call (no launch): (block_n, tma_store, dynamic shared memory bytes, CTA pairs); sms: the
+  // SM count of the tile-width rule (0: this device's)
   m.def("gemm_plan", [](int64_t block_n, bool out_f32, int64_t out_addr, int64_t ldc, int64_t n, int64_t split_k, int64_t m,
-                        int64_t m_per_group, int64_t pair, int64_t k) {
+                        int64_t m_per_group, int64_t pair, int64_t k, int64_t n_per_group, bool accumulate, int64_t sms) {
     rb::GemmDesc d;
     d.block_n = (int)block_n; d.out_f32 = out_f32; d.out = reinterpret_cast<void*>(out_addr); d.ldc = ldc; d.N = (int)n;
     d.M = (int)m; d.m_per_group = (int)m_per_group; d.pair = (int)pair; d.K1 = (int)k;
-    const int bn = rb::gemm_block_n(d);
+    d.n_per_group = (int)n_per_group; d.accumulate = accumulate; d.split_k = (int)split_k;
+    const int bn = rb::gemm_block_n(d, (int)sms);
     return py::make_tuple(bn, rb::gemm_uses_tma_store(d, bn, (int)split_k), rb::gemm_smem_bytes(bn), rb::gemm_pairs(d, bn));
   }, py::arg("block_n"), py::arg("out_f32"), py::arg("out_addr"), py::arg("ldc"), py::arg("n"), py::arg("split_k"),
-     py::arg("m") = 0, py::arg("m_per_group") = 0, py::arg("pair") = -1, py::arg("k") = 0);
+     py::arg("m") = 0, py::arg("m_per_group") = 0, py::arg("pair") = -1, py::arg("k") = 0, py::arg("n_per_group") = 0,
+     py::arg("accumulate") = false, py::arg("sms") = 0);
   // (CTA pairs, TMA-store epilogue) of one lora_dx call with G = 1 and rank r
   m.def("lora_dx_plan", [](int64_t m, int64_t n, int64_t pair, int64_t kb, int64_t r) {
     rb::LoraDxDesc d;
@@ -750,7 +755,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("interleaved") = false, py::arg("nkv") = -1);
   m.def("attention_ds_workspace_elems", &rb::attention_ds_workspace_elems);
   m.def("lora_dx", &lora_dx, py::arg("dy"), py::arg("w"), py::arg("du"), py::arg("a"), py::arg("out"), py::arg("seed"), py::arg("keys"),
-        py::arg("p"), py::arg("base") = py::none(), py::arg("pair") = -1);
+        py::arg("p"), py::arg("base") = py::none(), py::arg("pair") = -1, py::arg("block_n") = 0);
   m.def("rope_inplace", &rope_inplace);
   m.def("rope_pack_bwd", &rope_pack_bwd, py::arg("dq"), py::arg("dk"), py::arg("dv"), py::arg("out"), py::arg("rotary_dim"), py::arg("cos"),
         py::arg("sin"), py::arg("pos0"), py::arg("nkv") = -1);

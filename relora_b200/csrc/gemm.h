@@ -44,7 +44,7 @@ struct GemmDesc {
   const float* alpha_dev = nullptr;  // optional device scalar multiplied into alpha
   bool fp8_a_e5m2 = false;  // with fp8: A1 is E5M2 (gradients), B1 stays E4M3
   bool fp8 = false;  // A1 / B1 hold E4M3 bytes (K-major, leading dimensions in bytes); A2 / B2 (the LoRA branch) stay bf16
-  int block_n = 0;  // 0 = auto, else 128 or 256
+  int block_n = 0;  // 0 = auto (gemm_block_n), else 128, 192 or 256
   int split_k = 1;  // 1 = off, 0 = auto, >1 = fixed (fp32 accumulate outputs only: partial sums via atomics)
   int pair = -1;    // CTA pairs sharing the B tile (gemm_pairs): -1 = auto, 0 = off, 1 = wherever the call form allows
   // dropout-combine epilogue (backward of the LoRA branch): if n_lora_acc > 0 the A2/B2 products of
@@ -70,7 +70,8 @@ struct GemmExtents {
 GemmExtents gemm_operand_extents(const GemmDesc& d);
 // Schedule choices of gemm_bf16 (host side): the tile width, whether the epilogue stores through shared memory with TMA,
 // and the dynamic shared memory of a tile width.
-int gemm_block_n(const GemmDesc& d);
+// sms: the SM count the wave rule fills (0: this device's)
+int gemm_block_n(const GemmDesc& d, int sms = 0);
 bool gemm_uses_tma_store(const GemmDesc& d, int block_n, int split_k);
 int gemm_smem_bytes(int block_n);
 // whether the call runs as CTA pairs: 128-wide tiles, at least two M tiles, M groups of whole pairs; auto: long reductions
@@ -96,9 +97,11 @@ struct LoraDxDesc {
   const uint32_t* seed_ptr = nullptr;
   uint32_t seed_key[3] = {0, 0, 0};
   int pair = -1;  // CTA pairs sharing the A / W tile: -1 = auto (gemm_pairs' rule), 0 = off, 1 = on when M has two tiles or more
+  int block_n = 0;  // output tile width: 0 = auto (the GEMM's wave rule), 128 or 192 (192 never pairs)
 };
 void lora_dx(const LoraDxDesc& d, cudaStream_t stream);
 bool lora_dx_pairs(const LoraDxDesc& d);
+int lora_dx_block_n(const LoraDxDesc& d);
 // the output leaves through shared memory and TMA stores unless a row is not a whole number of 16-byte chunks
 bool lora_dx_uses_tma_store(const LoraDxDesc& d);
 

@@ -1,6 +1,7 @@
 // Persistent warp-specialised bf16 / fp8 GEMM for sm_90a: TMA -> shared memory (128B swizzle) -> wgmma with fp32
-// accumulators in registers -> epilogue.  bf16 outputs of the 128-wide tile leave through a shared-memory staging buffer
-// and TMA stores that drain while the next tile's k-loop runs; fp32, split-K and unaligned outputs are stored from registers.
+// accumulators in registers -> epilogue.  bf16 outputs of the 128- and 192-wide tiles leave through a shared-memory staging
+// buffer and TMA stores that drain while the next tile's k-loop runs; fp32, split-K and unaligned outputs are stored from
+// registers.
 //
 //   D[M,N] = alpha * ( A1[M,K1]·B1[N,K1]ᵀ + A2[M,K2]·B2[N,K2]ᵀ ) (+ bias) (+ residual) (+ D)
 //
@@ -53,6 +54,7 @@ struct KernelArgs {
   int split_k;  // >1: each output tile is computed by split_k CTAs over disjoint K ranges, combined with fp32 atomics
   int tma_store;  // bf16 output through shared memory and TMA stores (map_out); else stored from registers
   int paired;     // clusters of 2 CTAs own M-tiles (2i, 2i + 1) of one N tile and multicast the B tile (CtaPair)
+  int block_n;    // tile width: 128 or 192 in gemm_kernel<128, ...>, 256 in gemm_kernel<256, ...>
 };
 
 template <int BLOCK_N>
@@ -60,15 +62,17 @@ struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;  // 16 KB
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (192 * 1024) / kStageBytes;  // 6 stages of 128-wide tiles, 4 of 256-wide tiles
+  static constexpr int kStages = (192 * 1024) / kStageBytes;  // 6 stages of 128-wide tiles, 4 of 192- and 256-wide tiles
   static constexpr int kTileBytes = kStages * kStageBytes;
   static constexpr int kRingTotal = kTileBytes + 1024 + 1024;  // ring, barriers, manual 1024-byte alignment (lora_dx)
-  // gemm_kernel: + the store staging of the bf16 epilogue, two 64 x 64 sub-tiles (8 KB, 128B-swizzled) per consumer
-  // warpgroup.  128-wide tiles only: with the 128 accumulator registers of a 256-wide tile the staging code spills.
-  static constexpr int kStoreBytes = BLOCK_N == 128 ? 2 * 2 * 64 * 64 * 2 : 0;
+  // + the store staging of the bf16 epilogue, one 64 x 64 sub-tile (8 KB, 128B-swizzled) per 64 columns of each consumer
+  // warpgroup's rows.  Not for 256-wide tiles: with their 128 accumulator registers the staging code spills.
+  static constexpr int kSubTiles = BLOCK_N == 256 ? 0 : BLOCK_N / 64;
+  static constexpr int kStoreBytes = 2 * kSubTiles * 64 * 64 * 2;
   static constexpr int kTotal = kRingTotal + kStoreBytes;
 };
-static_assert(SmemLayout<256>::kTotal <= 232448 && SmemLayout<128>::kTotal <= 232448, "shared memory budget");
+static_assert(SmemLayout<128>::kTotal <= 232448 && SmemLayout<192>::kTotal <= 232448 && SmemLayout<256>::kTotal <= 232448,
+              "shared memory budget");
 
 // Issue the TMA loads of one operand tile (BLOCK_MN x BLOCK_K) into `dst`.
 template <int BLOCK_MN, bool MN_MAJOR>
@@ -139,6 +143,7 @@ __device__ __forceinline__ void mma_bf16_kblock(float (&acc)[BLOCK_N / 2], uint3
 #pragma unroll
   for (int k = 0; k < BLOCK_K / 16; ++k) {
     if constexpr (BLOCK_N == 256) wgmma_bf16_ss_n256<A_MN, B_MN>(acc, da + kStepA * k, db + kStepB * k);
+    else if constexpr (BLOCK_N == 192) wgmma_bf16_ss_n192<A_MN, B_MN>(acc, da + kStepA * k, db + kStepB * k);
     else if constexpr (BLOCK_N == 128) wgmma_bf16_ss_n128<A_MN, B_MN>(acc, da + kStepA * k, db + kStepB * k);
     else wgmma_bf16_ss_n64<A_MN, B_MN>(acc, da + kStepA * k, db + kStepB * k);
   }
@@ -197,11 +202,10 @@ struct MmaRing {
   }
 };
 
+// The whole persistent schedule of one tile width (the body of gemm_kernel).
 template <int BLOCK_N, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ CUtensorMap map_b1,
-            const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b2,
-            const __grid_constant__ CUtensorMap map_out, const KernelArgs p) {
+__device__ __forceinline__ void gemm_tiles(const CUtensorMap& map_a1, const CUtensorMap& map_b1, const CUtensorMap& map_a2,
+                                           const CUtensorMap& map_b2, const CUtensorMap& map_out, const KernelArgs& p) {
   using L = SmemLayout<BLOCK_N>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -295,6 +299,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
   const bool store_lead = (threadIdx.x & 127) == 0;  // issues and waits for this warpgroup's TMA stores
   const uint32_t stage_u32 = smem0 + L::kTileBytes;  // store staging, 1024-byte aligned (128B swizzle)
   const bool plain = p.bias == nullptr && p.residual == nullptr && !p.accumulate;
+  const bool res_only = p.bias == nullptr && res_vec && !p.accumulate;  // residual, read as aligned column pairs
   float acc[BLOCK_N / 2];
   for (int work = pair.first_unit(); work < num_work; work += pair.unit_stride()) {
     const int tile = work / p.split_k, split = work % p.split_k;
@@ -310,7 +315,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
     fence_regs(acc);
     // The operand type is chosen once per segment, so each loop body is one straight batch of wgmma.
-    if (p.fp8 == 2) {
+    if constexpr (BLOCK_N == 192) {  // bf16 operands only (the host refuses fp8 at this width)
+      ring.run(kb_mid - kb_begin, [&](uint32_t s) { mma_bf16_kblock<BLOCK_N, A_MN, B_MN>(acc, s + a_ofs, s + L::kABytes); });
+    } else if (p.fp8 == 2) {
       ring.run(kb_mid - kb_begin, [&](uint32_t s) { mma_fp8_kblock<BLOCK_N, true>(acc, s + a_ofs, s + L::kABytes); });
     } else if (p.fp8) {
       ring.run(kb_mid - kb_begin, [&](uint32_t s) { mma_fp8_kblock<BLOCK_N, false>(acc, s + a_ofs, s + L::kABytes); });
@@ -321,20 +328,37 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
     ring.drain();
     fence_regs(acc);
     if (m0 >= p.M) continue;  // a pair's second tile past M
-    if (BLOCK_N == 128 && p.tma_store) {
-      // ---- bf16 epilogue through shared memory: both 64-column sub-tiles of the warpgroup's 64 rows are written to staging
-      // buffers in the TMA box layout, then one proxy fence and one barrier, and one thread stores them; the stores drain
+    if (L::kSubTiles > 0 && p.tma_store) {
+      // ---- bf16 epilogue through shared memory: every 64-column sub-tile of the warpgroup's 64 rows is written to a staging
+      // buffer in the TMA box layout, then one proxy fence and one barrier, and one thread stores them; the stores drain
       // while the next tile's k-loop runs.  Same fp32 operations in the same order as the register path below, one
       // rounding.  A group's ragged last tile stores only the sub-tiles inside the group (group widths are multiples of 64);
       // the TMA unit clips rows and columns past the tensor, so without bias, residual or accumulation (`plain`) no element
       // needs a bounds check: that path is a multiply, a pack and a shared store per column pair, where the general one
-      // spends tens of instructions on uniform tests and bounds (about 3 us per tile at N 5120, K 768).
+      // spends tens of instructions on uniform tests and bounds (about 3 us per tile at N 5120, K 768).  A residual alone
+      // over a sub-tile wholly inside M and the group adds one 4-byte load per column pair to that path.
       if (store_lead) bulk_wait_read<0>();  // the previous tile's stores, issued a whole k-loop ago, have read the staging
       named_bar_sync(1 + cw, 128);
 #pragma unroll
-      for (int j = 0; j < BLOCK_N / 64; ++j) {
+      for (int j = 0; j < L::kSubTiles; ++j) {
         if (n0 + j * 64 >= n_lim) break;
-        const uint32_t buf = stage_u32 + (cw * 2 + j) * 8192;
+        const uint32_t buf = stage_u32 + (cw * L::kSubTiles + j) * 8192;
+        if (res_only && m0 + cw * 64 + 64 <= p.M && n0 + j * 64 + 64 <= n_lim) {
+          // the thread's two rows (frag_row: r and r + 8), column pair (threadIdx.x & 3) of each 8-column chunk
+          const uint32_t* res = reinterpret_cast<const uint32_t*>(p.residual + (long long)(m0 + cw * 64 + frag_row(0)) * p.ldr + n0 +
+                                                                  j * 64 + (threadIdx.x & 3) * 2);
+          const long long res8 = 4 * p.ldr;  // 8 rows, in 4-byte pairs
+#pragma unroll
+          for (int q = 0; q < 32; q += 2) {
+            const int i = j * 32 + q;
+            const int r = frag_row(i);
+            const float2 rv = unpack_bf16x2(res[((q >> 1) & 1) * res8 + (q >> 2) * 4]);
+            // __fadd_rn: a product and a sum, never contracted into one fma, as in the general path
+            st_shared_u32(buf + r * 128 + (((q >> 2) ^ (r & 7)) << 4) + (threadIdx.x & 3) * 4,
+                          pack_bf16x2(__fadd_rn(acc[i] * alpha_eff, rv.x), __fadd_rn(acc[i + 1] * alpha_eff, rv.y)));
+          }
+          continue;
+        }
         if (plain) {
 #pragma unroll
           for (int q = 0; q < 32; q += 2) {
@@ -357,7 +381,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
               v0 += __bfloat162float(p.bias[col]);
               if (pair_ok) v1 += __bfloat162float(p.bias[col + 1]);
             }
-            const long long ofs = (long long)row * p.ldc + col;
             if (p.residual != nullptr) {
               const bf16* rp = p.residual + (long long)row * p.ldr + col;
               if (pair_ok && res_vec) {
@@ -370,7 +393,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
               }
             }
             if (p.accumulate) {
-              const bf16* op = reinterpret_cast<const bf16*>(p.out) + ofs;
+              const bf16* op = reinterpret_cast<const bf16*>(p.out) + (long long)row * p.ldc + col;
               v0 += __bfloat162float(op[0]);
               if (pair_ok) v1 += __bfloat162float(op[1]);
             }
@@ -383,9 +406,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
       named_bar_sync(1 + cw, 128);
       if (store_lead) {
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 64; ++j) {
+        for (int j = 0; j < L::kSubTiles; ++j) {
           if (n0 + j * 64 >= n_lim) break;
-          tma_store_2d(&map_out, stage_u32 + (cw * 2 + j) * 8192, n0 + j * 64, m0 + cw * 64);
+          tma_store_2d(&map_out, stage_u32 + (cw * L::kSubTiles + j) * 8192, n0 + j * 64, m0 + cw * 64);
         }
         bulk_commit();
       }
@@ -453,6 +476,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
   pair.finish();
 }
 
+// One kernel per operand-major combination and tile family: the 128-wide instantiation also runs 192-wide tiles (p.block_n),
+// whose shared-memory layout fits in the 128-wide one's opt-in; the 256-wide tile has its own.
+template <int BLOCK_N, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ CUtensorMap map_b1,
+            const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b2,
+            const __grid_constant__ CUtensorMap map_out, const KernelArgs p) {
+  if constexpr (BLOCK_N == 128) {
+    if (p.block_n == 192) {
+      gemm_tiles<192, A_MN, B_MN>(map_a1, map_b1, map_a2, map_b2, map_out, p);
+      return;
+    }
+  }
+  gemm_tiles<BLOCK_N, A_MN, B_MN>(map_a1, map_b1, map_a2, map_b2, map_out, p);
+}
+
 // =============================================================================================
 // Fused backward of a stacked LoRA group (input gradient):
 //
@@ -463,7 +502,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a1, const __grid_constant__ 
 // frozen path.  Each consumer warpgroup runs the G short LoRA products first into one register accumulator, folds each
 // one, masked, into a second, and then lets the long frozen-path reduction accumulate on top of the combined term: one
 // write of dx instead of base-GEMM + parts-GEMM + dropout_combine.  With Kb == 0 the frozen-path product `base` was
-// computed by a separate GEMM and is added from global memory.
+// computed by a separate GEMM and is added from global memory.  With one group (kOneGroup) the mask is applied to the LoRA
+// product in place, so a 192-wide tile needs only its 96 accumulator registers.  Two or three groups keep the 128-wide
+// tile: a 192-wide one would hold two 96-register accumulators, and ptxas spills it (288 bytes) within the kernel's 168
+// registers per thread.
 // Reference math: backward of relora.py:319-322 with nn.Dropout on the LoRA input.
 struct LoraDxArgs {
   int M, N, Kb, r, G;
@@ -478,13 +520,14 @@ struct LoraDxArgs {
   uint32_t keys[3];
   int paired;     // CTA pairs share the MN-major A / W tile (CtaPair)
   int tma_store;  // output through shared memory and TMA stores (map_out); else stored from registers
+  int block_n;    // 128, or 192 (one group only)
 };
 
-__global__ void __launch_bounds__(kNumThreads, 1)
-lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_w,
-               const __grid_constant__ CUtensorMap map_du, const __grid_constant__ CUtensorMap map_a,
-               const __grid_constant__ CUtensorMap map_out, const LoraDxArgs p) {
-  constexpr int BLOCK_N = 128;
+// The whole persistent schedule of one tile width (the body of lora_dx_kernel).
+template <int BLOCK_N, bool kOneGroup>
+__device__ __forceinline__ void lora_dx_tiles(const CUtensorMap& map_dy, const CUtensorMap& map_w, const CUtensorMap& map_du,
+                                              const CUtensorMap& map_a, const CUtensorMap& map_out, const LoraDxArgs& p) {
+  static_assert(BLOCK_N == 128 || kOneGroup, "two or more groups run on the 128-wide tile");
   using L = SmemLayout<BLOCK_N>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -564,27 +607,42 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
     ring.drain();
     fence_regs(acc);
   };
-  float acc[BLOCK_N / 2], cmb[BLOCK_N / 2];
+  float acc[BLOCK_N / 2], cmb[kOneGroup ? 1 : BLOCK_N / 2];
   for (int work = pair.first_unit(); work < num_work; work += pair.unit_stride()) {
     const int m0 = pair.m_tile(work / p.num_n_tiles) * BLOCK_M + cw * 64;
     const int n0 = (work % p.num_n_tiles) * BLOCK_N;
-#pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) cmb[i] = 0.f;
-    for (int g = 0; g < p.G; ++g) {
+    if constexpr (kOneGroup) {
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
       mma_blocks(acc, kb_lora);
-      const uint32_t seed = mix_seed(seed0, g == 0 ? p.keys[0] : g == 1 ? p.keys[1] : p.keys[2]);
+      const uint32_t seed = mix_seed(seed0, p.keys[0]);
+      // (0 + acc) * inv_keep where kept, else 0: the values of the G >= 2 form below, the sign of a zero included
 #pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; i += 2) {  // one hash per column pair (common.cuh:keep_drop)
+      for (int i = 0; i < BLOCK_N / 2; i += 2) {
         const uint32_t row = m0 + frag_row(i), col = n0 + frag_col(i);
         const uint32_t hsh = lowbias32((row * 0x9E3779B1u) ^ seed ^ ((col >> 1) * 0x85EBCA77u));
-        if ((hsh & 0xFFFFu) >= p.thr16) cmb[i] += acc[i];
-        if ((hsh >> 16) >= p.thr16) cmb[i + 1] += acc[i + 1];
+        acc[i] = (hsh & 0xFFFFu) >= p.thr16 ? __fmul_rn(__fadd_rn(0.f, acc[i]), p.inv_keep) : 0.f;
+        acc[i + 1] = (hsh >> 16) >= p.thr16 ? __fmul_rn(__fadd_rn(0.f, acc[i + 1]), p.inv_keep) : 0.f;
       }
-    }
+    } else {
 #pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = cmb[i] * p.inv_keep;
+      for (int i = 0; i < BLOCK_N / 2; ++i) cmb[i] = 0.f;
+      for (int g = 0; g < p.G; ++g) {
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+        mma_blocks(acc, kb_lora);
+        const uint32_t seed = mix_seed(seed0, g == 0 ? p.keys[0] : g == 1 ? p.keys[1] : p.keys[2]);
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; i += 2) {  // one hash per column pair (common.cuh:keep_drop)
+          const uint32_t row = m0 + frag_row(i), col = n0 + frag_col(i);
+          const uint32_t hsh = lowbias32((row * 0x9E3779B1u) ^ seed ^ ((col >> 1) * 0x85EBCA77u));
+          if ((hsh & 0xFFFFu) >= p.thr16) cmb[i] += acc[i];
+          if ((hsh >> 16) >= p.thr16) cmb[i + 1] += acc[i + 1];
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = cmb[i] * p.inv_keep;
+    }
     if (kb_base > 0) mma_blocks(acc, kb_base);  // the frozen-path product accumulates on top of the combined LoRA term
     if (m0 >= p.M) continue;  // rows past M: a ragged last tile's second warpgroup, or a pair's second tile past M
     if (p.tma_store) {
@@ -599,7 +657,7 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
           else bulk_wait_read<1>();
         }
         named_bar_sync(1 + cw, 128);
-        const uint32_t buf = stage_u32 + (cw * 2 + j) * 8192;
+        const uint32_t buf = stage_u32 + (cw * L::kSubTiles + j) * 8192;
 #pragma unroll
         for (int q = 0; q < 32; q += 2) {
           const int i = j * 32 + q;
@@ -637,6 +695,14 @@ lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant
   }
   if (store_lead && p.tma_store) bulk_wait_all();  // the staging buffers must outlive the stores that read them
   pair.finish();
+}
+
+__global__ void __launch_bounds__(kNumThreads, 1)
+lora_dx_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_w,
+               const __grid_constant__ CUtensorMap map_du, const __grid_constant__ CUtensorMap map_a,
+               const __grid_constant__ CUtensorMap map_out, const LoraDxArgs p) {
+  if (p.block_n == 192) lora_dx_tiles<192, true>(map_dy, map_w, map_du, map_a, map_out, p);
+  else lora_dx_tiles<128, false>(map_dy, map_w, map_du, map_a, map_out, p);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -780,7 +846,7 @@ GemmExtents gemm_operand_extents(const GemmDesc& d) {
 // chunk it writes beyond column N.  fp32 outputs (weight gradients, accumulated or split-K with atomics) and 256-wide tiles
 // keep the register epilogue.
 bool gemm_uses_tma_store(const GemmDesc& d, int block_n, int split_k) {
-  return block_n == 128 && !d.out_f32 && split_k == 1 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && d.ldc % 8 == 0 &&
+  return block_n != 256 && !d.out_f32 && split_k == 1 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && d.ldc % 8 == 0 &&
          d.N % 8 == 0;
 }
 
@@ -814,6 +880,7 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
   if (d.fp8 && (A_MN || B_MN)) throw std::runtime_error("gemm: fp8 operands must be K-major");
   CUtensorMap ma1 = operand_map(d.a1, e.a1, BLOCK_M, d.fp8);
   if (d.m_per_group > 0 && (d.m_per_group % BLOCK_M) != 0) throw std::runtime_error("gemm: m_per_group must be a multiple of the M tile");
+  if (BLOCK_N == 192 && d.fp8) throw std::runtime_error("gemm: fp8 operands run on the 128- or 256-wide tile");
   const bool paired = gemm_pairs(d, BLOCK_N);
   p.paired = paired ? 1 : 0;
   const int b_box = paired ? BLOCK_N / 2 : BLOCK_N;  // each CTA of a pair loads half of the B tile
@@ -824,11 +891,16 @@ static void launch(const GemmDesc& d, cudaStream_t stream) {
     ma2 = operand_map(d.a2, e.a2, BLOCK_M);
     mb2 = operand_map(d.b2, e.b2, b_box);
   }
-  auto kern = gemm_kernel<BLOCK_N, A_MN, B_MN>;
+  // 192-wide tiles run in the 128-wide kernel, whose opt-in covers both layouts
+  constexpr int kKernelN = BLOCK_N == 192 ? 128 : BLOCK_N;
+  constexpr int kOptIn = SmemLayout<kKernelN>::kTotal;
+  static_assert(L::kTotal <= kOptIn, "a tile's layout must fit in its kernel's opt-in");
+  auto kern = gemm_kernel<kKernelN, A_MN, B_MN>;
+  p.block_n = BLOCK_N;
   static int max_pairs = 0;  // clusters of 2 resident at once
   if (max_pairs == 0) {
-    check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal), "cudaFuncSetAttribute(gemm)");
-    max_pairs = max_active_clusters(kern, 2, kNumThreads, L::kTotal);
+    check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptIn), "cudaFuncSetAttribute(gemm)");
+    max_pairs = max_active_clusters(kern, 2, kNumThreads, kOptIn);
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int num_kb = ceil_div(d.K1, d.fp8 ? 2 * BLOCK_K : BLOCK_K) + ceil_div(d.K2, BLOCK_K);
@@ -863,14 +935,37 @@ static void dispatch_major(const GemmDesc& d, cudaStream_t s) {
   }
 }
 
-// Tile width: 128 unless the caller asks for 256 (block_n 0 = auto).  On an H100 80GB HBM3 at 700 W (bench/gemm_bench.py, M 12288, plain
-// bf16 GEMM with the register epilogue) the 256-wide tile ran at 192 - 387 TFLOP/s on the llama_1b shapes and 410 at 8192^3,
-// the 128-wide one at 466 - 548 and 440; with the fused LoRA branch the 256-wide tile took 2.0 - 2.5x as long on every
-// llama_250m / llama_1b projection.  The K sweep (bench/gemm_ksweep.py) puts the difference in the per-tile fixed cost:
-// 528 vs 260 us at K = 128, N = 5120.  Only the 128-wide tile has the TMA-store epilogue (the 256-wide one would spill).
-int gemm_block_n(const GemmDesc& d) { return d.block_n == 256 ? 256 : 128; }
+// Width of the output tiles by wave count: the grid is one CTA per SM and tiles go round-robin, so a width costs
+// ceil(tiles / SMs) tile-times, each tile-time scaled by the width's per-tile cost; a ragged tile counts whole.  The
+// 192-wide tile costs kCost192 of a 128-wide one.  It is taken only when strictly cheaper, so ties go to 128.  kCost192 = 1.5
+// is the ratio of the widths, not a measured per-tile cost (bench/gemm_ksweep.py's bn192 column measures it); at 1.5 the
+// llama_250m N 768 outputs and the qkv projection take 192 and N 5120 ties.  On an H100 80GB HBM3 at 700 W this rule took
+// bench.py's llama_250m from 213,744 - 214,913 tokens/s to 227,530 - 227,713 (3 runs each, alternating).
+int tile_width_by_waves(int m, int n, int n_per_group, int sms) {
+  constexpr double kCost192 = 1.5;
+  if (sms <= 0 || m <= 0 || n <= 0 || n_per_group <= 0) return 128;
+  const long long m_tiles = ceil_div(m, BLOCK_M), groups = ceil_div(n, n_per_group);
+  const auto waves = [&](int bn) { return ceil_div(m_tiles * groups * ceil_div(n_per_group, bn), sms); };
+  return kCost192 * waves(192) < waves(128) ? 192 : 128;
+}
 
-int gemm_smem_bytes(int block_n) { return block_n == 256 ? SmemLayout<256>::kTotal : SmemLayout<128>::kTotal; }
+// Tile width (block_n 0 = auto; 128, 192 or 256 on request).  Auto runs bf16 outputs of bf16 operands at 192 where the
+// wave count says so (tile_width_by_waves), and at 128 otherwise: fp32, accumulated and split-K outputs, fp8 operands, and
+// calls that pair at 128 (gemm_pairs), whose shared B tile is worth more than a wave.  On an H100 80GB HBM3 at 700 W
+// (bench/gemm_bench.py, M 12288, plain bf16 GEMM with the register epilogue) the 256-wide tile ran at 192 - 387 TFLOP/s
+// on the llama_1b shapes and 410 at 8192^3, the 128-wide one at 466 - 548 and 440; with the fused LoRA branch the
+// 256-wide tile took 2.0 - 2.5x as long on every llama_250m / llama_1b projection.  The K sweep (bench/gemm_ksweep.py)
+// puts the difference in the per-tile fixed cost: 528 vs 260 us at K = 128, N = 5120.  The 256-wide tile has no
+// TMA-store epilogue (it would spill), so auto never picks it.
+int gemm_block_n(const GemmDesc& d, int sms) {
+  if (d.block_n != 0) return d.block_n == 256 || d.block_n == 192 ? d.block_n : 128;
+  if (d.out_f32 || d.accumulate || d.split_k > 1 || d.fp8 || gemm_pairs(d, 128)) return 128;
+  return tile_width_by_waves(d.M, d.N, gemm_n_per_group(d), sms > 0 ? sms : num_sms());
+}
+
+int gemm_smem_bytes(int block_n) {
+  return block_n == 256 ? SmemLayout<256>::kTotal : block_n == 192 ? SmemLayout<192>::kTotal : SmemLayout<128>::kTotal;
+}
 
 // CTA pairs (CtaPair): the 128-wide tile only, M of at least two tiles, and M groups (weight gradients) that hold whole
 // pairs, since a pair shares one B tile.  Auto (pair = -1) pairs long reductions into wide outputs: N >= 2048 and at least
@@ -888,34 +983,46 @@ bool gemm_pairs(const GemmDesc& d, int block_n) {
 void gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
   if (d.n_lora_acc != 0) throw std::runtime_error("gemm: dropout-combine epilogue not built into this kernel variant");
   if (d.M <= 0 || d.N <= 0) return;
-  if (gemm_block_n(d) == 256) dispatch_major<256>(d, stream);
+  const int bn = gemm_block_n(d);
+  if (bn == 256) dispatch_major<256>(d, stream);
+  else if (bn == 192) dispatch_major<192>(d, stream);
   else dispatch_major<128>(d, stream);
 }
 
-// Pairs share the A / W tile (MN-major, 64-wide chunks); every call form of this kernel can pair.  Auto: the GEMM's rule
+// Pairs share the A / W tile (MN-major, 64-wide chunks); every call form of the 128-wide tile can pair.  Auto: the GEMM's rule
 // (bench/lora_dx_bench.py, same card: pairs 15 % faster on llama_1b down (N 5504) and 3 % on o (N 2048), 7 - 13 % slower
 // at N 768).
-bool lora_dx_pairs(const LoraDxDesc& d) {
+static bool lora_dx_pairs_at_128(const LoraDxDesc& d) {
   if (d.pair == 0 || ceil_div(d.M, BLOCK_M) < 2) return false;
   const int num_kb = d.groups * d.r / BLOCK_K + ceil_div(d.Kb, BLOCK_K);
   return d.pair == 1 || (d.N >= 2048 && num_kb >= 32);
 }
+// Tile width: 128 for two or three groups (lora_dx_kernel); with one group, 192 on request, and on auto the GEMM's wave
+// rule over N unless the call pairs at 128.
+int lora_dx_block_n(const LoraDxDesc& d) {
+  if (d.groups > 1 || d.block_n == 128) return 128;
+  if (d.block_n == 192) return 192;
+  return lora_dx_pairs_at_128(d) ? 128 : tile_width_by_waves(d.M, d.N, d.N, num_sms());
+}
+bool lora_dx_pairs(const LoraDxDesc& d) { return lora_dx_block_n(d) == 128 && lora_dx_pairs_at_128(d); }
 // the base, pitch and alignment rules below hold for every call; only a ragged last 16-byte chunk of a row keeps the
 // register epilogue (a TMA store would write past column N)
 bool lora_dx_uses_tma_store(const LoraDxDesc& d) { return d.N % 8 == 0; }
 
-void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
-  if (d.M <= 0 || d.N <= 0) return;
-  if (d.r <= 0 || d.r % BLOCK_K != 0) throw std::runtime_error("lora_dx: the LoRA rank must be a multiple of 64");
-  if (d.Kb == 0 && d.base == nullptr) throw std::runtime_error("lora_dx: Kb == 0 needs the base product");
-  if (d.N % 2 != 0) throw std::runtime_error("lora_dx: N must be even");
-  using L = SmemLayout<128>;
+
+template <int BLOCK_N>
+static void lora_dx_launch(const LoraDxDesc& d, cudaStream_t stream) {
+  using L = SmemLayout<BLOCK_N>;
+  constexpr int kOptIn = SmemLayout<128>::kTotal;  // the larger layout: one opt-in for both widths
+  static_assert(L::kTotal <= kOptIn, "a tile's layout must fit in the kernel's opt-in");
+  auto kern = lora_dx_kernel;
   LoraDxArgs p;
+  p.block_n = BLOCK_N;
   p.M = d.M; p.N = d.N; p.Kb = d.Kb; p.r = d.r; p.G = d.groups;
   p.out = reinterpret_cast<bf16*>(d.out); p.ldc = d.ldc;
   p.base = reinterpret_cast<const bf16*>(d.base); p.ld_base = d.ld_base;
   p.num_m_tiles = ceil_div(d.M, BLOCK_M);
-  p.num_n_tiles = ceil_div(d.N, 128);
+  p.num_n_tiles = ceil_div(d.N, BLOCK_N);
   p.thr16 = d.drop_threshold16; p.inv_keep = d.inv_keep; p.seed_ptr = d.seed_ptr;
   for (int g = 0; g < 3; ++g) p.keys[g] = d.seed_key[g];
   CUtensorMap m_du = make_map_2d(d.du, (long long)d.groups * d.r, d.M, d.ld_du, BLOCK_K, BLOCK_M);
@@ -930,14 +1037,23 @@ void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
   const CUtensorMap m_out = p.tma_store ? make_map_2d(d.out, d.N, d.M, d.ldc, 64, 64) : m_du;
   static int max_pairs = 0;  // clusters of 2 resident at once
   if (max_pairs == 0) {
-    check(cudaFuncSetAttribute(lora_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal), "cudaFuncSetAttribute(lora_dx)");
-    max_pairs = max_active_clusters(lora_dx_kernel, 2, kNumThreads, L::kTotal);
+    check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptIn), "cudaFuncSetAttribute(lora_dx)");
+    max_pairs = max_active_clusters(kern, 2, kNumThreads, kOptIn);
   }
   const int cta_per_unit = p.paired ? 2 : 1;
   const int work = ceil_div(p.num_m_tiles, cta_per_unit) * p.num_n_tiles;
   const int grid = std::min(work, p.paired ? max_pairs : num_sms()) * cta_per_unit;
-  launch_k_cluster(cta_per_unit, lora_dx_kernel, grid, kNumThreads, L::kTotal, stream, m_dy, m_w, m_du, m_a, m_out, p);
+  launch_k_cluster(cta_per_unit, kern, grid, kNumThreads, L::kTotal, stream, m_dy, m_w, m_du, m_a, m_out, p);
   RB_CHECK_LAUNCH("lora_dx_kernel");
+}
+
+void lora_dx(const LoraDxDesc& d, cudaStream_t stream) {
+  if (d.M <= 0 || d.N <= 0) return;
+  if (d.r <= 0 || d.r % BLOCK_K != 0) throw std::runtime_error("lora_dx: the LoRA rank must be a multiple of 64");
+  if (d.Kb == 0 && d.base == nullptr) throw std::runtime_error("lora_dx: Kb == 0 needs the base product");
+  if (d.N % 2 != 0) throw std::runtime_error("lora_dx: N must be even");
+  if (lora_dx_block_n(d) == 192) lora_dx_launch<192>(d, stream);  // one group (lora_dx_block_n)
+  else lora_dx_launch<128>(d, stream);
 }
 
 }  // namespace rb

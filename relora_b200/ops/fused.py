@@ -91,6 +91,7 @@ def gemm(
 ) -> torch.Tensor:
     """``out[M,N] = alpha·(a1·b1ᵀ + a2·b2ᵀ) (+ residual) (+ out)`` on the wgmma kernel.
 
+    ``block_n``: output tile width, 0 = the dispatcher's wave-count rule (``gemm_block_n``), else 128, 192 or 256.
     ``pair``: CTA pairs, two M tiles of one N tile sharing each B tile through TMA multicast: -1 lets the dispatcher
     choose (``gemm_pairs``), 0 turns them off, 1 asks for them where the call form allows (the 256-wide tile does not).
     ``fp8``: 1 = ``a1`` / ``b1`` hold E4M3 bytes (K-major), 2 = ``a1`` is E5M2 (gradients); ``alpha_dev``: fp32 device scalar multiplied into ``alpha``.
