@@ -11,7 +11,7 @@ import json
 import os
 from typing import Any, Dict
 
-__all__ = ["load_config", "save_config", "SimpleConfig", "config_to_dict", "rope_settings"]
+__all__ = ["load_config", "save_config", "SimpleConfig", "config_to_dict", "rope_settings", "rope_scaling"]
 
 _LLAMA_DEFAULTS = dict(
     model_type="llama",
@@ -131,6 +131,17 @@ def rope_settings(config):
     if (scaling is None or not scaling.get("type", scaling.get("rope_type"))) and rp.get("rope_type") not in (None, "default"):
         scaling = {"type": rp["rope_type"], "factor": rp.get("factor", 1.0)}
     return float(pct), base, scaling
+
+
+def rope_scaling(config):
+    """The rotary scaling dict as the config declares it, with every key it carries: ``rope_scaling`` when that names a type,
+    else the ``rope_parameters`` of transformers >= 5 when its ``rope_type`` is not ``default``; None when rotary embeddings
+    are unscaled."""
+    scaling = getattr(config, "rope_scaling", None)
+    if scaling and scaling.get("type", scaling.get("rope_type")):
+        return scaling
+    rp = getattr(config, "rope_parameters", None) or {}
+    return rp if rp.get("rope_type") not in (None, "default") else None
 
 
 def config_to_dict(config) -> Dict[str, Any]:

@@ -12,8 +12,10 @@ This is a plain ``nn.Module`` tree (no ``PreTrainedModel`` machinery); ``save_pr
 ``from_pretrained`` also reads Hugging Face Llama-family checkpoint directories (``model.safetensors``, or a
 sharded ``*.index.json`` of either format), which carry no ``inv_freq`` buffers.
 
-Grouped-query attention (``num_key_value_heads < num_attention_heads``) and ``rope_theta`` are supported; rotary
-scaling, tied embeddings and biased projections are refused (:func:`check_llama_config`).
+Grouped-query attention (``num_key_value_heads < num_attention_heads``), ``rope_theta`` and Llama-3.1's ``llama3`` rotary
+scaling are supported; other rotary scaling types, tied embeddings and biased projections are refused
+(:func:`check_llama_config`).  The layers share one rotary module, so the cos/sin tables (fp32, ``max_position_embeddings``
+long: 128 MB at Llama-3.1's 131072 positions and head_dim 128) exist once per model.
 
 Two execution paths share these parameters:
 
@@ -34,7 +36,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .configs import load_config, rope_settings, save_config
+from .configs import load_config, rope_scaling, rope_settings, save_config
 
 __all__ = [
     "LlamaRMSNorm",
@@ -51,6 +53,7 @@ __all__ = [
     "apply_rotary_pos_emb",
     "repeat_kv",
     "check_llama_config",
+    "llama3_rope_parameters",
     "num_kv_heads",
 ]
 
@@ -108,13 +111,18 @@ class LlamaRMSNorm(nn.Module):
 
 
 class LlamaRotaryEmbedding(nn.Module):
-    """cos/sin tables in the half-rotation layout; built in fp32, cast with the module."""
+    """cos/sin tables in the half-rotation layout; built in fp32, cast with the module.  ``llama3`` (the dict of
+    :func:`llama3_rope_parameters`) applies Llama-3.1's frequency scaling to ``inv_freq`` before the tables are built."""
 
-    def __init__(self, dim: int, max_position_embeddings: int = 2048, base: float = 10000.0, device=None):
+    def __init__(self, dim: int, max_position_embeddings: int = 2048, base: float = 10000.0, device=None,
+                 llama3: Optional[dict] = None):
         super().__init__()
         self.dim = dim
         self.base = base
+        self.llama3 = llama3
         inv_freq = 1.0 / (base ** (torch.arange(0, dim, 2, dtype=torch.float32, device=device) / dim))
+        if llama3 is not None:
+            inv_freq = llama3_inv_freq(inv_freq, **llama3)
         self.register_buffer("inv_freq", inv_freq)  # persistent: appears in reference checkpoints
         self._build(max_position_embeddings, inv_freq)
 
@@ -133,6 +141,22 @@ class LlamaRotaryEmbedding(nn.Module):
             self.cos_cached[:, :, :seq_len].to(dtype=x.dtype),
             self.sin_cached[:, :, :seq_len].to(dtype=x.dtype),
         )
+
+
+def llama3_inv_freq(inv_freq: torch.Tensor, factor: float, low_freq_factor: float, high_freq_factor: float,
+                    original_max_position_embeddings: float) -> torch.Tensor:
+    """Llama-3.1's rotary frequencies, in fp32: wavelengths longer than ``orig / low_freq_factor`` are stretched by ``factor``,
+    those shorter than ``orig / high_freq_factor`` are kept, and the band between blends the two linearly in ``orig / wavelength``.
+    The expressions follow transformers' ``_compute_llama3_parameters`` term by term, so the fp32 results agree bit for bit."""
+    orig = original_max_position_embeddings
+    low_freq_wavelen = orig / low_freq_factor
+    high_freq_wavelen = orig / high_freq_factor
+    wavelen = 2 * math.pi / inv_freq
+    scaled = torch.where(wavelen > low_freq_wavelen, inv_freq / factor, inv_freq)
+    smooth = (orig / wavelen - low_freq_factor) / (high_freq_factor - low_freq_factor)
+    blended = (1 - smooth) * scaled / factor + smooth * scaled
+    medium = ~(wavelen < high_freq_wavelen) * ~(wavelen > low_freq_wavelen)
+    return torch.where(medium, blended, scaled)
 
 
 def rotate_half(x):
@@ -158,12 +182,32 @@ def num_kv_heads(config) -> int:
     return getattr(config, "num_key_value_heads", None) or config.num_attention_heads
 
 
+_LLAMA3_ROPE_KEYS = ("factor", "low_freq_factor", "high_freq_factor", "original_max_position_embeddings")
+
+
+def llama3_rope_parameters(config) -> Optional[dict]:
+    """None for unscaled rotary embeddings; for ``rope_type`` ``llama3`` (in ``rope_scaling`` or transformers >= 5's
+    ``rope_parameters``) the four settings :func:`llama3_inv_freq` takes.  Every other scaling type, and a llama3 dict
+    missing a setting, is refused with an error that names the field."""
+    scaling = rope_scaling(config)
+    kind = None if scaling is None else scaling.get("type", scaling.get("rope_type"))
+    if kind in (None, "default"):
+        return None
+    if kind != "llama3":
+        raise ValueError(f"rope_scaling={scaling} is not supported (only unscaled rotary embeddings and rope_type 'llama3')")
+    for key in _LLAMA3_ROPE_KEYS:
+        if scaling.get(key) is None:
+            raise ValueError(f"rope_scaling={scaling}: rope_type 'llama3' needs `{key}`")
+    out = {key: float(scaling[key]) for key in _LLAMA3_ROPE_KEYS}
+    if not 0 < out["low_freq_factor"] < out["high_freq_factor"] or out["factor"] <= 0:
+        raise ValueError(f"rope_scaling={scaling}: llama3 needs factor > 0 and 0 < low_freq_factor < high_freq_factor")
+    return out
+
+
 def check_llama_config(config) -> None:
     """Refuse the Llama-family options this model does not implement; the error names the config field."""
     h, nh, nkv = config.hidden_size, config.num_attention_heads, num_kv_heads(config)
-    scaling = rope_settings(config)[2]
-    if scaling is not None and scaling.get("type", scaling.get("rope_type")) not in (None, "default"):
-        raise ValueError(f"rope_scaling={scaling} is not supported (only unscaled rotary embeddings)")
+    llama3_rope_parameters(config)
     if getattr(config, "tie_word_embeddings", False):
         raise ValueError("tie_word_embeddings=True is not supported: lm_head and embed_tokens are separate weights")
     for field in ("attention_bias", "mlp_bias"):
@@ -192,7 +236,7 @@ class LlamaMLP(nn.Module):
 
 
 class LlamaAttention(nn.Module):
-    def __init__(self, config):
+    def __init__(self, config, rotary_emb: Optional[LlamaRotaryEmbedding] = None):
         super().__init__()
         self.hidden_size = config.hidden_size
         self.num_heads = config.num_attention_heads
@@ -206,8 +250,7 @@ class LlamaAttention(nn.Module):
         self.k_proj = nn.Linear(self.hidden_size, kv_size, bias=False)
         self.v_proj = nn.Linear(self.hidden_size, kv_size, bias=False)
         self.o_proj = nn.Linear(self.hidden_size, self.hidden_size, bias=False)
-        self.rotary_emb = LlamaRotaryEmbedding(self.head_dim, max_position_embeddings=self.max_position_embeddings,
-                                               base=float(rope_settings(config)[1]))
+        self.rotary_emb = rotary_emb if rotary_emb is not None else make_rotary_embedding(config)
 
     def forward(self, hidden_states, position_ids=None, past_key_value=None, use_cache=False):
         B, T, _ = hidden_states.shape
@@ -249,11 +292,18 @@ def _use_native_attention(q: torch.Tensor, head_dim: int) -> bool:
     return dispatch.use_fused(q) and fused.attention_backend(head_dim, q=q) == "native"
 
 
+def make_rotary_embedding(config) -> LlamaRotaryEmbedding:
+    """The rotary module of a Llama config: head_dim wide, ``max_position_embeddings`` long, ``rope_theta``, llama3 scaling."""
+    head_dim = config.hidden_size // config.num_attention_heads
+    return LlamaRotaryEmbedding(head_dim, max_position_embeddings=config.max_position_embeddings,
+                                base=float(rope_settings(config)[1]), llama3=llama3_rope_parameters(config))
+
+
 class LlamaDecoderLayer(nn.Module):
-    def __init__(self, config):
+    def __init__(self, config, rotary_emb: Optional[LlamaRotaryEmbedding] = None):
         super().__init__()
         self.hidden_size = config.hidden_size
-        self.self_attn = LlamaAttention(config)
+        self.self_attn = LlamaAttention(config, rotary_emb)
         self.mlp = LlamaMLP(config.hidden_size, config.intermediate_size, getattr(config, "hidden_act", "silu"))
         self.input_layernorm = LlamaRMSNorm(config.hidden_size, eps=config.rms_norm_eps)
         self.post_attention_layernorm = LlamaRMSNorm(config.hidden_size, eps=config.rms_norm_eps)
@@ -359,7 +409,10 @@ class LlamaModel(nn.Module, _PretrainedMixin):
         self.padding_idx = pad
         self.vocab_size = config.vocab_size
         self.embed_tokens = nn.Embedding(config.vocab_size, config.hidden_size, padding_idx=pad)
-        self.layers = nn.ModuleList([LlamaDecoderLayer(config) for _ in range(config.num_hidden_layers)])
+        # one rotary module for every layer: each layer still lists it (its inv_freq stays in the state dict under every
+        # layer's name, as in reference checkpoints) but the cos/sin tables exist once
+        rotary = make_rotary_embedding(config)
+        self.layers = nn.ModuleList([LlamaDecoderLayer(config, rotary) for _ in range(config.num_hidden_layers)])
         self.norm = LlamaRMSNorm(config.hidden_size, eps=config.rms_norm_eps)
         self.gradient_checkpointing = False
 
