@@ -104,6 +104,18 @@ Dropout dropout(const Call& c, const OptTensor& seed, const std::vector<int64_t>
   return d;
 }
 
+// The optional MX copy of a producer's bf16 [rows, cols] output (the fused executor on packed weights): E4M3 bytes [rows, cols]
+// (8-byte stores) and blocked scales, as mx_quantize_rows writes them (cols a multiple of 128).  rmsnorm_fwd and swiglu_fwd take it
+// through their E4M3 output arguments: q8 the bytes, q_inv_scale absent (an MX block carries its own scale), q_amax the scale array.
+rb::MxOut mx_out(uint8_t* q, const OptTensor& qt, uint8_t* sf, int64_t cols) {
+  rb::MxOut m;
+  m.q = q;
+  m.ld = qt.has_value() ? qt->stride(0) : 0;
+  m.sf = sf;
+  m.kg = (int)((cols + 127) / 128);
+  return m;
+}
+
 rb::Fp8Out fp8_out(const Call& c, const OptTensor& q8, const OptTensor& inv_scale, const OptTensor& amax, int64_t rows, int64_t cols) {
   rb::Fp8Out f;
   if (!q8.has_value()) return f;
@@ -160,9 +172,15 @@ void rmsnorm_fwd(const Tensor& x, const Tensor& w, Tensor& y, Tensor& rstd, doub
   const void* wp = arg(c, w, "w", BF, {H}, 16);
   void* yp = arg(c, y, "y", BF, {M * H}, 16);
   float* rp = arg<float>(c, rstd, "rstd", F32, {M});
-  const rb::Fp8Out f8 = fp8_out(c, q8, q_inv_scale, q_amax, M, H);
+  // q8 without q_inv_scale: the MX copy instead of the per-tensor one, its blocked scales in q_amax (see mx_out)
+  const bool mx = q8.has_value() && !q_inv_scale.has_value();
+  TORCH_CHECK(!mx || q_amax.has_value(), "rmsnorm_fwd: the MX output q8 needs its scale array in q_amax");
+  const rb::Fp8Out f8 = mx ? rb::Fp8Out{} : fp8_out(c, q8, q_inv_scale, q_amax, M, H);
+  const rb::MxOut mo = mx ? mx_out(arg<uint8_t>(c, q8, "q8", at::kByte, {M, H}, 8), q8,
+                                   arg<uint8_t>(c, q_amax, "q_amax", at::kByte, {rb::mx_sf_bytes(M, H)}), H)
+                          : rb::MxOut{};
   c10::cuda::CUDAGuard guard(c.dev);
-  rb::rmsnorm_fwd(xp, wp, yp, rp, (int)M, (int)H, (float)eps, xdp, G, dr.seed, dr.keys, dr.thr16, dr.inv_keep, f8, cur_stream());
+  rb::rmsnorm_fwd(xp, wp, yp, rp, (int)M, (int)H, (float)eps, xdp, G, dr.seed, dr.keys, dr.thr16, dr.inv_keep, f8, mo, cur_stream());
 }
 
 void rmsnorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& w, const Tensor& rstd, const OptTensor& dx_add, Tensor& dx, Tensor& dw,
@@ -353,10 +371,16 @@ void swiglu_fwd(const Tensor& gu, Tensor& h, const OptTensor& hd, const OptTenso
   const void* gp = arg(c, gu, "gu", BF, {M, 2 * F}, 16);
   void* hdp = arg(c, hd, "hd", BF, {M, F}, 16);
   const Dropout dr = dropout(c, seed, {key}, p, 1, 1);
-  const rb::Fp8Out f8 = fp8_out(c, q8, q_inv_scale, q_amax, M, F);
+  // q8 without q_inv_scale: the MX copy instead of the per-tensor one, its blocked scales in q_amax (see mx_out)
+  const bool mx = q8.has_value() && !q_inv_scale.has_value();
+  TORCH_CHECK(!mx || q_amax.has_value(), "swiglu_fwd: the MX output q8 needs its scale array in q_amax");
+  const rb::Fp8Out f8 = mx ? rb::Fp8Out{} : fp8_out(c, q8, q_inv_scale, q_amax, M, F);
+  const rb::MxOut mo = mx ? mx_out(arg<uint8_t>(c, q8, "q8", at::kByte, {M, F}, 8), q8,
+                                   arg<uint8_t>(c, q_amax, "q_amax", at::kByte, {rb::mx_sf_bytes(M, F)}), F)
+                          : rb::MxOut{};
   c10::cuda::CUDAGuard guard(c.dev);
   rb::swiglu_fwd(gp, gu.stride(0), hp, h.stride(0), (int)M, (int)F, hdp, hd.has_value() ? hd->stride(0) : 0, dr.seed, dr.keys[0],
-                 dr.thr16, dr.inv_keep, f8, cur_stream());
+                 dr.thr16, dr.inv_keep, f8, mo, cur_stream());
 }
 void swiglu_bwd(const Tensor& dh, const Tensor& gu, Tensor& dgu) {
   const Call c{"swiglu_bwd", dh.device()};
@@ -401,8 +425,10 @@ void mx_dequantize_weight(const Tensor& q, const Tensor& sf_fwd, Tensor& out) {
   c10::cuda::CUDAGuard guard(c.dev);
   rb::mx_dequantize_weight(qp, q.stride(0), fp, op, out.stride(0), (int)N, (int)K, cur_stream());
 }
+// n_per_group / a2_group_kofs: grouped LoRA segment (output columns of group g read a2 columns from g·a2_group_kofs; K2 is then
+// b2's width, as a2 holds every group's columns)
 void gemm_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tensor& sfb, Tensor& out, int64_t M, int64_t N, int64_t K, bool b_mn_major,
-             const OptTensor& a2, const OptTensor& b2, const OptTensor& residual) {
+             const OptTensor& a2, const OptTensor& b2, const OptTensor& residual, int64_t n_per_group, int64_t a2_group_kofs) {
   TORCH_CHECK(!a2.has_value() || b2.has_value(), "gemm_mx: a2 needs b2");
   const Call c{"gemm_mx", out.device()};
   rb::MxGemmDesc d;
@@ -413,8 +439,10 @@ void gemm_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tensor& 
   d.sfb = arg(c, sfb, "sfb", at::kByte, {rb::mx_sf_bytes(N, K)});
   d.out = arg(c, out, "out", BF, {M, N}, 16); d.ldc = out.stride(0);
   d.b_mn_major = b_mn_major; d.M = (int)M; d.N = (int)N; d.K = (int)K;
+  d.n_per_group = (int)n_per_group; d.a2_group_kofs = (int)a2_group_kofs;
   if (a2.has_value()) {
-    d.a2 = arg(c, a2, "a2", BF, {M, 0}, 16); d.lda2 = a2->stride(0); d.K2 = (int)a2->size(1);
+    d.K2 = (int)(n_per_group > 0 ? b2->size(1) : a2->size(1));
+    d.a2 = arg(c, a2, "a2", BF, {M, rb::mx_a2_cols(d)}, 16); d.lda2 = a2->stride(0);
     d.b2 = arg(c, b2, "b2", BF, {N, d.K2}, 16); d.ldb2 = b2->stride(0);
   }
   d.residual = arg(c, residual, "residual", BF, {M, N}, 16); d.ldr = residual.has_value() ? residual->stride(0) : 0;
@@ -767,7 +795,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mx_quantize_weight_2d", &mx_quantize_weight_2d);
   m.def("mx_dequantize_weight", &mx_dequantize_weight);
   m.def("gemm_mx", &gemm_mx, py::arg("a"), py::arg("sfa"), py::arg("b"), py::arg("sfb"), py::arg("out"), py::arg("M"), py::arg("N"), py::arg("K"),
-        py::arg("b_mn_major") = false, py::arg("a2") = py::none(), py::arg("b2") = py::none(), py::arg("residual") = py::none());
+        py::arg("b_mn_major") = false, py::arg("a2") = py::none(), py::arg("b2") = py::none(), py::arg("residual") = py::none(),
+        py::arg("n_per_group") = 0, py::arg("a2_group_kofs") = 0);
   m.def("layernorm_fwd", &layernorm_fwd, py::arg("x"), py::arg("w"), py::arg("b"), py::arg("y"), py::arg("mean"), py::arg("rstd"), py::arg("eps"),
         py::arg("w2") = py::none(), py::arg("b2") = py::none(), py::arg("y2") = py::none(), py::arg("xd") = py::none(), py::arg("xd2") = py::none(),
         py::arg("seed") = py::none(), py::arg("keys") = std::vector<int64_t>{}, py::arg("p") = 0.0);

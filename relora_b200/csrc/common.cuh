@@ -107,6 +107,57 @@ inline int num_sms() {
 }
 inline int ceil_div(long long a, long long b) { return int((a + b - 1) / b); }
 
+// ---------------------------------------------------------------------------------------------- MXFP8 (gemm_mx.cu, producers)
+__device__ __forceinline__ float ue8m0_value(uint8_t e) { return __uint_as_float(e == 0 ? 0x00400000u : uint32_t(e) << 23); }
+__device__ __forceinline__ uint32_t sf_offset(long long row, int sfcol, int kg_per_block) {
+  // byte offset of scale (row, scale column) in the [row block][k group][512] layout
+  const long long rb = row >> 7;
+  const int r = int(row & 127), kg = sfcol >> 2, j = sfcol & 3;
+  return uint32_t(((rb * kg_per_block + kg) << 9) + ((r & 31) << 4) + ((r >> 5) << 2) + j);
+}
+// Scale of a block whose largest magnitude is `amax` (NaN elements ignored): the smallest e with amax <= 448 * 2^e (E4M3 max),
+// clamped to [-127, 127] (an all-zero block gets -127); returns the biased UE8M0 byte e + 127 and 1/2^e.  Exact, from the bits:
+// amax = (1 + F/2^23) * 2^(E-127) <= 1.75 * 2^(E-126) = 448 * 2^(E-135) exactly when F <= 0x600000, else 448 * 2^(E-134) bounds
+// it.  A block holding +-Inf gets the OCP MX NaN scale 0xFF (ue8m0_value decodes it as Inf), so every product it feeds is
+// non-finite; its elements are encoded times 0 (zeros, NaN for the infinities).
+__device__ __forceinline__ uint8_t ue8m0_for(float amax, float& inv_scale) {
+  if (isinf(amax)) {
+    inv_scale = 0.f;
+    return 0xFF;
+  }
+  int e = -127;
+  if (amax > 0.f) {  // false for NaN: a block of NaN only counts as zero
+    const uint32_t bits = __float_as_uint(amax);
+    const int E = int(bits >> 23);
+    e = max(-127, E - 135 + ((bits & 0x7FFFFFu) > 0x600000u ? 1 : 0));  // <= 120 for finite amax
+  }
+  inv_scale = ue8m0_value(uint8_t(127 - e));
+  return (uint8_t)(e + 127);
+}
+
+// The MX copy of 8 consecutive values o at (row, col) of one lane (col a multiple of 8): the lanes lane ^ 1, lane ^ 2 (all in
+// `mask`) hold the rest of the 32-column block.  Same scale and bytes as mx_quantize_rows of the bf16 values o.
+__device__ __forceinline__ void mx_emit8(const MxOut& mo, long long row, int col, const float (&o)[8], unsigned mask) {
+  float amax = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(o[j]));
+  amax = fmaxf(amax, __shfl_xor_sync(mask, amax, 1));
+  amax = fmaxf(amax, __shfl_xor_sync(mask, amax, 2));
+  float inv;
+  const uint8_t e = ue8m0_for(amax, inv);
+  if ((col & 31) == 0) mo.sf[sf_offset(row, col >> 5, mo.kg)] = e;
+  uint32_t w[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(o[4 * h] * inv, o[4 * h + 1] * inv), __NV_SATFINITE, __NV_E4M3);
+    const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(o[4 * h + 2] * inv, o[4 * h + 3] * inv), __NV_SATFINITE, __NV_E4M3);
+    w[h] = (uint32_t)lo | ((uint32_t)hi << 16);
+  }
+  *reinterpret_cast<uint2*>(mo.q + row * mo.ld + col) = make_uint2(w[0], w[1]);
+}
+// the 4 lanes of this lane's 32-column block
+__device__ __forceinline__ unsigned mx_group_mask() { return 0xFu << (threadIdx.x & 28); }
+
 }  // namespace rb
 
 // ---------------------------------------------------------------------------------------------

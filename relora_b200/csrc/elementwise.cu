@@ -13,7 +13,7 @@ template <int VPT>  // bf16x8 vectors per thread
 __global__ void __launch_bounds__(256) rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, bf16* __restrict__ y,
                                                           float* __restrict__ rstd_out, int M, int H, float eps, bf16* __restrict__ xd,
                                                           int G, const uint32_t* __restrict__ seed_ptr, uint4 keys, uint32_t thr16,
-                                                          float inv_keep) {
+                                                          float inv_keep, MxOut mo) {
   __shared__ float scratch[32];
   const int row = blockIdx.x;
   const int nvec = H / 8;
@@ -49,6 +49,7 @@ __global__ void __launch_bounds__(256) rmsnorm_fwd_kernel(const bf16* __restrict
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = bf16_round(wf[j] * bf16_round(v[i][j] * rstd));
       yr[c] = pack8(o);
+      if (mo.q != nullptr) mx_emit8(mo, row, c * 8, o, mx_group_mask());  // H % 128 == 0: whole 4-thread groups are active
       for (int g = 0; g < G; ++g) {
         float d[8];
 #pragma unroll
@@ -60,18 +61,19 @@ __global__ void __launch_bounds__(256) rmsnorm_fwd_kernel(const bf16* __restrict
 }
 
 void rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int M, int H, float eps, void* xd, int G,
-                 const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s) {
+                 const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo, cudaStream_t s) {
   if (H % 8 != 0 || H > 8 * 256 * 4) throw std::runtime_error("rmsnorm: H must be a multiple of 8 and <= 8192");
+  if (mo.q != nullptr && H % 128) throw std::runtime_error("rmsnorm: the MX output needs H to be a multiple of 128");
   uint4 k = make_uint4(0, 0, 0, 0);
   if (G > 0) k = make_uint4(keys[0], G > 1 ? keys[1] : 0, G > 2 ? keys[2] : 0, G > 3 ? keys[3] : 0);
-  if (rmsnorm_fwd_warp(x, w, y, rstd, M, H, eps, xd, G, seed_ptr, k, thr16, inv_keep, f8, s)) return;
+  if (rmsnorm_fwd_warp(x, w, y, rstd, M, H, eps, xd, G, seed_ptr, k, thr16, inv_keep, f8, mo, s)) return;
   if (f8.q != nullptr) throw std::runtime_error("rmsnorm: the fused fp8 output needs the warp-per-row kernel (H <= 2048)");
   const int nvec = H / 8;
   const bf16 *xp = (const bf16*)x, *wp = (const bf16*)w;
   bf16 *yp = (bf16*)y, *xdp = (bf16*)xd;
-  if (nvec <= 256) rmsnorm_fwd_kernel<1><<<M, 256, 0, s>>>(xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, k, thr16, inv_keep);
-  else if (nvec <= 512) rmsnorm_fwd_kernel<2><<<M, 256, 0, s>>>(xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, k, thr16, inv_keep);
-  else rmsnorm_fwd_kernel<4><<<M, 256, 0, s>>>(xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, k, thr16, inv_keep);
+  if (nvec <= 256) rmsnorm_fwd_kernel<1><<<M, 256, 0, s>>>(xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, k, thr16, inv_keep, mo);
+  else if (nvec <= 512) rmsnorm_fwd_kernel<2><<<M, 256, 0, s>>>(xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, k, thr16, inv_keep, mo);
+  else rmsnorm_fwd_kernel<4><<<M, 256, 0, s>>>(xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, k, thr16, inv_keep, mo);
   RB_CHECK_LAUNCH("rmsnorm_fwd");
 }
 
@@ -289,7 +291,7 @@ void rope_inplace(void* buf, long long ld, int M, int T, int n_rot_heads, int hd
 __global__ void __launch_bounds__(256) swiglu_fwd_kernel(const bf16* __restrict__ gu, long long ldgu, bf16* __restrict__ h, long long ldh,
                                                          int M, int F, bf16* __restrict__ hd, long long ldhd,
                                                          const uint32_t* __restrict__ seed_ptr, uint32_t key, uint32_t thr16, float inv_keep,
-                                                         Fp8Out f8) {
+                                                         Fp8Out f8, MxOut mo) {
   pdl_wait();
   pdl_launch_dependents();
   const float q_inv = f8.q != nullptr ? *f8.inv_scale : 0.f;
@@ -319,6 +321,11 @@ __global__ void __launch_bounds__(256) swiglu_fwd_kernel(const bf16* __restrict_
       for (int j = 0; j < 8; ++j) o[j] = __fdividef(g[j], 1.f + __expf(-g[j])) * u[j];  // MUFU.EX2 + MUFU.RCP, no IEEE division sequence
       const bf16x8 packed = pack8(o);
       *reinterpret_cast<bf16x8*>(h + row * ldh + c) = packed;
+      if (mo.q != nullptr) {  // F % 128 == 0 and the stride is a multiple of 4: each 4-thread group holds one 32-column block
+        float ob8[8];
+        unpack8(packed, ob8);
+        mx_emit8(mo, row, c, ob8, mx_group_mask());
+      }
       if (f8.q != nullptr) {
         float ob8[8];
         unpack8(packed, ob8);
@@ -361,11 +368,12 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const bf16* __restrict_
   }
 }
 void swiglu_fwd(const void* gu, long long ldgu, void* h, long long ldh, int M, int F, void* hd, long long ldhd,
-                const uint32_t* seed_ptr, uint32_t key, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s) {
+                const uint32_t* seed_ptr, uint32_t key, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo, cudaStream_t s) {
   if (F % 8) throw std::runtime_error("swiglu: F must be a multiple of 8");
+  if (mo.q != nullptr && F % 128) throw std::runtime_error("swiglu: the MX output needs F to be a multiple of 128");
   const long long total = (long long)M * (F / 8);
   const int grid = (int)std::min<long long>((total + 511) / 512, (long long)num_sms() * 8);
-  launch_k(swiglu_fwd_kernel, grid > 0 ? grid : 1, 256, 0, s, (const bf16*)gu, ldgu, (bf16*)h, ldh, M, F, (bf16*)hd, ldhd, seed_ptr, key, thr16, inv_keep, f8);
+  launch_k(swiglu_fwd_kernel, grid > 0 ? grid : 1, 256, 0, s, (const bf16*)gu, ldgu, (bf16*)h, ldh, M, F, (bf16*)hd, ldhd, seed_ptr, key, thr16, inv_keep, f8, mo);
   RB_CHECK_LAUNCH("swiglu_fwd");
 }
 void swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, void* dgu, long long lddgu, int M, int F,

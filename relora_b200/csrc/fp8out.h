@@ -12,4 +12,13 @@ struct Fp8Out {
   float* amax = nullptr;
 };
 
+// Optional MXFP8 side output of a producer kernel (fused executor on packed weights): the bytes and blocked scales
+// mx_quantize_rows would write for the bf16 result, rows < M only.  kg: 128-column groups per row (K rounded up to 128).
+struct MxOut {
+  uint8_t* q = nullptr;
+  long long ld = 0;
+  uint8_t* sf = nullptr;
+  int kg = 0;
+};
+
 }  // namespace rb

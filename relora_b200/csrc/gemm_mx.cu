@@ -48,11 +48,11 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gsrc, 
                "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ float ue8m0_value(uint8_t e) { return __uint_as_float(e == 0 ? 0x00400000u : uint32_t(e) << 23); }
 __device__ __forceinline__ int sf_byte(int r, int j) { return (r & 31) * 16 + (r >> 5) * 4 + j; }
 
 struct MxArgs {
   int M, N, K8, K2;                 // K8: fp8 reduction length (multiple of 128), K2: bf16 LoRA segment (multiple of 64, may be 0)
+  int n_per_group, a2_group_kofs;   // grouped LoRA segment: the tile at column n reads a2 columns from (n / n_per_group) * a2_group_kofs
   const uint8_t* sfa;               // [m blocks][sfa_kg][512]
   const uint8_t* sfb;               // [n blocks][sfb_kg][512]
   int sfa_kg, sfb_kg;               // 128-element k groups per row block in the arrays
@@ -76,6 +76,68 @@ __device__ __forceinline__ void transpose_fp8_tile(const uint8_t* src, uint8_t* 
       w[e >> 2] |= v << ((e & 3) * 8);
     }
     *reinterpret_cast<uint4*>(dst + n * 128 + ((c ^ (n & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+// D[64 x 64] = A[64 x 32] (e4m3) * B[64 x 32] (e4m3), both K-major; D's old value is ignored (scale-d 0)
+__device__ __forceinline__ void wgmma_e4m3_ss_n64_set(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 0, 0;\n\twgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, "
+      "%27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+        "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+        "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+        "+f"(d[31])
+      : "l"(da), "l"(db));
+}
+
+// acc[half · 32 + i] = fmaf(part[i], s_row(i) · s_col(half), acc[...]): the scale of B is that of its 32 x 32 weight tile, so one
+// read per 32-column block (fragment entries 16j .. 16j + 15 lie in column block j of the 128-wide tile)
+__device__ __forceinline__ void mx_scale_into(float (&acc)[BN / 2], const float (&part)[32], int half, const uint8_t* sfa,
+                                              const uint8_t* sfb, int cw, int kk) {
+  const float s_lo = ue8m0_value(sfa[sf_byte(cw * 64 + frag_row(0), kk)]);
+  const float s_hi = ue8m0_value(sfa[sf_byte(cw * 64 + frag_row(2), kk)]);
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const float sbv = ue8m0_value(sfb[sf_byte(half * 64 + 32 * j, kk)]);
+#pragma unroll
+    for (int i = 16 * j; i < 16 * j + 16; ++i) acc[half * 32 + i] = fmaf(part[i], (((i >> 1) & 1) ? s_hi : s_lo) * sbv, acc[half * 32 + i]);
+  }
+}
+
+// One 128-deep fp8 k-block: 4 scale columns x 2 column halves = 8 K = 32 MMAs of 64 x 64, each scaled into the accumulator while
+// the next one runs (two 32-register partials).  Every accumulator entry still takes its 4 scale columns in order, with the
+// same fmaf, so the result is bit-identical to one wgmma per scale column waited on before its scaling.
+// p0 / p1: the partials, whose values on entry are not read (every MMA here overwrites its partial)
+__device__ __forceinline__ void mx_kblock(float (&acc)[BN / 2], float (&p0)[32], float (&p1)[32], uint32_t sa, uint32_t sb,
+                                          const uint8_t* sfa, int cw) {
+  const uint8_t* sfb = sfa + kSfBytes;
+  // the descriptors encode address / 16 in their low bits: the 32-byte steps along K and the 64-row step of B are additions
+  const uint64_t da = desc_kmajor(sa), db = desc_kmajor(sb);
+  wgmma_fence();
+  wgmma_e4m3_ss_n64_set(p0, da, db);
+  wgmma_commit();
+#pragma unroll
+  for (int s = 0; s < 8; ++s) {  // step s: MMA s + 1 goes out, then MMA s (scale column s / 2, half s % 2) is scaled
+    const int kk = s >> 1, half = s & 1;
+    if (s < 7) {
+      const int kn = (s + 1) >> 1, hn = (s + 1) & 1;
+      wgmma_fence();
+      if (hn) wgmma_e4m3_ss_n64_set(p1, da + (kn * 32 >> 4), db + ((64 * 128 + kn * 32) >> 4));
+      else wgmma_e4m3_ss_n64_set(p0, da + (kn * 32 >> 4), db + (kn * 32 >> 4));
+      wgmma_commit();
+      wgmma_wait<1>();
+    } else {
+      wgmma_wait<0>();
+    }
+    if (half) {
+      fence_regs(p1);
+      mx_scale_into(acc, p1, 1, sfa, sfb, cw, kk);
+    } else {
+      fence_regs(p0);
+      mx_scale_into(acc, p0, 0, sfa, sfb, cw, kk);
+    }
   }
 }
 
@@ -134,8 +196,9 @@ gemm_mx_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         &full_bar[stage]);
         } else {  // bf16 LoRA segment: [x | u]·[W | B]ᵀ shares the accumulator
           const int k = (kb - kb8) * KB16;
+          const int k_a2 = k + (p.n_per_group > 0 ? n0 / p.n_per_group * p.a2_group_kofs : 0);
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_2d(&map_a2, &full_bar[stage], sa, k, m0, kEvictNormal);
+          tma_load_2d(&map_a2, &full_bar[stage], sa, k_a2, m0, kEvictNormal);
           tma_load_2d(&map_b2, &full_bar[stage], sb, k, n0, kEvictLast);
         }
         __syncwarp();
@@ -155,50 +218,41 @@ gemm_mx_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const uint32_t smem0 = smem_u32(smem);
   int stage = 0;
   uint32_t phase = 0;
-  float acc[BN / 2], part[BN / 2];
+  float acc[BN / 2], p0[32], p1[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) p0[i] = p1[i] = 0.f;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int m0 = (tile / p.num_n_tiles) * BM, n0 = (tile % p.num_n_tiles) * BN;
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < kb8 + kb16; ++kb) {
+    for (int kb = 0; kb < kb8; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       const uint32_t sa = smem0 + stage * kStageBytes + cw * 8192;
       uint32_t sb = smem0 + stage * kStageBytes + kTileBytes;
-      if (kb < kb8) {
-        if constexpr (B_MN) {
-          named_bar_sync(1, 256);  // both warpgroups are done with the previous transposed tile
-          transpose_fp8_tile(smem + stage * kStageBytes + kTileBytes, bt, ct);
-          fence_proxy_async_smem();
-          named_bar_sync(1, 256);
-          sb = smem_u32(bt);
-        }
-        const uint8_t* sfa = sf_base + stage * 2 * kSfBytes;
-        const uint8_t* sfb = sfa + kSfBytes;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {  // one K = 32 wgmma per scale column, scaled into the accumulator
-#pragma unroll
-          for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-          wgmma_fence();
-          wgmma_e4m3_ss_n128(part, desc_kmajor(sa + kk * 32), desc_kmajor(sb + kk * 32));
-          wgmma_commit();
-          wgmma_wait<0>();
-          fence_regs(part);
-          const float s_lo = ue8m0_value(sfa[sf_byte(cw * 64 + frag_row(0), kk)]);
-          const float s_hi = ue8m0_value(sfa[sf_byte(cw * 64 + frag_row(2), kk)]);
-#pragma unroll
-          for (int i = 0; i < BN / 2; ++i) {
-            const float sbv = ue8m0_value(sfb[sf_byte(frag_col(i), kk)]);
-            acc[i] = fmaf(part[i], (((i >> 1) & 1) ? s_hi : s_lo) * sbv, acc[i]);
-          }
-        }
-      } else {
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < KB16 / 16; ++k) wgmma_bf16_ss_n128<0, 0>(acc, desc_kmajor(sa + k * 32), desc_kmajor(sb + k * 32));
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(acc);
+      if constexpr (B_MN) {
+        named_bar_sync(1, 256);  // both warpgroups are done with the previous transposed tile
+        transpose_fp8_tile(smem + stage * kStageBytes + kTileBytes, bt, ct);
+        fence_proxy_async_smem();
+        named_bar_sync(1, 256);
+        sb = smem_u32(bt);
       }
+      mx_kblock(acc, p0, p1, sa, sb, sf_base + stage * 2 * kSfBytes, cw);
+      mbar_arrive(&empty_bar[stage]);
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    for (int kb = 0; kb < kb16; ++kb) {  // bf16 LoRA segment: [x | u]·[W | B]ᵀ shares the accumulator
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem0 + stage * kStageBytes + cw * 8192;
+      const uint32_t sb = smem0 + stage * kStageBytes + kTileBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < KB16 / 16; ++k) wgmma_bf16_ss_n128<0, 0>(acc, desc_kmajor(sa + k * 32), desc_kmajor(sb + k * 32));
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(acc);
       mbar_arrive(&empty_bar[stage]);
       if (++stage == kStages) {
         stage = 0;
@@ -222,32 +276,6 @@ gemm_mx_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
 
 // ---------------------------------------------------------------------------------------------- quantisation
-__device__ __forceinline__ uint32_t sf_offset(long long row, int sfcol, int kg_per_block) {
-  // byte offset of scale (row, scale column) in the [row block][k group][512] layout
-  const long long rb = row >> 7;
-  const int r = int(row & 127), kg = sfcol >> 2, j = sfcol & 3;
-  return uint32_t(((rb * kg_per_block + kg) << 9) + ((r & 31) << 4) + ((r >> 5) << 2) + j);
-}
-// Scale of a block whose largest magnitude is `amax` (NaN elements ignored): the smallest e with amax <= 448 * 2^e (E4M3 max),
-// clamped to [-127, 127] (an all-zero block gets -127); returns the biased UE8M0 byte e + 127 and 1/2^e.  Exact, from the bits:
-// amax = (1 + F/2^23) * 2^(E-127) <= 1.75 * 2^(E-126) = 448 * 2^(E-135) exactly when F <= 0x600000, else 448 * 2^(E-134) bounds
-// it.  A block holding +-Inf gets the OCP MX NaN scale 0xFF (ue8m0_value decodes it as Inf), so every product it feeds is
-// non-finite; its elements are encoded times 0 (zeros, NaN for the infinities).
-__device__ __forceinline__ uint8_t ue8m0_for(float amax, float& inv_scale) {
-  if (isinf(amax)) {
-    inv_scale = 0.f;
-    return 0xFF;
-  }
-  int e = -127;
-  if (amax > 0.f) {  // false for NaN: a block of NaN only counts as zero
-    const uint32_t bits = __float_as_uint(amax);
-    const int E = int(bits >> 23);
-    e = max(-127, E - 135 + ((bits & 0x7FFFFFu) > 0x600000u ? 1 : 0));  // <= 120 for finite amax
-  }
-  inv_scale = ue8m0_value(uint8_t(127 - e));
-  return (uint8_t)(e + 127);
-}
-
 // rows: one warp per (row, 4 blocks of 32 columns): lane l holds 4 consecutive elements of column block l / 8
 __global__ void __launch_bounds__(256) mx_quantize_rows_kernel(const bf16* __restrict__ x, long long ldx, uint8_t* __restrict__ q, long long ldq,
                                                                uint8_t* __restrict__ sf, int M, int K, int Kpad, int kg_per_block) {
@@ -381,6 +409,11 @@ __global__ void __launch_bounds__(256) mx_dequantize_weight_kernel(const uint8_t
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------- host
+long long mx_a2_cols(const MxGemmDesc& d) {
+  const int groups = d.n_per_group > 0 ? ceil_div(d.N, d.n_per_group) : 1;
+  return d.K2 + (long long)(groups - 1) * (d.n_per_group > 0 ? d.a2_group_kofs : 0);
+}
+
 long long mx_sf_bytes(long long rows, long long k_elems) { return ((rows + 127) / 128) * ((k_elems + 127) / 128) * 512; }
 
 void mx_quantize_rows(const void* x, long long ldx, void* q, long long ldq, void* sf, int M, int K, cudaStream_t s) {
@@ -421,8 +454,11 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   const int K8 = (d.K + 127) / 128 * 128;
   if (d.K2 % KB16) throw std::runtime_error("gemm_mx: the bf16 segment must be a multiple of 64");
   if (d.N % 8) throw std::runtime_error("gemm_mx: N must be a multiple of 8");
+  // a 128-wide output tile must lie inside one group, so that one A2 column window feeds all of it
+  if (d.n_per_group < 0 || d.n_per_group % BN) throw std::runtime_error("gemm_mx: n_per_group must be a multiple of 128");
   MxArgs p;
   p.M = d.M; p.N = d.N; p.K8 = K8; p.K2 = d.K2;
+  p.n_per_group = d.n_per_group; p.a2_group_kofs = d.n_per_group > 0 ? d.a2_group_kofs : 0;
   p.sfa = reinterpret_cast<const uint8_t*>(d.sfa); p.sfb = reinterpret_cast<const uint8_t*>(d.sfb);
   p.sfa_kg = K8 / 128; p.sfb_kg = K8 / 128;
   p.num_m_tiles = ceil_div(d.M, BM); p.num_n_tiles = ceil_div(d.N, BN);
@@ -433,7 +469,7 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   CUtensorMap mb = d.b_mn_major ? make_map_2d_sw128(d.b, d.N, K8, d.ldb, 128, KB8, 1) : make_map_2d_sw128(d.b, K8, d.N, d.ldb, KB8, BN, 1);
   CUtensorMap ma2 = ma, mb2 = mb;
   if (d.K2 > 0) {
-    ma2 = make_map_2d_sw128(d.a2, d.K2, d.M, d.lda2, KB16, BM, 2);
+    ma2 = make_map_2d_sw128(d.a2, mx_a2_cols(d), d.M, d.lda2, KB16, BM, 2);
     mb2 = make_map_2d_sw128(d.b2, d.K2, d.N, d.ldb2, KB16, BN, 2);
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;

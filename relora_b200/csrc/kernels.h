@@ -11,7 +11,7 @@ namespace rb {
 // y = w * bf16(x * rstd),  rstd = rsqrt(mean(x^2) + eps).  Optionally also writes G dropout-masked copies
 // xd[m, g*H + k] = keep(seed_g, m, k) ? y[m,k] / (1-p) : 0   (inputs of the LoRA down-projections).
 void rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int M, int H, float eps, void* xd, int G,
-                 const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s);
+                 const uint32_t* seed_ptr, const uint32_t* keys, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo, cudaStream_t s);
 // dx = rstd * (g - xhat * mean(g * xhat)) with g = dy * w (+ dx_add);  dw_f32[H] += sum_m dy * bf16(xhat)
 // `ws` (fp32 [rmsnorm_bwd_ws_blocks(), H]) + `ticket` (zeroed uint32) enable the warp-per-row kernel (H <= 2048); without
 // them the block-per-row fallback with global atomics on dw is used.
@@ -19,7 +19,7 @@ void rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd
                  int M, int H, float* ws, unsigned int* ticket, cudaStream_t s);
 int rmsnorm_bwd_ws_blocks();
 bool rmsnorm_fwd_warp(const void* x, const void* w, void* y, float* rstd, int M, int H, float eps, void* xd, int G,
-                      const uint32_t* seed_ptr, uint4 keys, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s);
+                      const uint32_t* seed_ptr, uint4 keys, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo, cudaStream_t s);
 bool rmsnorm_bwd_warp(const void* dy, const void* x, const void* w, const float* rstd, const void* dx_add, void* dx, float* dw, int M,
                       int H, float* ws, unsigned int* ticket, cudaStream_t s);
 
@@ -49,7 +49,7 @@ void rope_pack_bwd(const void* dq, const void* dk, const void* dv, long long sB,
 // gu: [M, 2F] (gate | up) -> h[M, F] = silu(gate) * up
 // optional hd[M, F] = keep(mix(seed, key); row, col) ⊙ h / (1-p): the dropout-expanded copy for the next LoRA down-projection
 void swiglu_fwd(const void* gu, long long ldgu, void* h, long long ldh, int M, int F, void* hd, long long ldhd,
-                const uint32_t* seed_ptr, uint32_t key, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s);
+                const uint32_t* seed_ptr, uint32_t key, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo, cudaStream_t s);
 void swiglu_bwd(const void* dh, long long lddh, const void* gu, long long ldgu, void* dgu, long long lddgu, int M, int F,
                 cudaStream_t s);
 
@@ -124,8 +124,13 @@ struct MxGemmDesc {
   long long ldc = 0;
   const void* residual = nullptr;
   long long ldr = 0;
+  // grouped LoRA segment (as in GemmDesc): output columns [g·n_per_group, (g+1)·n_per_group) read a2 columns
+  // [g·a2_group_kofs, g·a2_group_kofs + K2); n_per_group a multiple of 128, 0 = one group
+  int n_per_group = 0, a2_group_kofs = 0;
 };
 void gemm_mx(const MxGemmDesc& d, cudaStream_t stream);
+// columns of a2 the LoRA segment of `d` reads (K2, plus the group offsets of a grouped segment)
+long long mx_a2_cols(const MxGemmDesc& d);
 
 // ---- embedding -----------------------------------------------------------------------------
 void embedding_fwd(const int64_t* ids, const void* table, void* out, int M, int H, cudaStream_t s);

@@ -15,7 +15,7 @@ constexpr int kWarpsPerBlock = 8;
 template <int VPL>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) rmsnorm_fwd_warp_kernel(
     const bf16* __restrict__ x, const bf16* __restrict__ w, bf16* __restrict__ y, float* __restrict__ rstd_out, int M, int H, float eps,
-    bf16* __restrict__ xd, int G, const uint32_t* __restrict__ seed_ptr, uint4 keys, uint32_t thr16, float inv_keep, Fp8Out f8) {
+    bf16* __restrict__ xd, int G, const uint32_t* __restrict__ seed_ptr, uint4 keys, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo) {
   pdl_wait();
   pdl_launch_dependents();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -58,6 +58,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) rmsnorm_fwd_warp_kernel(
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = bf16_round(wf[j] * bf16_round(f[j] * rstd));
       yr[c] = pack8(o);
+      if (mo.q != nullptr) mx_emit8(mo, row, c * 8, o, mx_group_mask());  // H % 128 == 0: whole 4-lane groups are active
       if (f8.q != nullptr) {
         *reinterpret_cast<uint2*>(f8.q + (long long)row * f8.ld + c * 8) = pack8_e4m3(o, q_inv);
         q_max = fmaxf(q_max, absmax8(o));
@@ -188,13 +189,13 @@ static int pick_vpl(int nvec) {
 }
 
 bool rmsnorm_fwd_warp(const void* x, const void* w, void* y, float* rstd, int M, int H, float eps, void* xd, int G,
-                      const uint32_t* seed_ptr, uint4 keys, uint32_t thr16, float inv_keep, Fp8Out f8, cudaStream_t s) {
+                      const uint32_t* seed_ptr, uint4 keys, uint32_t thr16, float inv_keep, Fp8Out f8, MxOut mo, cudaStream_t s) {
   const int vpl = pick_vpl(H / 8);
   if (vpl == 0) return false;
   const int grid = ceil_div(M, kWarpsPerBlock);
   const bf16 *xp = (const bf16*)x, *wp = (const bf16*)w;
   bf16 *yp = (bf16*)y, *xdp = (bf16*)xd;
-#define L(V) launch_k(rmsnorm_fwd_warp_kernel<V>, grid, kWarpsPerBlock * 32, 0, s, xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, keys, thr16, inv_keep, f8)
+#define L(V) launch_k(rmsnorm_fwd_warp_kernel<V>, grid, kWarpsPerBlock * 32, 0, s, xp, wp, yp, rstd, M, H, eps, xdp, G, seed_ptr, keys, thr16, inv_keep, f8, mo)
   switch (vpl) {
     case 1: L(1); break;
     case 2: L(2); break;

@@ -115,6 +115,7 @@ class FusedStepperBase(Stepper):
         self._attn_saved: List = []  # SDPA: (o, q, k, v) of every layer of the training forward
         self.side = torch.cuda.Stream(device=self.device) if overlap_wgrad else None
         self.fp8 = self.fp8_bwd = False  # E4M3 frozen weights (csrc/fp8.cu): an executor that has them turns them on
+        self.mx = False  # MXFP8-packed frozen stacks (csrc/gemm_mx.cu): likewise
         self.fused_dx = True
         # stacked output width from which the LoRA input gradient uses two kernels (see _lora_group_bwd); 0: the executor's default
         self.dx_split_k = int(os.environ.get("RELORA_B200_DX_SPLIT_K", "0"))
@@ -241,8 +242,11 @@ class FusedStepperBase(Stepper):
         self._loss_and_head_backward(False)
 
     # ------------------------------------------------------------------ LoRA groups
-    def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False, bias=None, Nq=None):
+    def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False, bias=None, Nq=None,
+                        mx_ready=False):
         """u = s·xd_g·A_gᵀ (grouped) ; out = [xn | u]·[W | B]ᵀ (+ bias) (+ residual).
+
+        ``mx_ready`` (packed stacks): the producer of xn already wrote its MX rows into ``self.xq[K]``.
 
         ``Nq``: width of the first group when it differs from the other G-1 groups' ``Ng`` (the q | k | v projections of
         grouped-query attention); its output columns and the rest are then two launches into column windows of ``out``.
@@ -257,6 +261,22 @@ class FusedStepperBase(Stepper):
             g(xn, W, out, M=M, N=W.shape[0], K1=K, residual=residual, bias=bias)
             return
         drop = self.p > 0 and xd.shape[1] == G * K
+        if self.mx:
+            # packed stack W: xn's E4M3 rows and block scales (the bytes the module path's mx.linear quantises), then
+            # out = [xq | u]·[W | B]ᵀ on the block-scaled GEMM, the LoRA segment of group g reading u's columns g·r ..
+            xq, sfx = self.xq[K]
+            if not mx_ready:
+                self.C.mx_quantize_rows(xn, xq, sfx)
+            g(xd, A, u, M=M, N=G * r, K1=K, n_per_group=r, a1_group_kofs=K if drop else 0, alpha=self.scale)
+            if Nq is not None and Nq != Ng:
+                assert residual is None and bias is None and G > 1
+                o = self.C.mx_sf_bytes(Nq, K)
+                self.C.gemm_mx(xq, sfx, W.q[:Nq], W.sf_fwd[:o], out[:, :Nq], M, Nq, K, False, u[:, :r], B[:Nq])
+                self.C.gemm_mx(xq, sfx, W.q[Nq:], W.sf_fwd[o:], out[:, Nq:], M, (G - 1) * Ng, K, False, u[:, r:], B[Nq:], None,
+                               Ng if G > 2 else 0, r)
+                return
+            self.C.gemm_mx(xq, sfx, W.q, W.sf_fwd, out, M, G * Ng, K, False, u, B, residual, Ng if G > 1 else 0, r)
+            return
         if self.fp8 and site is not None:
             l, s_i = site
             x8 = self.x8_h if K == self.h else self.x8_f
@@ -329,7 +349,15 @@ class FusedStepperBase(Stepper):
 
         if self.side is not None:
             self._fork_wgrads(tag, wgrads)
-        if self.fused_dx:
+        if self.mx:
+            # packed stack S_W: base = dy·W on the block-scaled GEMM (W's bytes read MN-major with the stack's input-gradient
+            # scales), then one pass adds the masked low-rank terms
+            sd, ks, pp = (self.seed, list(keys), self.p) if drop else (None, [0] * G, 0.0)
+            dq, sfd = self.xq[width]
+            C.mx_quantize_rows(dy, dq, sfd)
+            C.gemm_mx(dq, sfd, S_W.q, S_W.sf_bwd, base_out, M, K, width, True)
+            C.lora_dx(None, None, du, S_A, out, sd, ks, pp, base_out)
+        elif self.fused_dx:
             sd, ks, pp = (self.seed, list(keys), self.p) if drop else (None, [0] * G, 0.0)
             if width >= self.dx_split_k:
                 # long reductions: the frozen-path product runs on the GEMM, whose TMA-store epilogue overlaps the next
@@ -463,16 +491,20 @@ class FusedStepperBase(Stepper):
         index), B = 0."""
         if self.full:
             raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
-        from ..ops import reference as ref
-
         g, r = fused.gemm, self.r
         for S in self.layers:
             for m, (Bm, Am, Wm) in zip(S.mods, S.merge):
                 g(Bm, Am, Wm, M=Wm.shape[0], N=Wm.shape[1], K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
-                sd = ref.mix_seed(self.model.seed, self.model.n_restarts, m.module_index)
-                self.C.fill_uniform_hash(m.lora_A.weight.data, sd, 1.0 / math.sqrt(m.in_features))
-                m.lora_B.weight.data.zero_()
+                self._reinit_lora(m)
         self.model.n_restarts += 1
+
+    def _reinit_lora(self, m) -> None:
+        """The module path's re-init of one module after its merge: A ~ U(±1/√in) keyed by (seed, restart, module index), B = 0."""
+        from ..ops import reference as ref
+
+        sd = ref.mix_seed(self.model.seed, self.model.n_restarts, m.module_index)
+        self.C.fill_uniform_hash(m.lora_A.weight.data, sd, 1.0 / math.sqrt(m.in_features))
+        m.lora_B.weight.data.zero_()
 
     def launches_in_window(self, n_steps: int) -> int:
         """Kernel launches of this extension since ``reset_launch_count`` (graph replays included)."""

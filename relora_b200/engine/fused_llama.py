@@ -28,15 +28,16 @@ from __future__ import annotations
 
 import math
 import os
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
 from ..models.llama import LlamaForCausalLM, num_kv_heads
-from ..ops import fused, native
+from ..ops import fused, mx, native
+from ..ops.quant import canonical_format
 from ..parallel.dist import DistInfo
 from ..parallel.flat import _ALIGN as _STORE_ALIGN
-from ..relora import ReLoRaLinear
+from ..relora import ReLoRaLinear, ReLoRaModel
 from .fused_common import (FusedStepperBase, LayerViews, device_refusal, full_rank_refusal, native_attention_refusal,
                            relora_refusal)
 
@@ -47,6 +48,37 @@ def supports(model, args=None) -> Tuple[bool, str]:
     why = relora_refusal(model, LlamaForCausalLM, "only Llama is fused")
     if why:
         return False, why
+    return _relora_shapes(model, args)
+
+
+def supports_quantized(model, args=None) -> Tuple[bool, str]:
+    """Whether the executor can train ``model`` with MXFP8-packed frozen weights (``--engine fused --quantize 8bit``), and if
+    not, why.  ``--engine auto`` does not ask: it keeps quantised models on the module path."""
+    if not isinstance(model, ReLoRaModel):
+        return False, "quantized frozen weights need a ReLoRA model; full-rank training has no frozen weights"
+    if not isinstance(model.wrapped_model, LlamaForCausalLM):
+        return False, "quantized frozen weights are fused for Llama only; other models use --engine module"
+    fmt = canonical_format(model._config.quantize)
+    if fmt is None:
+        return False, "the model's frozen weights are not quantized"
+    if fmt != "mxfp8":
+        return False, (f"--quantize {model._config.quantize}: only 8bit (mxfp8) frozen weights run on the fused executor; "
+                       "4bit (nvfp4) uses --engine module")
+    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return False, f"--frozen_dtype {args.frozen_dtype} cannot be combined with --quantize: the frozen weights are already MXFP8"
+    if model.lora_only or model.trainable_scaling:
+        return False, "lora_only / trainable scaling with quantized frozen weights use --engine module"
+    if any(isinstance(m, ReLoRaLinear) and m.bias is not None for m in model.wrapped_model.modules()):
+        return False, "biased projections use the module path"
+    f = model.wrapped_model.config.intermediate_size
+    if f % 8:
+        # the module path keeps such weights in ops/quant.py's 1 x 32-block layout; repacking them into 32 x 32 tiles would round
+        # the frozen weights a second time
+        return False, f"quantized frozen weights need an intermediate size that is a multiple of 8 (got {f}) for the tensor-core layout"
+    return _relora_shapes(model, args)
+
+
+def _relora_shapes(model, args) -> Tuple[bool, str]:
     inner = model.wrapped_model
     cfg = inner.config
     h, f, nh = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads
@@ -118,8 +150,15 @@ class FusedLlamaStepper(FusedStepperBase):
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
                  overlap_wgrad: bool = True, attention: str = "auto", fp8: bool = False, fp8_backward: bool = False,
-                 deterministic: bool = False):
-        super().__init__(model, info, supports, supports_full_rank, grad_accumulation=grad_accumulation,
+                 deterministic: bool = False, quantize: Optional[str] = None):
+        """``quantize="mxfp8"``: the model's frozen weights are MXFP8-packed (``--quantize 8bit``) and stay so; the stacks below
+        are then packed too and the projections run on the block-scaled GEMM (csrc/gemm_mx.cu)."""
+        if quantize is not None and canonical_format(quantize) != "mxfp8":
+            raise RuntimeError(f"quantize={quantize!r}: only mxfp8 frozen weights run on the fused executor")
+        if quantize is not None and (fp8 or fp8_backward):
+            raise RuntimeError("--frozen_dtype fp8 cannot be combined with --quantize: the frozen weights are already MXFP8")
+        super().__init__(model, info, supports_quantized if quantize is not None else supports, supports_full_rank,
+                         grad_accumulation=grad_accumulation,
                          clip_grad_norm=clip_grad_norm, cuda_graphs=cuda_graphs, ce_chunk=ce_chunk, overlap_wgrad=overlap_wgrad,
                          attention=attention, deterministic=deterministic)
         if self.full and fp8:
@@ -139,7 +178,11 @@ class FusedLlamaStepper(FusedStepperBase):
         kv = self.kv
         layers = self.inner.model.layers
         self.Wqkv = self.Wo = self.Wgu = self.Wd = None  # full rank: the trainable weights are stacked views into the flat store
-        if not self.full:
+        self.mx = quantize is not None
+        self.Wmx: List[List[mx.MxWeight]] = []  # per layer: the packed qkv, o, gate|up and down stacks
+        if self.mx:
+            self._pack_stacks(layers)
+        elif not self.full:
             self.Wqkv = torch.empty(L, h + 2 * kv, h, dtype=BF, device=dev)
             self.Wo = torch.empty(L, h, h, dtype=BF, device=dev)
             self.Wgu = torch.zeros(L, 2 * fp, h, dtype=BF, device=dev)
@@ -203,7 +246,10 @@ class FusedLlamaStepper(FusedStepperBase):
                 assert S.Wd.data_ptr() == mlp.down_proj.weight.data_ptr() and S.Wd.shape == (h, fp)
                 self.layers.append(S)
                 continue
-            S.Wqkv, S.Wo, S.Wgu, S.Wd = self.Wqkv[l], self.Wo[l], self.Wgu[l], self.Wd[l]
+            if self.mx:
+                S.Wqkv, S.Wo, S.Wgu, S.Wd = self.Wmx[l]
+            else:
+                S.Wqkv, S.Wo, S.Wgu, S.Wd = self.Wqkv[l], self.Wo[l], self.Wgu[l], self.Wd[l]
             S.A_qkv, S.gA_qkv = pv(at.q_proj.lora_A.weight, 3)
             S.B_qkv, S.gB_qkv = pv(at.q_proj.lora_B.weight, 3) if kv == h else pv(at.q_proj.lora_B.weight, rows=h + 2 * kv)
             S.A_o, S.gA_o = pv(at.o_proj.lora_A.weight)
@@ -222,9 +268,14 @@ class FusedLlamaStepper(FusedStepperBase):
             assert S.B_qkv[h + kv:].data_ptr() == at.v_proj.lora_B.weight.data_ptr() and S.B_qkv.shape == (h + 2 * kv, r)
             assert S.B_gu[fp:].data_ptr() == mlp.up_proj.lora_B.weight.data_ptr()
             assert S.A_d.data_ptr() == mlp.down_proj.lora_A.weight.data_ptr() and S.A_d.shape == (r, fp)
-            # (B, A, W) blocks of the merge GEMM  W += s·B·A  (padded blocks where the module views are strided)
-            S.merge = [(m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data) for m in S.mods[:4]]
-            S.merge += [(S.B_gu[:fp], S.A_gu[:r], S.Wgu[:fp]), (S.B_gu[fp:], S.A_gu[r:], S.Wgu[fp:]), (S.B_d, S.A_d, S.Wd)]
+            if self.mx:  # (B, A, first stack row) of each module of each packed stack: the merge's fp32 delta s·B·A
+                kvB = [S.B_qkv[:h], S.B_qkv[h:h + kv], S.B_qkv[h + kv:]]
+                S.merge = [[(kvB[i], S.A_qkv[i * r:(i + 1) * r], (0, h, h + kv)[i]) for i in range(3)], [(S.B_o, S.A_o, 0)],
+                           [(S.B_gu[:fp], S.A_gu[:r], 0), (S.B_gu[fp:], S.A_gu[r:], fp)], [(S.B_d, S.A_d, 0)]]
+            else:
+                # (B, A, W) blocks of the merge GEMM  W += s·B·A  (padded blocks where the module views are strided)
+                S.merge = [(m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data) for m in S.mods[:4]]
+                S.merge += [(S.B_gu[:fp], S.A_gu[:r], S.Wgu[:fp]), (S.B_gu[fp:], S.A_gu[r:], S.Wgu[fp:]), (S.B_d, S.A_d, S.Wd)]
             self.layers.append(S)
         emb = self.inner.model.embed_tokens
         self.W_emb, self.gW_emb = pv(emb.weight)
@@ -274,6 +325,26 @@ class FusedLlamaStepper(FusedStepperBase):
         dst.copy_(param.data)
         param.data = dst
 
+    # (module, first stack row) of the qkv, o, gate|up and down stacks of a layer
+    def _stack_rows(self, layer):
+        at, mlp, h, kv, fp = layer.self_attn, layer.mlp, self.h, self.kv, self.fp
+        return [[(at.q_proj, 0), (at.k_proj, h), (at.v_proj, h + kv)], [(at.o_proj, 0)], [(mlp.gate_proj, 0), (mlp.up_proj, fp)],
+                [(mlp.down_proj, 0)]]
+
+    @torch.no_grad()
+    def _pack_stacks(self, layers):
+        """The packed stacks of every layer, built from the modules' packed bytes as they are, then each module's ``qweight``
+        re-pointed at its rows of them, so the stacks are the only resident copy of the frozen weights."""
+        for layer in layers:
+            stacks = []
+            for group in self._stack_rows(layer):
+                st = mx.stack_weights([m.qweight for m, _ in group])  # every part starts on a 128-row boundary
+                for m, r0 in group:
+                    m.qweight = mx.stack_part(st, r0, m.out_features)
+                    m.qweight.K = m.in_features  # the down projection of a padded intermediate size: K is the module's own
+                stacks.append(st)
+            self.Wmx.append(stacks)
+
     @torch.no_grad()
     def _quantize_weights(self):
         """(Re)build the E4M3 copies of the frozen weights and their per-tensor scales (at start-up and after every merge)."""
@@ -320,6 +391,11 @@ class FusedLlamaStepper(FusedStepperBase):
             self.u_d = e(L, M, r)
             self.dxn, self.dhmid = e(M, h), e(M, f)
             self.du_bufs = {"d": e(M, r), "gu": e(M, 2 * r), "o": e(M, r), "qkv": e(M, 3 * r)}
+        if self.mx:  # E4M3 rows + block scales of every GEMM input: [M, width] per width
+            widths = {h, f, self.qkv_w, 2 * f}
+            # zeros: the scale bytes of the rows past M that no producer writes are those mx_quantize_rows gives zero rows
+            self.xq = {w: (torch.empty(M, w, dtype=torch.uint8, device=dev),
+                           torch.zeros(self.C.mx_sf_bytes(M, w), dtype=torch.uint8, device=dev)) for w in widths}
         if self.fp8:
             self.x8_h = torch.empty(M, h, dtype=torch.uint8, device=dev)
             self.x8_f = torch.empty(M, f, dtype=torch.uint8, device=dev)
@@ -350,10 +426,18 @@ class FusedLlamaStepper(FusedStepperBase):
         return self._sdpa(q, k, v, train, **gqa).transpose(1, 2).reshape(self.M_, self.h)
 
     def _q8(self, l, s_i, K):
-        """(q8, inv_scale, amax_cur) arguments that make a producer kernel also emit the E4M3 copy of its output."""
+        """(q8, inv_scale, amax_cur) arguments that make a producer kernel also emit the E4M3 copy of its output; on packed
+        stacks, the MX rows of its [M, K] output (see ``_mx``) for the norms and SwiGLU, none for the attention's dropout copy
+        (site 1: the o projection quantises the attention output itself)."""
+        if self.mx:
+            return (self.xq[K][0], None, self.xq[K][1]) if s_i != 1 else (None, None, None)
         if not self.fp8:
             return (None, None, None)
         return (self.x8_h if K == self.h else self.x8_f, self.inv_sx[l, s_i:s_i + 1], self.act_state[l, s_i, 1:2])
+
+    def _mx(self, K):
+        """Keyword arguments that make a producer kernel also emit the MX rows of its [M, K] output (the next GEMM's input)."""
+        return dict(q8=self.xq[K][0], q_amax=self.xq[K][1]) if self.mx else {}  # no q_inv_scale: the MX form
 
     def _forward(self, train: bool):
         C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
@@ -374,10 +458,10 @@ class FusedLlamaStepper(FusedStepperBase):
             else:
                 xn = self.xd_qkv[sl][:, :h] if self.p == 0 else self.xn  # p==0: the normed input is what dA needs
                 xn = xn if xn.is_contiguous() else self.xn
-                C.rmsnorm_fwd(x, S.w1, xn, self.rstd1[sl], self.eps, None, None, [], 0.0)
+                C.rmsnorm_fwd(x, S.w1, xn, self.rstd1[sl], self.eps, None, None, [], 0.0, **self._mx(h))
                 xd = xn
             self._lora_group_fwd(xn, xd, S.A_qkv, S.B_qkv, S.Wqkv, self.u_qkv[sl], qkv, G=3, K=h, Ng=self.kv, site=(l, 0),
-                                 prequant=p > 0, Nq=h)
+                                 prequant=p > 0, Nq=h, mx_ready=True)
             C.rope_inplace(qkv, self.T_, self.nh + self.nkv, self.hd, self.hd, self.cos, self.sin, False, 0)
             attn = self._attention(qkv, train, sl)
             if p > 0:
@@ -395,18 +479,20 @@ class FusedLlamaStepper(FusedStepperBase):
                 xn = self.xn
             else:
                 xn = self.xd_gu[sl] if self.p == 0 else self.xn
-                C.rmsnorm_fwd(x1, S.w2, xn, self.rstd2[sl], self.eps, None, None, [], 0.0)
+                C.rmsnorm_fwd(x1, S.w2, xn, self.rstd2[sl], self.eps, None, None, [], 0.0, **self._mx(h))
                 xd = xn
-            self._lora_group_fwd(xn, xd, S.A_gu, S.B_gu, S.Wgu, self.u_gu[sl], gu, G=2, K=h, Ng=f, site=(l, 2), prequant=p > 0)
+            self._lora_group_fwd(xn, xd, S.A_gu, S.B_gu, S.Wgu, self.u_gu[sl], gu, G=2, K=h, Ng=f, site=(l, 2), prequant=p > 0,
+                                 mx_ready=True)
             if p > 0:
                 xd_d = self.xd_d[sl]
-                C.swiglu_fwd(gu, self.hmid, xd_d, seed, S.key_d, p, *self._q8(l, 3, f))  # activation, dropout copy (and E4M3 copy)
+                C.swiglu_fwd(gu, self.hmid, xd_d, seed, S.key_d, p, *self._q8(l, 3, f))  # activation, dropout copy (and E4M3 / MX copy)
             else:
                 C.swiglu_fwd(gu, self.hmid, None, None, 0, 0.0, *self._q8(l, 3, f))
                 xd_d = self.hmid
                 if train:
                     self.xd_d[sl].copy_(self.hmid)
-            self._lora_group_fwd(self.hmid, xd_d, S.A_d, S.B_d, S.Wd, self.u_d[sl], x_next, G=1, K=f, Ng=h, residual=x1, site=(l, 3), prequant=True)
+            self._lora_group_fwd(self.hmid, xd_d, S.A_d, S.B_d, S.Wd, self.u_d[sl], x_next, G=1, K=f, Ng=h, residual=x1, site=(l, 3), prequant=True,
+                                 mx_ready=True)
         C.rmsnorm_fwd(x_next, self.w_norm, self.xf, self.rstd_f, self.eps, None, None, [], 0.0)
         return x_next
 
@@ -497,7 +583,27 @@ class FusedLlamaStepper(FusedStepperBase):
 
     @torch.no_grad()
     def merge_and_reinit(self):
-        """The merge of every stacked block (see the base class), then the E4M3 copies of the merged weights."""
-        super().merge_and_reinit()
-        if self.fp8:
-            self._quantize_weights()
+        """The merge of every stacked block (see the base class), then the E4M3 copies of the merged weights.  Packed stacks:
+        the fp32 delta s·B·A of each stack on the GEMM, then every 32 x 32 tile requantised in place (``ops/mx.merge_``'s
+        contract) and the modules' input-gradient scales refreshed; the delta scratch is the size of the largest stack and is
+        released afterwards."""
+        if not self.mx:
+            super().merge_and_reinit()
+            if self.fp8:
+                self._quantize_weights()
+            return
+        g, r = fused.gemm, self.r
+        delta = torch.empty(max(st.N * st.K for st in self.Wmx[0]), dtype=torch.float32, device=self.device)
+        for l, S in enumerate(self.layers):
+            for st, blocks in zip(self.Wmx[l], S.merge):
+                d = delta[:st.N * st.K].view(st.N, st.K).zero_()
+                for Bm, Am, r0 in blocks:
+                    g(Bm, Am, d[r0:r0 + Bm.shape[0]], M=Bm.shape[0], N=st.K, K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
+                self.C.mx_quantize_weight_2d(None, d, st.q, st.sf_fwd, st.sf_bwd, st.N, st.K)
+            for group, st in zip(self._stack_rows(self.inner.model.layers[l]), self.Wmx[l]):
+                for m, r0 in group:
+                    mx.refresh_part(st, m.qweight, r0)
+            for m in S.mods:
+                self._reinit_lora(m)
+        del delta
+        self.model.n_restarts += 1

@@ -171,7 +171,15 @@ def make_stepper(model, info: DistInfo, args, *, native=None, dropout_seed: Opti
         frozen = getattr(args, "frozen_dtype", None)
         ok, why = fused_llama.supports(model, args)
         cls = fused_llama.FusedLlamaStepper if ok else None
-        if cls is None and engine == "fused":
+        quantized = isinstance(model, ReLoRaModel) and model._config.quantize is not None
+        if cls is None and engine == "fused" and quantized:
+            # MXFP8-packed frozen weights run fused only on request; `auto` keeps quantised models on the module path
+            ok, why_q = fused_llama.supports_quantized(model, args)
+            if not ok:
+                raise RuntimeError(f"--engine fused requested but not applicable: {why_q}")
+            cls = fused_llama.FusedLlamaStepper
+            kw["quantize"] = "mxfp8"
+        elif cls is None and engine == "fused":
             # Pythia (GPT-NeoX) and full-rank Llama run fused only on request; `auto` keeps both on the module path
             inner = getattr(model, "wrapped_model", model)
             if isinstance(model, LlamaForCausalLM):
@@ -186,7 +194,7 @@ def make_stepper(model, info: DistInfo, args, *, native=None, dropout_seed: Opti
                 keep_llama_why = check is fused_pythia.supports and not isinstance(inner, GPTNeoXForCausalLM)
                 raise RuntimeError(f"--engine fused requested but not applicable: {why if keep_llama_why else why_fused}")
         if cls is not None:
-            if cls is fused_llama.FusedLlamaStepper:
+            if cls is fused_llama.FusedLlamaStepper and "quantize" not in kw:
                 kw.update(fp8=frozen in ("fp8", "fp8_full"), fp8_backward=frozen == "fp8_full")
             return cls(model, info, cuda_graphs=getattr(args, "cuda_graphs", True), attention=getattr(args, "attention", "auto"),
                        deterministic=bool(getattr(args, "deterministic", False)), **kw)

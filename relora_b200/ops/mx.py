@@ -21,7 +21,7 @@ import torch
 from . import native, reference
 
 __all__ = ["MxWeight", "quantize_weight", "dequantize_weight", "quantize_rows", "linear", "merge_", "supported",
-           "ref_quantize_rows", "ref_quantize_weight_2d"]
+           "sf_blocks", "stack_weights", "stack_part", "refresh_part", "ref_quantize_rows", "ref_quantize_weight_2d"]
 
 _BF16 = torch.bfloat16
 
@@ -71,6 +71,45 @@ def dequantize_weight(mw: MxWeight, dtype=_BF16) -> torch.Tensor:
     out = torch.empty(mw.N, mw.K, dtype=_BF16, device=mw.q.device)
     native.require().mx_dequantize_weight(mw.q, mw.sf_fwd, out)
     return out if dtype == _BF16 else out.to(dtype)
+
+
+# ----------------------------------------------------------------------------- stacked weights (the fused executor)
+# A stack is the row concatenation of packed weights that share K, each part starting on a 128-row boundary (its Npad rows).
+# Its q and forward scale array are the parts' bytes one after another, so a part is a slice of them.  The input-gradient scale
+# array is not: its 512-byte blocks are ordered [128-row block of K][128-group of N], so a part's blocks are a strided window of
+# the stack's, and a part keeps a copy of its own.
+def sf_blocks(sf: torch.Tensor, rows: int, k: int) -> torch.Tensor:
+    """The scale array of a ``[rows, k]`` operand as its ``[pad128(rows)/128, pad128(k)/128, 512]`` blocks."""
+    return sf.view(_pad128(rows) // 128, _pad128(k) // 128, 512)
+
+
+def stack_weights(parts) -> MxWeight:
+    """The stack of packed weights ``parts`` (one K): byte for byte what quantising the stacked matrix gives, since every
+    32 x 32 tile lies inside one part."""
+    K = parts[0].K
+    assert all(p.K == K for p in parts)
+    q = torch.cat([p.q for p in parts])
+    N = q.shape[0]
+    sf_fwd = torch.cat([p.sf_fwd for p in parts])
+    sf_bwd = torch.cat([sf_blocks(p.sf_bwd, K, p.N) for p in parts], dim=1).reshape(-1)
+    return MxWeight(q, sf_fwd, sf_bwd, N, K)
+
+
+def stack_part(stack: MxWeight, r0: int, N: int) -> MxWeight:
+    """The packed weight of rows ``[r0, r0 + N)`` of ``stack`` (``r0`` a multiple of 128): q and the forward scales alias the
+    stack, the input-gradient scales are a copy (:func:`refresh_part`)."""
+    kg = _pad128(stack.K) // 128
+    o = r0 // 128 * kg * 512
+    part = MxWeight(stack.q[r0:r0 + _pad128(N)], stack.sf_fwd[o:o + _pad128(N) // 128 * kg * 512],
+                    torch.empty(reference.mx_sf_bytes(stack.K, N), dtype=torch.uint8, device=stack.q.device), N, stack.K)
+    refresh_part(stack, part, r0)
+    return part
+
+
+def refresh_part(stack: MxWeight, part: MxWeight, r0: int) -> None:
+    """Copy the input-gradient scales of ``part`` (rows ``[r0, ...)`` of ``stack``) out of the stack's."""
+    g0 = r0 // 128
+    sf_blocks(part.sf_bwd, part.K, part.N).copy_(sf_blocks(stack.sf_bwd, stack.K, stack.N)[:, g0:g0 + _pad128(part.N) // 128])
 
 
 @torch.no_grad()

@@ -1170,21 +1170,33 @@ def mx_quantize_weight_2d_exact(w: Optional[torch.Tensor] = None, q_old: Optiona
 
 def gemm_mx_ref(a: torch.Tensor, sfa: torch.Tensor, b: torch.Tensor, sfb: torch.Tensor, M: int, N: int, K: int,
                 b_mn_major: bool = False, a2: Optional[torch.Tensor] = None, b2: Optional[torch.Tensor] = None,
-                residual: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """fp64 ``(ref, bound)`` of ``gemm_mx(a, sfa, b, sfb, out, M, N, K, b_mn_major, a2, b2, residual)``:
+                residual: Optional[torch.Tensor] = None, n_per_group: int = 0,
+                a2_group_kofs: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp64 ``(ref, bound)`` of ``gemm_mx(a, sfa, b, sfb, out, M, N, K, b_mn_major, a2, b2, residual, n_per_group, a2_group_kofs)``:
 
-        out[m, n] = Σ_{k < Kpad} A[m, k]·B[n, k]  +  Σ_j a2[m, j]·b2[n, j]  +  residual[m, n]
+        out[m, n] = Σ_{k < Kpad} A[m, k]·B[n, k]  +  Σ_{j < K2} a2[m, o(n) + j]·b2[n, j]  +  residual[m, n]
+
+    with K2 the width of ``b2`` and o(n) = (n // n_per_group)·a2_group_kofs for a grouped LoRA segment (``n_per_group`` > 0),
+    else 0 and K2 the width of ``a2``.
 
     A the decoded ``a [M, Kpad]`` with scales ``sfa`` (rows M); B the decoded ``b [N, Kpad]`` (K-major) or ``b[:Kpad, :N]ᵀ``
     (``b_mn_major``, the weight read for the input gradient), with scales ``sfb`` for rows N, reduction K.  The reduction runs
-    over the padded Kpad = K rounded up to 128 (the quantisers write zeros there).  ``bound`` is Σ|terms| for
+    over the padded Kpad = K rounded up to 128 (the quantisers write zeros there).  B is a packed weight: its scales are those
+    of its 32 x 32 tiles, the same for each 32 rows, and the kernel reads one per 32-row block.  ``bound`` is Σ|terms| for
     :func:`assert_gemm_close` with ``fp8=True``.  An Inf scale or a NaN element makes the outputs it feeds non-finite."""
     Kp = _pad128(K)
     A = mx_decode(a, sfa, M, K)
     bb = b[:Kp, :N].t() if b_mn_major else b[:N, :Kp]
     B = mx_decode(bb, sfb, N, K)
     ref, bound = A @ B.t(), A.abs() @ B.abs().t()
-    if a2 is not None:
+    if a2 is not None and n_per_group > 0:
+        k2 = b2.shape[1]
+        for n0 in range(0, N, n_per_group):
+            n1, o = min(N, n0 + n_per_group), n0 // n_per_group * a2_group_kofs
+            x, y = a2[:M, o:o + k2].to(_F64), b2[n0:n1].to(_F64)
+            ref[:, n0:n1] += x @ y.t()
+            bound[:, n0:n1] += x.abs() @ y.abs().t()
+    elif a2 is not None:
         x, y = a2[:M].to(_F64), b2[:N].to(_F64)
         ref, bound = ref + x @ y.t(), bound + x.abs() @ y.abs().t()
     if residual is not None:
