@@ -427,8 +427,10 @@ void mx_dequantize_weight(const Tensor& q, const Tensor& sf_fwd, Tensor& out) {
 }
 // n_per_group / a2_group_kofs: grouped LoRA segment (output columns of group g read a2 columns from g·a2_group_kofs; K2 is then
 // b2's width, as a2 holds every group's columns)
+// bias: bf16 [N], added in fp32 before the residual (K-major B only)
 void gemm_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tensor& sfb, Tensor& out, int64_t M, int64_t N, int64_t K, bool b_mn_major,
-             const OptTensor& a2, const OptTensor& b2, const OptTensor& residual, int64_t n_per_group, int64_t a2_group_kofs) {
+             const OptTensor& a2, const OptTensor& b2, const OptTensor& residual, int64_t n_per_group, int64_t a2_group_kofs,
+             const OptTensor& bias) {
   TORCH_CHECK(!a2.has_value() || b2.has_value(), "gemm_mx: a2 needs b2");
   const Call c{"gemm_mx", out.device()};
   rb::MxGemmDesc d;
@@ -446,6 +448,7 @@ void gemm_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Tensor& 
     d.b2 = arg(c, b2, "b2", BF, {N, d.K2}, 16); d.ldb2 = b2->stride(0);
   }
   d.residual = arg(c, residual, "residual", BF, {M, N}, 16); d.ldr = residual.has_value() ? residual->stride(0) : 0;
+  d.bias = arg(c, bias, "bias", BF, {N}, 4);  // pairs of columns
   c10::cuda::CUDAGuard guard(c.dev);
   rb::gemm_mx(d, cur_stream());
 }
@@ -796,7 +799,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mx_dequantize_weight", &mx_dequantize_weight);
   m.def("gemm_mx", &gemm_mx, py::arg("a"), py::arg("sfa"), py::arg("b"), py::arg("sfb"), py::arg("out"), py::arg("M"), py::arg("N"), py::arg("K"),
         py::arg("b_mn_major") = false, py::arg("a2") = py::none(), py::arg("b2") = py::none(), py::arg("residual") = py::none(),
-        py::arg("n_per_group") = 0, py::arg("a2_group_kofs") = 0);
+        py::arg("n_per_group") = 0, py::arg("a2_group_kofs") = 0, py::arg("bias") = py::none());
   m.def("layernorm_fwd", &layernorm_fwd, py::arg("x"), py::arg("w"), py::arg("b"), py::arg("y"), py::arg("mean"), py::arg("rstd"), py::arg("eps"),
         py::arg("w2") = py::none(), py::arg("b2") = py::none(), py::arg("y2") = py::none(), py::arg("xd") = py::none(), py::arg("xd2") = py::none(),
         py::arg("seed") = py::none(), py::arg("keys") = std::vector<int64_t>{}, py::arg("p") = 0.0);

@@ -61,6 +61,7 @@ struct MxArgs {
   long long ldc;
   const bf16* residual;
   long long ldr;
+  const bf16* bias;                 // [N] or nullptr, added in fp32 before the residual (the order of the bf16 GEMM's epilogue)
 };
 
 // 256 consumer threads: MN-major [128 K rows][128 N bytes] (128-byte swizzle) -> K-major [128 N rows][128 K bytes] (same swizzle)
@@ -141,7 +142,8 @@ __device__ __forceinline__ void mx_kblock(float (&acc)[BN / 2], float (&p0)[32],
   }
 }
 
-template <bool B_MN>
+// BIAS: a kernel of its own, so that the calls without a bias run the epilogue they had before it existed
+template <bool B_MN, bool BIAS>
 __global__ void __launch_bounds__(384, 1)
 gemm_mx_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_a2,
                const __grid_constant__ CUtensorMap map_b2, const MxArgs p) {
@@ -259,11 +261,25 @@ gemm_mx_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         phase ^= 1;
       }
     }
+    // the bias of this thread's 16 column pairs (entries 4j and 4j + 2 share one), all loaded before the first is needed
+    uint32_t bias2[BN / 8];
+    if constexpr (BIAS) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + frag_col(4 * j);
+        bias2[j] = col < p.N ? __ldg(reinterpret_cast<const unsigned int*>(p.bias + col)) : 0u;
+      }
+    }
 #pragma unroll
     for (int i = 0; i < BN / 2; i += 2) {
       const int row = m0 + cw * 64 + frag_row(i), col = n0 + frag_col(i);
       if (row >= p.M || col >= p.N) continue;  // N is a multiple of 8: column pairs are whole
       float v0 = acc[i], v1 = acc[i + 1];
+      if constexpr (BIAS) {  // in fp32 before the residual, the order of the bf16 GEMM's epilogue
+        const float2 b = unpack_bf16x2(bias2[i >> 2]);
+        v0 += b.x;
+        v1 += b.y;
+      }
       if (p.residual != nullptr) {
         const float2 r = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.residual + (long long)row * p.ldr + col));
         v0 += r.x;
@@ -456,6 +472,7 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   if (d.N % 8) throw std::runtime_error("gemm_mx: N must be a multiple of 8");
   // a 128-wide output tile must lie inside one group, so that one A2 column window feeds all of it
   if (d.n_per_group < 0 || d.n_per_group % BN) throw std::runtime_error("gemm_mx: n_per_group must be a multiple of 128");
+  if (d.bias != nullptr && d.b_mn_major) throw std::runtime_error("gemm_mx: a bias needs K-major B (the input-gradient form has none)");
   MxArgs p;
   p.M = d.M; p.N = d.N; p.K8 = K8; p.K2 = d.K2;
   p.n_per_group = d.n_per_group; p.a2_group_kofs = d.n_per_group > 0 ? d.a2_group_kofs : 0;
@@ -464,6 +481,7 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   p.num_m_tiles = ceil_div(d.M, BM); p.num_n_tiles = ceil_div(d.N, BN);
   p.out = reinterpret_cast<bf16*>(d.out); p.ldc = d.ldc;
   p.residual = reinterpret_cast<const bf16*>(d.residual); p.ldr = d.ldr;
+  p.bias = reinterpret_cast<const bf16*>(d.bias);
   // operands: fp8 bytes; A [M, K8] K-major (pitch lda); B K-major [N, K8] (pitch ldb) or MN-major [K8 rows, N] (pitch ldb)
   CUtensorMap ma = make_map_2d_sw128(d.a, K8, d.M, d.lda, KB8, BM, 1);
   CUtensorMap mb = d.b_mn_major ? make_map_2d_sw128(d.b, d.N, K8, d.ldb, 128, KB8, 1) : make_map_2d_sw128(d.b, K8, d.N, d.ldb, KB8, BN, 1);
@@ -476,12 +494,16 @@ void gemm_mx(const MxGemmDesc& d, cudaStream_t stream) {
   const int grid = tiles < num_sms() ? tiles : num_sms();
   if (d.b_mn_major) {
     static bool cfg = false;
-    if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
-    launch_k(gemm_mx_kernel<true>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
+    if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
+    launch_k(gemm_mx_kernel<true, false>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
+  } else if (d.bias != nullptr) {
+    static bool cfg = false;
+    if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
+    launch_k(gemm_mx_kernel<false, true>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
   } else {
     static bool cfg = false;
-    if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
-    launch_k(gemm_mx_kernel<false>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
+    if (!cfg) { check(cudaFuncSetAttribute(gemm_mx_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal), "attr(gemm_mx)"); cfg = true; }
+    launch_k(gemm_mx_kernel<false, false>, grid, 384, kSmemTotal, stream, ma, mb, ma2, mb2, p);
   }
   RB_CHECK_LAUNCH("gemm_mx");
 }

@@ -111,7 +111,7 @@ void mx_quantize_rows(const void* x, long long ldx, void* q, long long ldq, void
 void mx_quantize_weight_2d(const void* w, long long ldw, const void* q_old, const void* sf_old, const float* delta, long long ldd, void* q,
                            long long ldq, void* sf_fwd, void* sf_bwd, int N, int K, cudaStream_t s);
 void mx_dequantize_weight(const void* q, long long ldq, const void* sf_fwd, void* out, long long ldo, int N, int K, cudaStream_t s);
-// out[M,N] (bf16) = A8[M,K]·B8ᵀ (block-scaled E4M3, kind::mxf8f6f4) + A2[M,K2]·B2[N,K2]ᵀ (bf16, same accumulator) (+ residual)
+// out[M,N] (bf16) = A8[M,K]·B8ᵀ (block-scaled E4M3, kind::mxf8f6f4) + A2[M,K2]·B2[N,K2]ᵀ (bf16, same accumulator) (+ bias) (+ residual)
 struct MxGemmDesc {
   const void *a = nullptr, *b = nullptr;   // fp8 bytes; a [M, Kpad] K-major; b [N, Kpad] K-major, or (b_mn_major) [Kpad rows, N] as stored
   long long lda = 0, ldb = 0;
@@ -127,6 +127,8 @@ struct MxGemmDesc {
   // grouped LoRA segment (as in GemmDesc): output columns [g·n_per_group, (g+1)·n_per_group) read a2 columns
   // [g·a2_group_kofs, g·a2_group_kofs + K2); n_per_group a multiple of 128, 0 = one group
   int n_per_group = 0, a2_group_kofs = 0;
+  // bf16 [N] (optional, K-major B only): added to the accumulator in fp32 before the residual, as in the bf16 GEMM's epilogue
+  const void* bias = nullptr;
 };
 void gemm_mx(const MxGemmDesc& d, cudaStream_t stream);
 // columns of a2 the LoRA segment of `d` reads (K2, plus the group offsets of a grouped segment)

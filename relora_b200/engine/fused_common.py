@@ -10,7 +10,7 @@ provides the rest:
   fp32-gradient parameter store with stacked views; the gradient transport, ``update()`` and the optimizer are those of every
   stepper (:class:`.stepper.Stepper`, ``parallel.grad_sync``);
 * the buffers both executors share, the per-layer slot selection, the SDPA fallback attention and the embedding backward;
-* ``merge_and_reinit()``;
+* ``merge_and_reinit()``, on bf16 weights and on MXFP8-packed ones;
 * one CUDA graph per micro-batch shape, capture / replay and launch counting;
 * the LoRA group forward / backward on the wgmma GEMM and the fused input-gradient kernel, and the chunked LM head + CE.
 """
@@ -275,7 +275,8 @@ class FusedStepperBase(Stepper):
                 self.C.gemm_mx(xq, sfx, W.q[Nq:], W.sf_fwd[o:], out[:, Nq:], M, (G - 1) * Ng, K, False, u[:, r:], B[Nq:], None,
                                Ng if G > 2 else 0, r)
                 return
-            self.C.gemm_mx(xq, sfx, W.q, W.sf_fwd, out, M, G * Ng, K, False, u, B, residual, Ng if G > 1 else 0, r)
+            self.C.gemm_mx(xq, sfx, W.q, W.sf_fwd, out, M, G * Ng, K, False, u, B, residual, Ng if G > 1 else 0, r,
+                           *(() if bias is None else (bias,)))
             return
         if self.fp8 and site is not None:
             l, s_i = site
@@ -488,15 +489,41 @@ class FusedStepperBase(Stepper):
     def merge_and_reinit(self):
         """W += s·B@A for every module of every layer and its (B, A, W) block (``mods`` / ``merge`` of the layer views; wgmma GEMM
         accumulating into W in fp32), then the hash re-init of the module path: A ~ U(±1/√in) keyed by (seed, restart, module
-        index), B = 0."""
+        index), B = 0.  Packed weights: see ``_merge_packed``."""
         if self.full:
             raise RuntimeError("merge_and_reinit needs a ReLoRA model; full-rank training has no low-rank factors")
+        if self.mx:
+            self._merge_packed()
+            return
         g, r = fused.gemm, self.r
         for S in self.layers:
             for m, (Bm, Am, Wm) in zip(S.mods, S.merge):
                 g(Bm, Am, Wm, M=Wm.shape[0], N=Wm.shape[1], K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
                 self._reinit_lora(m)
         self.model.n_restarts += 1
+
+    @torch.no_grad()
+    def _merge_packed(self) -> None:
+        """The merge on MXFP8-packed weights: for each packed weight ``self.Wmx[l][i]`` of a layer, the fp32 delta s·B·A of its
+        blocks ``S.merge[i]`` ((B, A, first row) each) on the GEMM, then every 32 x 32 tile requantised in place (``ops/mx.merge_``'s
+        contract); then ``_packed_merged(l)`` and the re-init of the layer's modules.  The delta scratch is the size of the
+        largest packed weight of a layer and is released afterwards."""
+        g, r = fused.gemm, self.r
+        delta = torch.empty(max(st.N * st.K for st in self.Wmx[0]), dtype=torch.float32, device=self.device)
+        for l, S in enumerate(self.layers):
+            for st, blocks in zip(self.Wmx[l], S.merge):
+                d = delta[:st.N * st.K].view(st.N, st.K).zero_()
+                for Bm, Am, r0 in blocks:
+                    g(Bm, Am, d[r0:r0 + Bm.shape[0]], M=Bm.shape[0], N=st.K, K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
+                self.C.mx_quantize_weight_2d(None, d, st.q, st.sf_fwd, st.sf_bwd, st.N, st.K)
+            self._packed_merged(l)
+            for m in S.mods:
+                self._reinit_lora(m)
+        del delta
+        self.model.n_restarts += 1
+
+    def _packed_merged(self, l: int) -> None:
+        """Runs after layer ``l``'s packed weights were requantised (an executor whose modules keep copies of them refreshes those)."""
 
     def _reinit_lora(self, m) -> None:
         """The module path's re-init of one module after its merge: A ~ U(±1/√in) keyed by (seed, restart, module index), B = 0."""

@@ -583,27 +583,13 @@ class FusedLlamaStepper(FusedStepperBase):
 
     @torch.no_grad()
     def merge_and_reinit(self):
-        """The merge of every stacked block (see the base class), then the E4M3 copies of the merged weights.  Packed stacks:
-        the fp32 delta s·B·A of each stack on the GEMM, then every 32 x 32 tile requantised in place (``ops/mx.merge_``'s
-        contract) and the modules' input-gradient scales refreshed; the delta scratch is the size of the largest stack and is
-        released afterwards."""
-        if not self.mx:
-            super().merge_and_reinit()
-            if self.fp8:
-                self._quantize_weights()
-            return
-        g, r = fused.gemm, self.r
-        delta = torch.empty(max(st.N * st.K for st in self.Wmx[0]), dtype=torch.float32, device=self.device)
-        for l, S in enumerate(self.layers):
-            for st, blocks in zip(self.Wmx[l], S.merge):
-                d = delta[:st.N * st.K].view(st.N, st.K).zero_()
-                for Bm, Am, r0 in blocks:
-                    g(Bm, Am, d[r0:r0 + Bm.shape[0]], M=Bm.shape[0], N=st.K, K1=r, b1_mn=True, alpha=self.scale, accumulate=True)
-                self.C.mx_quantize_weight_2d(None, d, st.q, st.sf_fwd, st.sf_bwd, st.N, st.K)
-            for group, st in zip(self._stack_rows(self.inner.model.layers[l]), self.Wmx[l]):
-                for m, r0 in group:
-                    mx.refresh_part(st, m.qweight, r0)
-            for m in S.mods:
-                self._reinit_lora(m)
-        del delta
-        self.model.n_restarts += 1
+        """The merge of every stacked block (see the base class), then the E4M3 copies of the merged weights.  Packed stacks
+        (``_merge_packed``): afterwards the modules' input-gradient scales are refreshed from their stacks'."""
+        super().merge_and_reinit()
+        if self.fp8:
+            self._quantize_weights()
+
+    def _packed_merged(self, l: int) -> None:
+        for group, st in zip(self._stack_rows(self.inner.model.layers[l]), self.Wmx[l]):
+            for m, r0 in group:
+                mx.refresh_part(st, m.qweight, r0)

@@ -22,6 +22,12 @@ residual) epilogue, the input gradient is ``dy·W``, and the fp32 weight gradien
 ``dA`` / ``dB`` run under ReLoRA.  ``x`` is what the executor already saves with p = 0: the norm outputs, the attention output and
 the GELU output.
 
+MXFP8-packed frozen weights (``--quantize 8bit``, ``quantize="mxfp8"``): each projection's frozen operand is the module's own packed
+weight (``qweight``, an ``ops/mx.MxWeight``; ``query_key_value`` is already one module, so nothing is stacked), the only resident
+copy.  Every projection quantises its input to MX rows (``mx_quantize_rows``) and runs ``[xq | u]·[W | B]ᵀ + b (+ residual)`` on
+the block-scaled GEMM with the bias in its epilogue.  The backward quantises each output gradient and reads the packed bytes
+MN-major; the merge requantises each module's bytes in place.
+
 Parallel residual:   x_next = x + dense(attn(LN1 x)) + b_o + mlp(LN2 x) + b_4
 Sequential residual: x1 = x + dense(attn(LN1 x)) + b_o ;  x_next = x1 + mlp(LN2 x1) + b_4
 """
@@ -34,7 +40,10 @@ import torch
 import torch.nn as nn
 
 from ..models.pythia import GPTNeoXForCausalLM
+from ..ops import mx
+from ..ops.quant import canonical_format
 from ..parallel.dist import DistInfo
+from ..relora import ReLoRaModel
 from .fused_common import (FusedStepperBase, LayerViews, device_refusal, full_rank_refusal, native_attention_refusal,
                            relora_refusal)
 
@@ -78,6 +87,27 @@ def supports(model, args=None) -> Tuple[bool, str]:
     return (False, why) if why else (True, "ok")
 
 
+def supports_quantized(model, args=None) -> Tuple[bool, str]:
+    """Whether the executor can train ``model`` with MXFP8-packed frozen weights (``--engine fused --quantize 8bit``), and if
+    not, why.  ``--engine auto`` does not ask: it keeps quantised models on the module path."""
+    if not isinstance(model, ReLoRaModel):
+        return False, "quantized frozen weights need a ReLoRA model; full-rank training has no frozen weights"
+    if not isinstance(model.wrapped_model, GPTNeoXForCausalLM):
+        return False, "not a GPT-NeoX (Pythia) model"
+    fmt = canonical_format(model._config.quantize)
+    if fmt is None:
+        return False, "the model's frozen weights are not quantized"
+    if fmt != "mxfp8":
+        return False, (f"--quantize {model._config.quantize}: only 8bit (mxfp8) frozen weights run on the fused executor; "
+                       "4bit (nvfp4) uses --engine module")
+    if getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return False, f"--frozen_dtype {args.frozen_dtype} cannot be combined with --quantize: the frozen weights are already MXFP8"
+    if model.lora_only or model.trainable_scaling:
+        return False, "lora_only / trainable scaling with quantized frozen weights use --engine module"
+    why = _neox_refusal(model.wrapped_model, model.r) or device_refusal(model.wrapped_model)
+    return (False, why) if why else (True, "ok")
+
+
 def supports_full_rank(model, args=None) -> Tuple[bool, str]:
     """Whether the executor can train ``model`` (an unwrapped GPT-NeoX) full-rank, and if not, why."""
     why = full_rank_refusal(model, GPTNeoXForCausalLM, "only GPT-NeoX (Pythia) is fused for full-rank training here", args)
@@ -96,13 +126,22 @@ class _Layer(LayerViews):
 class FusedPythiaStepper(FusedStepperBase):
     """``model`` is a ``ReLoRaModel`` around a GPT-NeoX (ReLoRA: frozen weights, trainable LoRA factors) or a bare
     ``GPTNeoXForCausalLM`` (full-rank training: the projection weights are trainable and live in the flat store; every projection
-    is the ReLoRA one without its low-rank branch)."""
+    is the ReLoRA one without its low-rank branch).  ``quantize="mxfp8"``: the model's frozen weights are MXFP8-packed
+    (``--quantize 8bit``) and stay so; the projections then run on the block-scaled GEMM (csrc/gemm_mx.cu)."""
 
     def __init__(self, model, info: DistInfo, *, lr: float, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
-                 overlap_wgrad: bool = True, attention: str = "auto", deterministic: bool = False):
-        super().__init__(model, info, supports, supports_full_rank, grad_accumulation=grad_accumulation,
+                 overlap_wgrad: bool = True, attention: str = "auto", deterministic: bool = False, quantize: Optional[str] = None,
+                 fp8: bool = False):
+        if quantize is not None and canonical_format(quantize) != "mxfp8":
+            raise RuntimeError(f"quantize={quantize!r}: only mxfp8 frozen weights run on the fused executor")
+        if quantize is not None and fp8:
+            raise RuntimeError("--frozen_dtype fp8 cannot be combined with --quantize: the frozen weights are already MXFP8")
+        if fp8:
+            raise RuntimeError("fp8 frozen weights are not supported for Pythia")
+        super().__init__(model, info, supports_quantized if quantize is not None else supports, supports_full_rank,
+                         grad_accumulation=grad_accumulation,
                          clip_grad_norm=clip_grad_norm, cuda_graphs=cuda_graphs, ce_chunk=ce_chunk, overlap_wgrad=overlap_wgrad,
                          attention=attention, deterministic=deterministic)
         neox = self.inner.gpt_neox
@@ -114,6 +153,8 @@ class FusedPythiaStepper(FusedStepperBase):
         at0 = layers[0].attention
         self.rot = at0.rotary_ndims
         self.rotary = at0.rotary_emb
+        self.mx = quantize is not None
+        self.Wmx: List[List[mx.MxWeight]] = []  # per layer: the packed query_key_value, dense, dense_h_to_4h, dense_4h_to_h
 
         # ---------------------------------------------------------------- flat trainable store
         params: List[torch.nn.Parameter] = []
@@ -143,7 +184,9 @@ class FusedPythiaStepper(FusedStepperBase):
                     assert W.data_ptr() == m.weight.data_ptr() and W.shape == m.weight.shape
                     assert b.data_ptr() == m.bias.data_ptr()
                     continue
-                setattr(S, "W_" + tag, m.weight.data)  # frozen weight, [out, in] contiguous as the module keeps it
+                # frozen weight: [out, in] contiguous as the module keeps it, or its packed bytes (``m.weight`` would be a transient
+                # dequantised copy)
+                setattr(S, "W_" + tag, m.qweight if self.mx else m.weight.data)
                 A, gA = pv(m.lora_A.weight)
                 B, gB = pv(m.lora_B.weight)
                 b, gb = pv(m.bias)
@@ -156,7 +199,12 @@ class FusedPythiaStepper(FusedStepperBase):
             S.w2, S.gw2 = pv(layer.post_attention_layernorm.weight)
             S.c2, S.gc2 = pv(layer.post_attention_layernorm.bias)
             S.mods = (at.query_key_value, at.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h)
-            if not self.full:  # (B, A, W) blocks of the merge GEMM  W += s·B·A
+            if self.mx:  # one packed weight per module: its (B, A, first row) block of the merge's fp32 delta s·B·A
+                if not all(isinstance(m.qweight, mx.MxWeight) for m in S.mods):
+                    raise RuntimeError("quantized frozen weights must be in the tensor-core layout (packed on the GPU)")
+                self.Wmx.append([m.qweight for m in S.mods])
+                S.merge = [[(m.lora_B.weight.data, m.lora_A.weight.data, 0)] for m in S.mods]
+            elif not self.full:  # (B, A, W) blocks of the merge GEMM  W += s·B·A
                 S.merge = [(m.lora_B.weight.data, m.lora_A.weight.data, m.weight.data) for m in S.mods]
             self.layers.append(S)
         self.W_emb, self.gW_emb = pv(neox.embed_in.weight)
@@ -205,6 +253,12 @@ class FusedPythiaStepper(FusedStepperBase):
         else:
             self.tmp_h, self.tmp_f = e(M, h), e(M, f)
             self.du_bufs = {"4": e(M, r), "h": e(M, r), "o": e(M, r), "qkv": e(M, r)}
+        if self.mx:
+            # E4M3 rows + block scales of every GEMM input, [M, width] per width: the norms' and the attention outputs (h), the
+            # GELU output (f) and the output gradients (h, f, 3h), each quantised right before the GEMM that reads it.  Zeros: the
+            # scale bytes of the rows past M, which no call writes, are those mx_quantize_rows gives zero rows.
+            u8 = lambda *s: torch.zeros(*s, dtype=torch.uint8, device=dev)  # noqa: E731
+            self.xq = {w: (u8(M, w), u8(self.C.mx_sf_bytes(M, w))) for w in (h, f, 3 * h)}
         # rotary tables of the module (linear / dynamic-NTK scaling, T beyond max_position_embeddings), fp32 [T, rot]
         if self.rot > 0:
             cos, sin = self.rotary(self.x_in, seq_len=T)

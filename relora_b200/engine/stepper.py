@@ -174,10 +174,11 @@ def make_stepper(model, info: DistInfo, args, *, native=None, dropout_seed: Opti
         quantized = isinstance(model, ReLoRaModel) and model._config.quantize is not None
         if cls is None and engine == "fused" and quantized:
             # MXFP8-packed frozen weights run fused only on request; `auto` keeps quantised models on the module path
-            ok, why_q = fused_llama.supports_quantized(model, args)
+            exe = fused_pythia if isinstance(model.wrapped_model, GPTNeoXForCausalLM) else fused_llama
+            ok, why_q = exe.supports_quantized(model, args)
             if not ok:
                 raise RuntimeError(f"--engine fused requested but not applicable: {why_q}")
-            cls = fused_llama.FusedLlamaStepper
+            cls = fused_pythia.FusedPythiaStepper if exe is fused_pythia else fused_llama.FusedLlamaStepper
             kw["quantize"] = "mxfp8"
         elif cls is None and engine == "fused":
             # Pythia (GPT-NeoX) and full-rank Llama run fused only on request; `auto` keeps both on the module path

@@ -1171,10 +1171,11 @@ def mx_quantize_weight_2d_exact(w: Optional[torch.Tensor] = None, q_old: Optiona
 def gemm_mx_ref(a: torch.Tensor, sfa: torch.Tensor, b: torch.Tensor, sfb: torch.Tensor, M: int, N: int, K: int,
                 b_mn_major: bool = False, a2: Optional[torch.Tensor] = None, b2: Optional[torch.Tensor] = None,
                 residual: Optional[torch.Tensor] = None, n_per_group: int = 0,
-                a2_group_kofs: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
-    """fp64 ``(ref, bound)`` of ``gemm_mx(a, sfa, b, sfb, out, M, N, K, b_mn_major, a2, b2, residual, n_per_group, a2_group_kofs)``:
+                a2_group_kofs: int = 0, bias: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp64 ``(ref, bound)`` of ``gemm_mx(a, sfa, b, sfb, out, M, N, K, b_mn_major, a2, b2, residual, n_per_group, a2_group_kofs,
+    bias)``:
 
-        out[m, n] = Σ_{k < Kpad} A[m, k]·B[n, k]  +  Σ_{j < K2} a2[m, o(n) + j]·b2[n, j]  +  residual[m, n]
+        out[m, n] = Σ_{k < Kpad} A[m, k]·B[n, k]  +  Σ_{j < K2} a2[m, o(n) + j]·b2[n, j]  +  bias[n]  +  residual[m, n]
 
     with K2 the width of ``b2`` and o(n) = (n // n_per_group)·a2_group_kofs for a grouped LoRA segment (``n_per_group`` > 0),
     else 0 and K2 the width of ``a2``.
@@ -1199,6 +1200,9 @@ def gemm_mx_ref(a: torch.Tensor, sfa: torch.Tensor, b: torch.Tensor, sfb: torch.
     elif a2 is not None:
         x, y = a2[:M].to(_F64), b2[:N].to(_F64)
         ref, bound = ref + x @ y.t(), bound + x.abs() @ y.abs().t()
+    if bias is not None:
+        c = bias[:N].to(_F64).unsqueeze(0)
+        ref, bound = ref + c, bound + c.abs()
     if residual is not None:
         r = residual[:M, :N].to(_F64)
         ref, bound = ref + r, bound + r.abs()
