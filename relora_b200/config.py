@@ -63,6 +63,7 @@ def _default_dtype() -> str:
 ENGINE_FLAGS = (
     "--device", "--backend", "--comm", "--engine", "--lora_dropout", "--cuda_graphs", "--frozen_dtype",
     "--init_lora_a", "--synthetic_data", "--log_every", "--parity_quirks", "--attention", "--deterministic",
+    "--activation_checkpointing",
 )
 
 
@@ -152,6 +153,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--synthetic_data", type=str, default=None,
                    help="'<n_sequences>' — train on random token ids instead of a dataset on disk")
     p.add_argument("--log_every", type=int, default=1)
+    _add_bool(p, "--activation_checkpointing", False,
+              help="keep only each layer's input (and the wgmma attention's output) for the backward and recompute the rest of the "
+                   "layer there: about one more forward of the projections per step for activation memory that no longer grows "
+                   "with the number of layers")
     _add_bool(p, "--parity_quirks", True, help="keep upstream quirks (dataset-size check units, token/sequence step math)")
     return p
 

@@ -12,6 +12,8 @@ provides the rest:
 * the buffers both executors share, the per-layer slot selection, the SDPA fallback attention and the embedding backward;
 * ``merge_and_reinit()``, on bf16 weights and on MXFP8-packed ones;
 * one CUDA graph per micro-batch shape, capture / replay and launch counting;
+* activation checkpointing (``activation_checkpointing=True``): the per-layer buffers shrink to two slots and the backward re-runs
+  each lower layer's forward (the executor's ``_layer_fwd``) before that layer's backward (``_recompute``);
 * the LoRA group forward / backward on the wgmma GEMM and the fused input-gradient kernel, and the chunked LM head + CE.
 """
 from __future__ import annotations
@@ -61,6 +63,15 @@ def native_attention_refusal(hd: int, args) -> Optional[str]:
     return None
 
 
+def checkpointing_refusal(args) -> Optional[str]:
+    """Activation checkpointing with the fp8 frozen-weight path: its forward records every site's activation amax, so a recomputed
+    layer would record it twice and change the delayed scales of the next step."""
+    if getattr(args, "activation_checkpointing", False) and getattr(args, "frozen_dtype", None) in ("fp8", "fp8_full"):
+        return (f"--activation_checkpointing cannot be combined with --frozen_dtype {args.frozen_dtype}: the fp8 forward records "
+                "activation amax for its delayed scales, and a recomputed layer would record it again")
+    return None
+
+
 def device_refusal(model) -> Optional[str]:
     """Checked after the shapes, so their reasons are visible on a CPU model."""
     p = next(model.parameters())
@@ -81,9 +92,11 @@ class LayerViews:
 class FusedStepperBase(Stepper):
     # ------------------------------------------------------------------ construction helpers
     def __init__(self, model, info, supports, supports_full_rank, *, grad_accumulation: int, clip_grad_norm: float,
-                 cuda_graphs: bool, ce_chunk: int, overlap_wgrad: bool, attention: str, deterministic: bool):
+                 cuda_graphs: bool, ce_chunk: int, overlap_wgrad: bool, attention: str, deterministic: bool,
+                 activation_checkpointing: bool = False):
         """Settings and sizes every executor has; ``supports`` / ``supports_full_rank`` are the executor's checks of a ReLoRA model
-        and of a bare one (full-rank training)."""
+        and of a bare one (full-rank training).  ``activation_checkpointing``: keep each layer's input (and the wgmma attention's
+        output and log-sum-exp) and recompute the rest of a layer in the backward (see ``_recompute``)."""
         self.full = not isinstance(model, ReLoRaModel)
         ok, why = supports_full_rank(model) if self.full else supports(model)
         if not ok:
@@ -112,7 +125,8 @@ class FusedStepperBase(Stepper):
         if attention == "native" and not self.native_attn:
             raise RuntimeError(f"--attention native supports head_dim <= {fused.NATIVE_ATTENTION_MAX_HEAD_DIM} (multiple of 8), "
                                f"got {self.hd}")
-        self._attn_saved: List = []  # SDPA: (o, q, k, v) of every layer of the training forward
+        self._attn_saved: Dict[int, tuple] = {}  # SDPA: (o, q, k, v) per layer of the training forward, until its backward
+        self.recompute = bool(activation_checkpointing)
         self.side = torch.cuda.Stream(device=self.device) if overlap_wgrad else None
         self.fp8 = self.fp8_bwd = False  # E4M3 frozen weights (csrc/fp8.cu): an executor that has them turns them on
         self.mx = False  # MXFP8-packed frozen stacks (csrc/gemm_mx.cu): likewise
@@ -165,7 +179,13 @@ class FusedStepperBase(Stepper):
 
     # ------------------------------------------------------------------ hooks of the subclasses
     def _alloc_layers(self, B: int, T: int) -> None:
-        """The executor's own buffers for a [B, T] micro-batch (``_alloc`` has set ``B_`` / ``T_`` / ``M_`` and ``x_in``)."""
+        """The executor's own buffers for a [B, T] micro-batch (``_alloc`` has set ``B_`` / ``T_`` / ``M_`` and ``x_in``); those
+        the backward reads per layer have ``n_slots`` slots and are listed in ``self._slotted``."""
+        raise NotImplementedError
+
+    def _layer_fwd(self, l: int, S, sl: int, x, x_next, train: bool, recompute: bool = False) -> None:
+        """Forward of layer ``l`` from ``x`` into ``x_next``, its saved activations in slot ``sl``.  ``recompute``: the backward's
+        re-run of a training layer (see ``_recompute``), which reuses the wgmma attention's saved output and writes no layer output."""
         raise NotImplementedError
 
     def _before_micro(self) -> None:
@@ -191,30 +211,74 @@ class FusedStepperBase(Stepper):
         self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         self._shape = (B, T)
 
+    @property
+    def n_slots(self) -> int:
+        """Slots of the per-layer saved activations: one per layer, or two under activation checkpointing."""
+        return min(2, self.L) if self.recompute else self.L
+
+    def _slot(self, l: int) -> int:
+        """The slot of layer ``l``'s saved activations in training."""
+        return l % 2 if self.recompute else l
+
+    def _kept(self, l: int) -> bool:
+        """Whether layer ``l``'s activations are still in their slot when its backward starts: always, or under activation
+        checkpointing for the top two layers only (no later forward writes their slots)."""
+        return not self.recompute or l >= self.L - 2
+
     def _layer_slots(self, train: bool):
         """(l, views, slot, x, x_next) per layer of the forward: ``slot`` indexes the per-layer saved activations and ``x`` /
-        ``x_next`` are the layer's input and output.  Training keeps every layer's; evaluation reuses slot 0 and alternates two
-        residual buffers."""
+        ``x_next`` are the layer's input and output.  Training keeps every layer's (two alternating slots under activation
+        checkpointing); evaluation reuses slot 0 and alternates two residual buffers."""
         for l, S in enumerate(self.layers):
             if train:
-                yield l, S, l, self.x_in[l], self.x_in[l + 1]
+                yield l, S, self._slot(l), self.x_in[l], self.x_in[l + 1]
             else:
                 yield l, S, 0, self.x_in[l % 2], self.x_in[(l + 1) % 2]
 
-    def _sdpa(self, q, k, v, train: bool, **kw):
-        """Causal torch SDPA over [B, heads, T, head_dim] views (the attention where the wgmma kernels are not used); in training
-        the call's autograd graph is kept for ``_sdpa_bwd``."""
+    def _recompute(self, l: int) -> None:
+        """Before layer ``l``'s backward under activation checkpointing: re-run its forward from the saved input ``x_in[l]`` into
+        slot ``l % 2`` (the top two layers are still there).
+
+        The recompute draws the forward's dropout masks: they hash (seed, key), and the seed advances only after the micro-batch's
+        backward.  It writes slot ``l % 2`` and the forward transients, on the main stream, while the side stream still runs layer
+        ``l + 1``'s weight gradients; those read slot ``(l + 1) % 2`` and the backward's gradient buffers, never what the recompute
+        writes.  The slot's previous owner is layer ``l + 2``: its weight gradients read it, and they are done, because the side
+        stream runs in FIFO order and layer ``l + 1``'s backward made the main stream wait for the last group layer ``l + 2`` forked
+        (``_join("qkv")``, before its attention backward) -- the executor's call site names its join order."""
+        if not self._kept(l):
+            self._layer_fwd(l, self.layers[l], self._slot(l), self.x_in[l], self.x_in[l + 1], True, recompute=True)
+
+    def saved_bytes_per_layer(self) -> int:
+        """Bytes the training forward keeps for one layer besides its input and the wgmma attention's output: one slot of every
+        per-layer buffer and, under SDPA, the kept graph's output and log-sum-exp.  Activation checkpointing keeps ``n_slots``
+        slots instead of L (and at most three graphs), so it saves about (L - 2) times this."""
+        n = sum(t[0].numel() * t.element_size() for t in self._slotted)
+        if not self.native_attn:
+            n += self.M_ * self.h * 2 + self.B_ * self.nh * self.T_ * 4
+        return n
+
+    def _sdpa(self, q, k, v, train: bool, keep: Optional[int] = None, **kw):
+        """Causal torch SDPA over [B, heads, T, head_dim] views (the attention where the wgmma kernels are not used).  In training
+        the call runs under autograd, so a forward and its recompute pick the same kernel; ``keep`` (a layer index) keeps the graph
+        for ``_sdpa_bwd``.  A kept graph reads its views of ``qkv`` in the backward, so it is kept only while their slot is not
+        rewritten."""
         if not train:
             return F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **kw)
         q, k, v = (t.detach().requires_grad_() for t in (q, k, v))
         with torch.enable_grad():
             o = F_.scaled_dot_product_attention(q, k, v, dropout_p=0.0, is_causal=True, **kw)
-        self._attn_saved.append((o, q, k, v))
+        if keep is not None:
+            self._attn_saved[keep] = (o, q, k, v)
         return o.detach()
+
+    def _sdpa_keep(self, l: int, train: bool, recompute: bool) -> Optional[int]:
+        """``keep`` for layer ``l``'s SDPA call: the training forward keeps the graphs of the layers whose slots survive until their
+        backward; a recompute keeps its own."""
+        return l if train and (recompute or self._kept(l)) else None
 
     def _sdpa_bwd(self, l: int):
         """(dq, dk, dv) of layer ``l``'s SDPA call for the attention-output gradient in ``dattn``."""
-        o, q, k, v = self._attn_saved[l]
+        o, q, k, v = self._attn_saved.pop(l)
         return torch.autograd.grad(o, (q, k, v), self.dattn.view(self.B_, self.T_, self.nh, self.hd).transpose(1, 2))
 
     def _embedding_bwd_and_join(self, dx, tags) -> None:
@@ -243,8 +307,10 @@ class FusedStepperBase(Stepper):
 
     # ------------------------------------------------------------------ LoRA groups
     def _lora_group_fwd(self, xn, xd, A, B, W, u, out, *, G, K, Ng, residual=None, site=None, prequant=False, bias=None, Nq=None,
-                        mx_ready=False):
+                        mx_ready=False, u_only=False):
         """u = s·xd_g·A_gᵀ (grouped) ; out = [xn | u]·[W | B]ᵀ (+ bias) (+ residual).
+
+        ``u_only`` (a recompute of a layer whose output is saved): u alone, by the same GEMM call as the full forward's.
 
         ``mx_ready`` (packed stacks): the producer of xn already wrote its MX rows into ``self.xq[K]``.
 
@@ -258,9 +324,14 @@ class FusedStepperBase(Stepper):
         Full-rank training (``A is None``): out = xn·Wᵀ (+ bias) (+ residual), one launch over the whole stacked group."""
         g, r, M = fused.gemm, self.r, self.M_
         if A is None:
-            g(xn, W, out, M=M, N=W.shape[0], K1=K, residual=residual, bias=bias)
+            if not u_only:
+                g(xn, W, out, M=M, N=W.shape[0], K1=K, residual=residual, bias=bias)
             return
         drop = self.p > 0 and xd.shape[1] == G * K
+        if u_only:
+            assert not self.fp8
+            g(xd, A, u, M=M, N=G * r, K1=K, n_per_group=r, a1_group_kofs=K if drop else 0, alpha=self.scale)
+            return
         if self.mx:
             # packed stack W: xn's E4M3 rows and block scales (the bytes the module path's mx.linear quantises), then
             # out = [xq | u]·[W | B]ᵀ on the block-scaled GEMM, the LoRA segment of group g reading u's columns g·r ..

@@ -26,6 +26,7 @@ with the module-by-module PyTorch path on identical weights and masks.
 """
 from __future__ import annotations
 
+import argparse
 import math
 import os
 from typing import Dict, List, Optional, Tuple
@@ -38,14 +39,14 @@ from ..ops.quant import canonical_format
 from ..parallel.dist import DistInfo
 from ..parallel.flat import _ALIGN as _STORE_ALIGN
 from ..relora import ReLoRaLinear, ReLoRaModel
-from .fused_common import (FusedStepperBase, LayerViews, device_refusal, full_rank_refusal, native_attention_refusal,
-                           relora_refusal)
+from .fused_common import (FusedStepperBase, LayerViews, checkpointing_refusal, device_refusal, full_rank_refusal,
+                           native_attention_refusal, relora_refusal)
 
 BF = torch.bfloat16
 
 
 def supports(model, args=None) -> Tuple[bool, str]:
-    why = relora_refusal(model, LlamaForCausalLM, "only Llama is fused")
+    why = relora_refusal(model, LlamaForCausalLM, "only Llama is fused") or checkpointing_refusal(args)
     if why:
         return False, why
     return _relora_shapes(model, args)
@@ -150,9 +151,10 @@ class FusedLlamaStepper(FusedStepperBase):
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
                  overlap_wgrad: bool = True, attention: str = "auto", fp8: bool = False, fp8_backward: bool = False,
-                 deterministic: bool = False, quantize: Optional[str] = None):
+                 deterministic: bool = False, quantize: Optional[str] = None, activation_checkpointing: bool = False):
         """``quantize="mxfp8"``: the model's frozen weights are MXFP8-packed (``--quantize 8bit``) and stay so; the stacks below
-        are then packed too and the projections run on the block-scaled GEMM (csrc/gemm_mx.cu)."""
+        are then packed too and the projections run on the block-scaled GEMM (csrc/gemm_mx.cu).  ``activation_checkpointing``:
+        see ``FusedStepperBase``; the fp8 path is refused with it (``fused_common.checkpointing_refusal``)."""
         if quantize is not None and canonical_format(quantize) != "mxfp8":
             raise RuntimeError(f"quantize={quantize!r}: only mxfp8 frozen weights run on the fused executor")
         if quantize is not None and (fp8 or fp8_backward):
@@ -160,7 +162,7 @@ class FusedLlamaStepper(FusedStepperBase):
         super().__init__(model, info, supports_quantized if quantize is not None else supports, supports_full_rank,
                          grad_accumulation=grad_accumulation,
                          clip_grad_norm=clip_grad_norm, cuda_graphs=cuda_graphs, ce_chunk=ce_chunk, overlap_wgrad=overlap_wgrad,
-                         attention=attention, deterministic=deterministic)
+                         attention=attention, deterministic=deterministic, activation_checkpointing=activation_checkpointing)
         if self.full and fp8:
             raise RuntimeError("--frozen_dtype fp8 has no frozen weights to act on in full-rank training")
         if fp8 and num_kv_heads(model.wrapped_model.config) != model.wrapped_model.config.num_attention_heads:
@@ -291,6 +293,10 @@ class FusedLlamaStepper(FusedStepperBase):
         self._init_optimizer(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, zero=zero, native=native)
         # ---- fp8 frozen-weight path: E4M3 copies of the stacked weights + per-site activation scales (csrc/fp8.cu)
         self.fp8 = not self.full and (bool(fp8) or os.environ.get("RELORA_B200_FP8", "0") == "1")
+        why = checkpointing_refusal(argparse.Namespace(activation_checkpointing=self.recompute,
+                                                       frozen_dtype="fp8" if self.fp8 else None))
+        if why:
+            raise RuntimeError(why)
         if self.fp8:
             u8 = lambda *sh: torch.zeros(*sh, dtype=torch.uint8, device=dev)  # noqa: E731
             self.W8 = [u8(L, 3 * h, h), u8(L, h, h), u8(L, 2 * fp, h), u8(L, h, fp)]  # sites: qkv, o, gate/up, down
@@ -356,7 +362,8 @@ class FusedLlamaStepper(FusedStepperBase):
         self._w_scale2[1].copy_(self._w_scale2[0])
 
     def _alloc_layers(self, B: int, T: int):
-        dev, h, f, r, L, M = self.device, self.h, self.fp, self.r, self.L, self.M_  # f: padded intermediate size
+        dev, h, f, r, M = self.device, self.h, self.fp, self.r, self.M_  # f: padded intermediate size
+        L = self.n_slots  # saved for the backward: one slot per layer, or two under activation checkpointing
         e = lambda *s: torch.empty(*s, dtype=BF, device=dev)  # noqa: E731
         self.x1 = e(L, M, h)
         self.rstd1 = torch.empty(L, M, dtype=torch.float32, device=dev)
@@ -391,6 +398,9 @@ class FusedLlamaStepper(FusedStepperBase):
             self.u_d = e(L, M, r)
             self.dxn, self.dhmid = e(M, h), e(M, f)
             self.du_bufs = {"d": e(M, r), "gu": e(M, 2 * r), "o": e(M, r), "qkv": e(M, 3 * r)}
+        self._slotted = [self.x1, self.rstd1, self.rstd2, self.xd_qkv, self.xd_o, self.xd_gu, self.xd_d, self.qkv, self.gu]
+        if not self.full:
+            self._slotted += [self.u_qkv, self.u_o, self.u_gu, self.u_d]
         if self.mx:  # E4M3 rows + block scales of every GEMM input: [M, width] per width
             widths = {h, f, self.qkv_w, 2 * f}
             # zeros: the scale bytes of the rows past M that no producer writes are those mx_quantize_rows gives zero rows
@@ -404,16 +414,17 @@ class FusedLlamaStepper(FusedStepperBase):
         self.parts = None if self.full else e(M, max(3 * h, f))
 
     # ------------------------------------------------------------------ forward + backward of one micro-batch
-    def _attention(self, qkv: torch.Tensor, train: bool, sl: int = 0):
+    def _attention(self, qkv: torch.Tensor, train: bool, al: int = 0, keep: Optional[int] = None):
+        """Attention of one layer; ``al`` indexes the wgmma kernels' saved output and log-sum-exp, ``keep`` is ``_sdpa``'s."""
         B, T, nh, hd = self.B_, self.T_, self.nh, self.hd
         if self.native_attn:
             # wgmma flash attention straight out of the packed projection buffer (csrc/attention.cu); the output and the
             # log-sum-exp of the layer are what the backward kernels need
-            out = self.attn_o[sl]
+            out = self.attn_o[al]
             if self.nkv == nh:
-                self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd))
+                self.C.attention_fwd(qkv, out, self.lse[al], B, T, nh, hd, 1.0 / math.sqrt(hd))
             else:
-                self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd), nkv=self.nkv)
+                self.C.attention_fwd(qkv, out, self.lse[al], B, T, nh, hd, 1.0 / math.sqrt(hd), nkv=self.nkv)
             return out
         if self.nkv == nh:
             v5 = qkv.view(B, T, 3, nh, hd)
@@ -423,7 +434,7 @@ class FusedLlamaStepper(FusedStepperBase):
             v3 = qkv.view(B, T, nh + 2 * self.nkv, hd)
             q, k, v = (v3[:, :, a:b].transpose(1, 2) for a, b in ((0, nh), (nh, nh + self.nkv), (nh + self.nkv, nh + 2 * self.nkv)))
             gqa = {"enable_gqa": True}
-        return self._sdpa(q, k, v, train, **gqa).transpose(1, 2).reshape(self.M_, self.h)
+        return self._sdpa(q, k, v, train, keep, **gqa).transpose(1, 2).reshape(self.M_, self.h)
 
     def _q8(self, l, s_i, K):
         """(q8, inv_scale, amax_cur) arguments that make a producer kernel also emit the E4M3 copy of its output; on packed
@@ -440,61 +451,69 @@ class FusedLlamaStepper(FusedStepperBase):
         return dict(q8=self.xq[K][0], q_amax=self.xq[K][1]) if self.mx else {}  # no q_inv_scale: the MX form
 
     def _forward(self, train: bool):
-        C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
-        p = self.p if train else 0.0
-        seed = self.seed
         if train and self.fp8 and not self._fp8_calibrating:
             self._fp8_prep()
-        C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
+        self.C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
         self._attn_saved.clear()
         for l, S, sl, x, x_next in self._layer_slots(train):
-            x1 = self.x1[sl]
-            qkv, gu = self.qkv[sl], self.gu[sl]
-            # ---- attention block
-            if p > 0:
-                xd = self.xd_qkv[sl]
-                C.rmsnorm_fwd(x, S.w1, self.xn, self.rstd1[sl], self.eps, xd, seed, S.keys_qkv, p, *self._q8(l, 0, h))
-                xn = self.xn
-            else:
-                xn = self.xd_qkv[sl][:, :h] if self.p == 0 else self.xn  # p==0: the normed input is what dA needs
-                xn = xn if xn.is_contiguous() else self.xn
-                C.rmsnorm_fwd(x, S.w1, xn, self.rstd1[sl], self.eps, None, None, [], 0.0, **self._mx(h))
-                xd = xn
-            self._lora_group_fwd(xn, xd, S.A_qkv, S.B_qkv, S.Wqkv, self.u_qkv[sl], qkv, G=3, K=h, Ng=self.kv, site=(l, 0),
-                                 prequant=p > 0, Nq=h, mx_ready=True)
-            C.rope_inplace(qkv, self.T_, self.nh + self.nkv, self.hd, self.hd, self.cos, self.sin, False, 0)
-            attn = self._attention(qkv, train, sl)
-            if p > 0:
-                xd_o = self.xd_o[sl]
-                C.dropout_expand(attn, xd_o, seed, [S.key_o], p, *self._q8(l, 1, h))
-            else:
-                xd_o = attn
-                if train:
-                    self.xd_o[sl].copy_(attn)
-            self._lora_group_fwd(attn, xd_o, S.A_o, S.B_o, S.Wo, self.u_o[sl], x1, G=1, K=h, Ng=h, residual=x, site=(l, 1), prequant=p > 0)
-            # ---- MLP block
-            if p > 0:
-                xd = self.xd_gu[sl]
-                C.rmsnorm_fwd(x1, S.w2, self.xn, self.rstd2[sl], self.eps, xd, seed, S.keys_gu, p, *self._q8(l, 2, h))
-                xn = self.xn
-            else:
-                xn = self.xd_gu[sl] if self.p == 0 else self.xn
-                C.rmsnorm_fwd(x1, S.w2, xn, self.rstd2[sl], self.eps, None, None, [], 0.0, **self._mx(h))
-                xd = xn
-            self._lora_group_fwd(xn, xd, S.A_gu, S.B_gu, S.Wgu, self.u_gu[sl], gu, G=2, K=h, Ng=f, site=(l, 2), prequant=p > 0,
-                                 mx_ready=True)
-            if p > 0:
-                xd_d = self.xd_d[sl]
-                C.swiglu_fwd(gu, self.hmid, xd_d, seed, S.key_d, p, *self._q8(l, 3, f))  # activation, dropout copy (and E4M3 / MX copy)
-            else:
-                C.swiglu_fwd(gu, self.hmid, None, None, 0, 0.0, *self._q8(l, 3, f))
-                xd_d = self.hmid
-                if train:
-                    self.xd_d[sl].copy_(self.hmid)
-            self._lora_group_fwd(self.hmid, xd_d, S.A_d, S.B_d, S.Wd, self.u_d[sl], x_next, G=1, K=f, Ng=h, residual=x1, site=(l, 3), prequant=True,
-                                 mx_ready=True)
-        C.rmsnorm_fwd(x_next, self.w_norm, self.xf, self.rstd_f, self.eps, None, None, [], 0.0)
+            self._layer_fwd(l, S, sl, x, x_next, train)
+        self.C.rmsnorm_fwd(x_next, self.w_norm, self.xf, self.rstd_f, self.eps, None, None, [], 0.0)
         return x_next
+
+    def _layer_fwd(self, l, S, sl, x, x_next, train, recompute=False):
+        """One decoder layer (see the base class).  A recompute reads the wgmma attention's saved output (SDPA runs again and keeps
+        its graph) and forms only the down projection's LoRA product u_d, since x_next is saved."""
+        C, M, h, f = self.C, self.M_, self.h, self.fp
+        p = self.p if train else 0.0
+        seed = self.seed
+        x1 = self.x1[sl]
+        qkv, gu = self.qkv[sl], self.gu[sl]
+        # ---- attention block
+        if p > 0:
+            xd = self.xd_qkv[sl]
+            C.rmsnorm_fwd(x, S.w1, self.xn, self.rstd1[sl], self.eps, xd, seed, S.keys_qkv, p, *self._q8(l, 0, h))
+            xn = self.xn
+        else:
+            xn = self.xd_qkv[sl][:, :h] if self.p == 0 else self.xn  # p==0: the normed input is what dA needs
+            xn = xn if xn.is_contiguous() else self.xn
+            C.rmsnorm_fwd(x, S.w1, xn, self.rstd1[sl], self.eps, None, None, [], 0.0, **self._mx(h))
+            xd = xn
+        self._lora_group_fwd(xn, xd, S.A_qkv, S.B_qkv, S.Wqkv, self.u_qkv[sl], qkv, G=3, K=h, Ng=self.kv, site=(l, 0),
+                             prequant=p > 0, Nq=h, mx_ready=True)
+        C.rope_inplace(qkv, self.T_, self.nh + self.nkv, self.hd, self.hd, self.cos, self.sin, False, 0)
+        if recompute and self.native_attn:
+            attn = self.attn_o[l]
+        else:
+            attn = self._attention(qkv, train, l if train else 0, self._sdpa_keep(l, train, recompute))
+        if p > 0:
+            xd_o = self.xd_o[sl]
+            C.dropout_expand(attn, xd_o, seed, [S.key_o], p, *self._q8(l, 1, h))
+        else:
+            xd_o = attn
+            if train:
+                self.xd_o[sl].copy_(attn)
+        self._lora_group_fwd(attn, xd_o, S.A_o, S.B_o, S.Wo, self.u_o[sl], x1, G=1, K=h, Ng=h, residual=x, site=(l, 1), prequant=p > 0)
+        # ---- MLP block
+        if p > 0:
+            xd = self.xd_gu[sl]
+            C.rmsnorm_fwd(x1, S.w2, self.xn, self.rstd2[sl], self.eps, xd, seed, S.keys_gu, p, *self._q8(l, 2, h))
+            xn = self.xn
+        else:
+            xn = self.xd_gu[sl] if self.p == 0 else self.xn
+            C.rmsnorm_fwd(x1, S.w2, xn, self.rstd2[sl], self.eps, None, None, [], 0.0, **self._mx(h))
+            xd = xn
+        self._lora_group_fwd(xn, xd, S.A_gu, S.B_gu, S.Wgu, self.u_gu[sl], gu, G=2, K=h, Ng=f, site=(l, 2), prequant=p > 0,
+                             mx_ready=True)
+        if p > 0:
+            xd_d = self.xd_d[sl]
+            C.swiglu_fwd(gu, self.hmid, xd_d, seed, S.key_d, p, *self._q8(l, 3, f))  # activation, dropout copy (and E4M3 / MX copy)
+        else:
+            C.swiglu_fwd(gu, self.hmid, None, None, 0, 0.0, *self._q8(l, 3, f))
+            xd_d = self.hmid
+            if train:
+                self.xd_d[sl].copy_(self.hmid)
+        self._lora_group_fwd(self.hmid, xd_d, S.A_d, S.B_d, S.Wd, self.u_d[sl], x_next, G=1, K=f, Ng=h, residual=x1, site=(l, 3), prequant=True,
+                             mx_ready=True, u_only=recompute)
 
     def _backward(self):
         C, g, M, h, f, r = self.C, fused.gemm, self.M_, self.h, self.fp, self.r
@@ -503,27 +522,31 @@ class FusedLlamaStepper(FusedStepperBase):
         ws, tk = fused.norm_workspace(self.device, h)
         C.rmsnorm_bwd(self.dxf, self.x_in[self.L], self.w_norm, self.rstd_f, None, dx, self.gw_norm, ws, tk)
         for l in range(self.L - 1, -1, -1):
-            S = self.layers[l]
+            S, sl = self.layers[l], self._slot(l)
+            # activation checkpointing: layer l into slot l % 2 (see _recompute).  Pending on the side stream are layer l + 1's
+            # gate/up, o and qkv weight gradients (its down_proj ones were joined at the end of its backward), which read slot
+            # (l + 1) % 2; layer l + 2's, the slot's previous readers, were all joined by layer l + 1's _join("qkv").
+            self._recompute(l)
             # ---- MLP: x_next = hmid·Wdᵀ + u_d·B_dᵀ + x1
-            self._lora_group_bwd(dx, S.B_d, S.Wd, S.A_d, S.gA_d, S.gB_d, self.xd_d[l], self.u_d[l], [S.key_d],
+            self._lora_group_bwd(dx, S.B_d, S.Wd, S.A_d, S.gA_d, S.gB_d, self.xd_d[sl], self.u_d[sl], [S.key_d],
                                  G=1, K=f, Ng=h, base_out=self.dhmid, out=self.dhmid2, tag="d", site=(l, 3), gW=S.gWd)
             self._join("gu")  # the previous layer's gate/up weight gradients read dgu / du_gu
-            C.swiglu_bwd(self.dhmid2, self.gu[l], self.dgu)
-            self._lora_group_bwd(self.dgu, S.B_gu, S.Wgu, S.A_gu, S.gA_gu, S.gB_gu, self.xd_gu[l], self.u_gu[l], S.keys_gu,
+            C.swiglu_bwd(self.dhmid2, self.gu[sl], self.dgu)
+            self._lora_group_bwd(self.dgu, S.B_gu, S.Wgu, S.A_gu, S.gA_gu, S.gB_gu, self.xd_gu[sl], self.u_gu[sl], S.keys_gu,
                                  G=2, K=h, Ng=f, base_out=self.dxn, out=self.dxn2, tag="gu", site=(l, 2), gW=S.gWgu)
             self._join("o")  # ... and its o_proj weight gradients read the buffer this norm backward writes
-            C.rmsnorm_bwd(self.dxn2, self.x1[l], S.w2, self.rstd2[l], dx, dx_other, S.gw2, ws, tk)
+            C.rmsnorm_bwd(self.dxn2, self.x1[sl], S.w2, self.rstd2[sl], dx, dx_other, S.gw2, ws, tk)
             dx, dx_other = dx_other, dx  # dx = grad wrt x1
             # ---- attention: x1 = attn·Woᵀ + u_o·B_oᵀ + x
-            self._lora_group_bwd(dx, S.B_o, S.Wo, S.A_o, S.gA_o, S.gB_o, self.xd_o[l], self.u_o[l], [S.key_o],
+            self._lora_group_bwd(dx, S.B_o, S.Wo, S.A_o, S.gA_o, S.gB_o, self.xd_o[sl], self.u_o[sl], [S.key_o],
                                  G=1, K=h, Ng=h, base_out=self.dxn, out=self.dattn, tag="o", site=(l, 1), gW=S.gWo)
             if self.native_attn:
                 self._join("qkv")  # the previous layer's qkv weight gradients read dqkv / du_qkv
                 if self.nkv == nh:
-                    C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
+                    C.attention_bwd(self.qkv[sl], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
                                     1.0 / math.sqrt(hd))
                 else:
-                    C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
+                    C.attention_bwd(self.qkv[sl], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
                                     1.0 / math.sqrt(hd), nkv=self.nkv)
                 C.rope_inplace(self.dqkv, T, nh + self.nkv, hd, hd, self.cos, self.sin, True, 0)  # back through the rotation of q, k
                 dq = None
@@ -543,11 +566,11 @@ class FusedLlamaStepper(FusedStepperBase):
                 d3[:, :, nh:nh + nkv].copy_(dk.transpose(1, 2))
                 d3[:, :, nh + nkv:].copy_(dv.transpose(1, 2))
                 C.rope_inplace(self.dqkv, T, nh + nkv, hd, hd, self.cos, self.sin, True, 0)
-            self._lora_group_bwd(self.dqkv, S.B_qkv, S.Wqkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd_qkv[l], self.u_qkv[l],
+            self._lora_group_bwd(self.dqkv, S.B_qkv, S.Wqkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd_qkv[sl], self.u_qkv[sl],
                                  S.keys_qkv, G=3, K=h, Ng=self.kv, base_out=self.dxn, out=self.dxn2, tag="qkv", site=(l, 0), Nq=h,
                                  gW=S.gWqkv)
             self._join("d")  # this layer's down_proj weight gradients read the buffer written next
-            C.rmsnorm_bwd(self.dxn2, self.x_in[l], S.w1, self.rstd1[l], dx, dx_other, S.gw1, ws, tk)
+            C.rmsnorm_bwd(self.dxn2, self.x_in[l], S.w1, self.rstd1[sl], dx, dx_other, S.gw1, ws, tk)
             dx, dx_other = dx_other, dx
         self._embedding_bwd_and_join(dx, ("d", "gu", "o", "qkv"))
         if self.fp8_bwd:

@@ -133,7 +133,7 @@ class FusedPythiaStepper(FusedStepperBase):
                  weight_decay: float = 0.0, clip_grad_norm: float = 1.0, grad_accumulation: int = 1, zero: bool = False,
                  transport: str = "nccl", native=None, cuda_graphs: bool = True, ce_chunk: int = 4096,
                  overlap_wgrad: bool = True, attention: str = "auto", deterministic: bool = False, quantize: Optional[str] = None,
-                 fp8: bool = False):
+                 fp8: bool = False, activation_checkpointing: bool = False):
         if quantize is not None and canonical_format(quantize) != "mxfp8":
             raise RuntimeError(f"quantize={quantize!r}: only mxfp8 frozen weights run on the fused executor")
         if quantize is not None and fp8:
@@ -143,7 +143,7 @@ class FusedPythiaStepper(FusedStepperBase):
         super().__init__(model, info, supports_quantized if quantize is not None else supports, supports_full_rank,
                          grad_accumulation=grad_accumulation,
                          clip_grad_norm=clip_grad_norm, cuda_graphs=cuda_graphs, ce_chunk=ce_chunk, overlap_wgrad=overlap_wgrad,
-                         attention=attention, deterministic=deterministic)
+                         attention=attention, deterministic=deterministic, activation_checkpointing=activation_checkpointing)
         neox = self.inner.gpt_neox
         layers = neox.layers
         self.parallel = bool(layers[0].use_parallel_residual)
@@ -223,10 +223,11 @@ class FusedPythiaStepper(FusedStepperBase):
 
     # ------------------------------------------------------------------ buffers
     def _alloc_layers(self, B: int, T: int):
-        dev, h, f, r, L, M = self.device, self.h, self.f, self.r, self.L, self.M_
+        dev, h, f, r, M = self.device, self.h, self.f, self.r, self.M_
+        L = self.n_slots
         e = lambda *s: torch.empty(*s, dtype=BF, device=dev)  # noqa: E731
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)  # noqa: E731
-        # saved for the backward, one slot per layer ([0] only in evaluation)
+        # saved for the backward, one slot per layer or two under activation checkpointing ([0] only in evaluation)
         self.mean1, self.rstd1 = f32(L, M), f32(L, M)
         self.xd1, self.xd2 = e(L, M, h), e(L, M, h)  # LoRA inputs of query_key_value / dense_h_to_4h (the norms' outputs when p = 0)
         self.qkv = e(L, M, 3 * h)                    # post-rotary, head-interleaved
@@ -240,6 +241,9 @@ class FusedPythiaStepper(FusedStepperBase):
         if not self.parallel:
             self.x1 = e(L, M, h)
             self.mean2, self.rstd2 = f32(L, M), f32(L, M)
+        self._slotted = [self.mean1, self.rstd1, self.xd1, self.xd2, self.qkv, self.xd_o, self.z, self.xd_4]
+        self._slotted += [] if self.full else [self.u_qkv, self.u_o, self.u_h, self.u_4]
+        self._slotted += [] if self.parallel else [self.x1, self.mean2, self.rstd2]
         # transients
         self.xn1, self.xn2, self.attn_t, self.x1_t = e(M, h), e(M, h), e(M, h), e(M, h)
         self.a = e(M, f)
@@ -266,14 +270,15 @@ class FusedPythiaStepper(FusedStepperBase):
             self.sin = sin[0, 0, :T].float().contiguous()
 
     # ------------------------------------------------------------------ forward
-    def _attention(self, qkv: torch.Tensor, train: bool, sl: int, out: torch.Tensor):
+    def _attention(self, qkv: torch.Tensor, train: bool, al: int, out: torch.Tensor, keep: Optional[int] = None):
+        """Attention of one layer into ``out``; ``al`` indexes the wgmma kernels' saved log-sum-exp, ``keep`` is ``_sdpa``'s."""
         B, T, nh, hd = self.B_, self.T_, self.nh, self.hd
         if self.native_attn:
-            self.C.attention_fwd(qkv, out, self.lse[sl], B, T, nh, hd, 1.0 / math.sqrt(hd), interleaved=True)
+            self.C.attention_fwd(qkv, out, self.lse[al], B, T, nh, hd, 1.0 / math.sqrt(hd), interleaved=True)
             return out
         v5 = qkv.view(B, T, nh, 3, hd)
         q, k, v = (v5[:, :, :, i].transpose(1, 2) for i in range(3))
-        out.view(B, T, nh, hd).copy_(self._sdpa(q, k, v, train).transpose(1, 2))
+        out.view(B, T, nh, hd).copy_(self._sdpa(q, k, v, train, keep).transpose(1, 2))
         return out
 
     def _norms(self, x, S, l, sl, train, p, both: bool, second_of=None):
@@ -305,46 +310,56 @@ class FusedPythiaStepper(FusedStepperBase):
         return [(o[2], o[3] if o[3] is not None else o[2]) for o in outs]
 
     def _forward(self, train: bool):
-        C, M, h, f = self.C, self.M_, self.h, self.f
-        p = self.p if train else 0.0
-        seed = self.seed
-        C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
+        self.C.embedding_fwd(self.ids.view(-1), self.W_emb, self.x_in[0])
         self._attn_saved.clear()
         for l, S, sl, x, x_next in self._layer_slots(train):
-            qkv = self.qkv[sl]
-            normed = self._norms(x, S, l, sl, train, p, both=self.parallel)
-            xn1, xd1 = normed[0]
-            # ---- attention: qkv = [xn1 | u]·[W | B]ᵀ + b, rotary in place, attention on the interleaved layout
-            self._lora_group_fwd(xn1, xd1, S.A_qkv, S.B_qkv, S.W_qkv, self.u_qkv[sl], qkv, G=1, K=h, Ng=3 * h, bias=S.b_qkv)
-            if self.rot > 0:
-                C.neox_rope(qkv, self.T_, self.nh, self.hd, self.rot, self.cos, self.sin, 0, False)
-            attn = self._attention(qkv, train, sl, self.attn_o[sl] if self.native_attn else (self.xd_o[sl] if train and self.p == 0 else self.attn_t))
-            if p > 0:
-                xd_o = self.xd_o[sl]
-                C.dropout_expand(attn, xd_o, seed, [S.key_o], p)
-            else:
-                xd_o = attn
-                if train and attn.data_ptr() != self.xd_o[sl].data_ptr():
-                    self.xd_o[sl].copy_(attn)
-            x1 = self.x1[sl] if (train and not self.parallel) else self.x1_t
-            self._lora_group_fwd(attn, xd_o, S.A_o, S.B_o, S.W_o, self.u_o[sl], x1, G=1, K=h, Ng=h, residual=x, bias=S.b_o)
-            # ---- MLP: z = [xn2 | u]·[W | B]ᵀ + b, GELU (+ dropout copy), x_next = [a | u]·[W | B]ᵀ + b + x1
-            if self.parallel:
-                xn2, xd2 = normed[1]
-            else:
-                xn2, xd2 = self._norms(x1, S, l, sl, train, p, both=False, second_of=x1)[0]
-            z = self.z[sl]
-            self._lora_group_fwd(xn2, xd2, S.A_h, S.B_h, S.W_h, self.u_h[sl], z, G=1, K=h, Ng=f, bias=S.b_h)
-            a = self.xd_4[sl] if (train and self.p == 0) else self.a
-            if p > 0:
-                xd_4 = self.xd_4[sl]
-                C.gelu_fwd(z, a, self.tanh, xd=xd_4, seed=seed, key=S.key_4, p=p)
-            else:
-                C.gelu_fwd(z, a, self.tanh)
-                xd_4 = a
-            self._lora_group_fwd(a, xd_4, S.A_4, S.B_4, S.W_4, self.u_4[sl], x_next, G=1, K=f, Ng=h, residual=x1, bias=S.b_4)
-        C.layernorm_fwd(x_next, self.w_norm, self.c_norm, self.xf, self.mean_f, self.rstd_f, self.eps_f)
+            self._layer_fwd(l, S, sl, x, x_next, train)
+        self.C.layernorm_fwd(x_next, self.w_norm, self.c_norm, self.xf, self.mean_f, self.rstd_f, self.eps_f)
         return x_next
+
+    def _layer_fwd(self, l, S, sl, x, x_next, train, recompute=False):
+        """One GPT-NeoX layer (see the base class).  A recompute reads the wgmma attention's saved output (SDPA runs again and keeps
+        its graph) and forms only the LoRA product u of the projections that write no saved activation: dense_4h_to_h and, under
+        parallel residual, dense, whose sum x1 only feeds x_next."""
+        C, h, f = self.C, self.h, self.f
+        p = self.p if train else 0.0
+        seed = self.seed
+        qkv = self.qkv[sl]
+        normed = self._norms(x, S, l, sl, train, p, both=self.parallel)
+        xn1, xd1 = normed[0]
+        # ---- attention: qkv = [xn1 | u]·[W | B]ᵀ + b, rotary in place, attention on the interleaved layout
+        self._lora_group_fwd(xn1, xd1, S.A_qkv, S.B_qkv, S.W_qkv, self.u_qkv[sl], qkv, G=1, K=h, Ng=3 * h, bias=S.b_qkv)
+        if self.rot > 0:
+            C.neox_rope(qkv, self.T_, self.nh, self.hd, self.rot, self.cos, self.sin, 0, False)
+        al = l if train else 0
+        out = self.attn_o[al] if self.native_attn else (self.xd_o[sl] if train and self.p == 0 else self.attn_t)
+        attn = out if recompute and self.native_attn else self._attention(qkv, train, al, out, self._sdpa_keep(l, train, recompute))
+        if p > 0:
+            xd_o = self.xd_o[sl]
+            C.dropout_expand(attn, xd_o, seed, [S.key_o], p)
+        else:
+            xd_o = attn
+            if train and attn.data_ptr() != self.xd_o[sl].data_ptr():
+                self.xd_o[sl].copy_(attn)
+        x1 = self.x1[sl] if (train and not self.parallel) else self.x1_t
+        self._lora_group_fwd(attn, xd_o, S.A_o, S.B_o, S.W_o, self.u_o[sl], x1, G=1, K=h, Ng=h, residual=x, bias=S.b_o,
+                             u_only=recompute and self.parallel)
+        # ---- MLP: z = [xn2 | u]·[W | B]ᵀ + b, GELU (+ dropout copy), x_next = [a | u]·[W | B]ᵀ + b + x1
+        if self.parallel:
+            xn2, xd2 = normed[1]
+        else:
+            xn2, xd2 = self._norms(x1, S, l, sl, train, p, both=False, second_of=x1)[0]
+        z = self.z[sl]
+        self._lora_group_fwd(xn2, xd2, S.A_h, S.B_h, S.W_h, self.u_h[sl], z, G=1, K=h, Ng=f, bias=S.b_h)
+        a = self.xd_4[sl] if (train and self.p == 0) else self.a
+        if p > 0:
+            xd_4 = self.xd_4[sl]
+            C.gelu_fwd(z, a, self.tanh, xd=xd_4, seed=seed, key=S.key_4, p=p)
+        else:
+            C.gelu_fwd(z, a, self.tanh)
+            xd_4 = a
+        self._lora_group_fwd(a, xd_4, S.A_4, S.B_4, S.W_4, self.u_4[sl], x_next, G=1, K=f, Ng=h, residual=x1, bias=S.b_4,
+                             u_only=recompute)
 
     # ------------------------------------------------------------------ backward
     def _backward(self):
@@ -353,28 +368,32 @@ class FusedPythiaStepper(FusedStepperBase):
         dx, dx_other = self.dx_a, self.dx_b
         C.layernorm_bwd(self.dxf, self.x_in[self.L], self.w_norm, self.mean_f, self.rstd_f, dx, self.gw_norm, self.gc_norm)
         for l in range(self.L - 1, -1, -1):
-            S = self.layers[l]
+            S, sl = self.layers[l], self._slot(l)
+            # activation checkpointing: layer l into slot l % 2 (see _recompute).  Pending on the side stream are layer l + 1's
+            # query_key_value weight gradients alone (its _join("o") covered the three groups it forked before), which read slot
+            # (l + 1) % 2; layer l + 2's, the slot's previous readers, were all joined by layer l + 1's _join("qkv").
+            self._recompute(l)
             # ---- MLP: x_next = a·W_4ᵀ + u_4·B_4ᵀ + b_4 + x1   (output gradient dx)
-            self._lora_group_bwd(dx, S.B_4, S.W_4, S.A_4, S.gA_4, S.gB_4, self.xd_4[l], self.u_4[l], [S.key_4],
+            self._lora_group_bwd(dx, S.B_4, S.W_4, S.A_4, S.gA_4, S.gB_4, self.xd_4[sl], self.u_4[sl], [S.key_4],
                                  G=1, K=f, Ng=h, base_out=self.tmp_f, out=self.da, tag="4", gW=S.gW_4)
             self._join("h")  # the previous layer's dense_h_to_4h weight gradients read dz / du
-            C.gelu_bwd(self.da, self.z[l], self.dz, self.tanh, dbias=S.gb_h)
-            self._lora_group_bwd(self.dz, S.B_h, S.W_h, S.A_h, S.gA_h, S.gB_h, self.xd2[l], self.u_h[l], [S.key_h],
+            C.gelu_bwd(self.da, self.z[sl], self.dz, self.tanh, dbias=S.gb_h)
+            self._lora_group_bwd(self.dz, S.B_h, S.W_h, S.A_h, S.gA_h, S.gB_h, self.xd2[sl], self.u_h[sl], [S.key_h],
                                  G=1, K=h, Ng=f, base_out=self.tmp_h, out=self.dxn2, tag="h", gW=S.gW_h)
             if self.parallel:
                 d_attn_out = dx  # dense's output gradient is the block's
             else:
                 # x_next = x1 + mlp(LN2 x1) + b_4:  dx1 = dx + LN2ᵀ(dxn2); Σ dx is the bias gradient of dense_4h_to_h
-                C.layernorm_bwd(self.dxn2, self.x1[l], S.w2, self.mean2[l], self.rstd2[l], dx_other, S.gw2, S.gc2, dres=dx,
+                C.layernorm_bwd(self.dxn2, self.x1[sl], S.w2, self.mean2[sl], self.rstd2[sl], dx_other, S.gw2, S.gc2, dres=dx,
                                 dres_sum=S.gb_4)
                 dx, dx_other = dx_other, dx
                 d_attn_out = dx
             # ---- attention: x1 = attn·W_oᵀ + u_o·B_oᵀ + b_o + x
-            self._lora_group_bwd(d_attn_out, S.B_o, S.W_o, S.A_o, S.gA_o, S.gB_o, self.xd_o[l], self.u_o[l], [S.key_o],
+            self._lora_group_bwd(d_attn_out, S.B_o, S.W_o, S.A_o, S.gA_o, S.gB_o, self.xd_o[sl], self.u_o[sl], [S.key_o],
                                  G=1, K=h, Ng=h, base_out=self.tmp_h, out=self.dattn, tag="o", gW=S.gW_o)
             if self.native_attn:
                 self._join("qkv")  # the previous layer's query_key_value weight gradients read dqkv / du
-                C.attention_bwd(self.qkv[l], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
+                C.attention_bwd(self.qkv[sl], self.attn_o[l], self.dattn, self.lse[l], self.delta, self.dqkv, B, T, nh, hd,
                                 1.0 / math.sqrt(hd), interleaved=True)
             else:
                 dq, dk, dv = self._sdpa_bwd(l)
@@ -385,15 +404,15 @@ class FusedPythiaStepper(FusedStepperBase):
             if self.rot > 0:
                 C.neox_rope(self.dqkv, T, nh, hd, self.rot, self.cos, self.sin, 0, True)  # back through the rotation of q, k
             C.colsum(self.dqkv, S.gb_qkv)
-            self._lora_group_bwd(self.dqkv, S.B_qkv, S.W_qkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd1[l], self.u_qkv[l], [S.key_qkv],
+            self._lora_group_bwd(self.dqkv, S.B_qkv, S.W_qkv, S.A_qkv, S.gA_qkv, S.gB_qkv, self.xd1[sl], self.u_qkv[sl], [S.key_qkv],
                                  G=1, K=h, Ng=3 * h, base_out=self.tmp_h, out=self.dxn1, tag="qkv", gW=S.gW_qkv)
             self._join("o")  # this layer's dense / dense_4h_to_h weight gradients read the buffer written next
             if self.parallel:
                 # dx = dx_next + LN1ᵀ(dxn1) + LN2ᵀ(dxn2); Σ dx_next is the bias gradient of both dense and dense_4h_to_h
-                C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[l], self.rstd1[l], dx_other, S.gw1, S.gc1, dres=dx,
+                C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[sl], self.rstd1[sl], dx_other, S.gw1, S.gc1, dres=dx,
                                 dy2=self.dxn2, w2=S.w2, dw2=S.gw2, db2=S.gc2, dres_sum=S.gb_o, dres_sum2=S.gb_4)
             else:
-                C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[l], self.rstd1[l], dx_other, S.gw1, S.gc1, dres=dx,
+                C.layernorm_bwd(self.dxn1, self.x_in[l], S.w1, self.mean1[sl], self.rstd1[sl], dx_other, S.gw1, S.gc1, dres=dx,
                                 dres_sum=S.gb_o)
             dx, dx_other = dx_other, dx
         self._embedding_bwd_and_join(dx, ("4", "h", "o", "qkv"))

@@ -139,7 +139,11 @@ def reset_optimizer(optimizer, lora_params, args, reset_index: int) -> float:
 def make_stepper(model, info: DistInfo, args, *, native=None, dropout_seed: Optional[int] = None):
     """Pick the executor for ``model`` on ``info.device`` according to ``--engine``.  On CUDA the optimizer runs on the extension's
     AdamW (``native``, created here unless given) and the LoRA-dropout counter starts from ``dropout_seed`` (a resumed run's saved
-    counter) or, without one, from a value derived from ``--seed``, so runs with different seeds draw different masks."""
+    counter) or, without one, from a value derived from ``--seed``, so runs with different seeds draw different masks.
+    ``--activation_checkpointing`` turns on the models' per-layer ``torch.utils.checkpoint`` and the fused executors' recompute."""
+    checkpointing = bool(getattr(args, "activation_checkpointing", False))
+    if checkpointing:
+        getattr(model, "wrapped_model", model).gradient_checkpointing_enable()
     if info.device.type == "cuda":
         from ..ops import fused, reference
         from ..ops import native as extension
@@ -197,6 +201,8 @@ def make_stepper(model, info: DistInfo, args, *, native=None, dropout_seed: Opti
         if cls is not None:
             if cls is fused_llama.FusedLlamaStepper and "quantize" not in kw:
                 kw.update(fp8=frozen in ("fp8", "fp8_full"), fp8_backward=frozen == "fp8_full")
+            if checkpointing:
+                kw["activation_checkpointing"] = True
             return cls(model, info, cuda_graphs=getattr(args, "cuda_graphs", True), attention=getattr(args, "attention", "auto"),
                        deterministic=bool(getattr(args, "deterministic", False)), **kw)
     if info.device.type != "cuda":
